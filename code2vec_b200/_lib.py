@@ -69,6 +69,12 @@ SYMBOLS = {
                                              c_i32, c_vp]),
     "c2v_label_dlogits": (ctypes.c_int, [_P(Dims), _P(Params), c_vp, c_vp, c_vp, c_i32, c_f32, c_vp, c_vp, c_vp, c_sz, c_i32,
                                          c_vp]),
+    "c2v_angular_loss_argmax": (ctypes.c_int, [_P(Dims), _P(Params), c_vp, c_vp, c_i32, c_f32, c_f32, c_vp, c_vp, c_vp, c_vp,
+                                               c_vp, c_vp, c_vp, c_sz, c_i32, c_vp]),
+    "c2v_angular_dlogits": (ctypes.c_int, [_P(Dims), _P(Params), c_vp, c_vp, c_vp, c_vp, c_i32, c_f32, c_f32, c_f32, c_vp, c_vp,
+                                           c_vp, c_sz, c_i32, c_vp]),
+    "c2v_angular_backward_ws": (ctypes.c_int, [_P(Dims), _P(Params), c_vp, c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_sz, c_i32,
+                                               c_vp]),
     "c2v_angular_logits": (ctypes.c_int, [_P(Dims), _P(Params), c_vp, c_vp, c_i32, c_f32, c_f32, c_vp, c_vp]),
     "c2v_angular_forward_train": (ctypes.c_int, [_P(Dims), _P(Params), c_vp, c_vp, c_i32, c_f32, c_f32, c_vp, c_vp, c_vp, c_vp]),
     "c2v_angular_backward": (ctypes.c_int, [_P(Dims), _P(Params), c_vp, c_vp, c_i32, c_f32, c_f32, c_vp, c_vp, c_vp, c_vp,

@@ -37,6 +37,8 @@ int launch_angular_backward(const c2v_dims *d, const c2v_params *p, const float 
                             float *d_out_inplace, float *d_cv, float *d_w, float *sums, cudaStream_t st);
 int launch_loss_argmax(const float *out, const long long *label, int B, long long C, float *loss,
                        long long *argmax, float *maxval, float *d_out, cudaStream_t st);
+int launch_row_inv_norm(const float *X, long long rows, int H, float *inv, cudaStream_t st);
+int launch_angular_project(float *d, const float *x, const float *inv, long long rows, int H, cudaStream_t st);
 int launch_colsum(const float *X, int B, long long C, float *out, cudaStream_t st);
 int launch_encode_backward(const c2v_dims *d, const c2v_params *p, const EncodeArgs &a, int B,
                            const float *cv, const float *attention, const float *d_cv,
@@ -420,6 +422,79 @@ int c2v_label_dlogits(const c2v_dims *d, const c2v_params *p, const float *code_
     la.label = reinterpret_cast<const long long *>(label); la.dlogits_lse = lse; la.dscale = scale; la.dscale_ptr = scale_device;
     return launch_label_tcgen05_ex(d, code_vector, B, p->output_weight, p->output_bias, d_outputs, nullptr, nullptr,
                                    workspace, workspace_bytes, reuse_prep, static_cast<cudaStream_t>(stream), &la);
+}
+
+int c2v_angular_loss_argmax(const c2v_dims *d, const c2v_params *p, const float *code_vector, const int64_t *label,
+                            int32_t B, float margin, float inverse_temp, float *outputs, float *loss, float *lse,
+                            int64_t *argmax, float *maxval, float *inv_norms, void *workspace, size_t workspace_bytes,
+                            int32_t algo, void *stream)
+{
+    if (!dims_ok(d)) return C2V_EINVAL;
+    if (!p || !p->output_weight || !code_vector || !label || !inv_norms || B < 1 || d->label_count < 1 || (!loss && !lse)) {
+        set_error("c2v_angular_loss_argmax: bad argument (NULL pointer, B < 1 or neither loss nor lse)");
+        return C2V_EINVAL;
+    }
+    if (!c2v_label_loss_supported(d, B)) {
+        set_error("c2v_angular_loss_argmax: the fused loss needs encode_size %% 4 == 0, <= 256 and B <= 2048 (got %d, %d); use "
+                  "c2v_angular_forward_train + c2v_loss_argmax", d->encode, B);
+        return C2V_EUNSUPPORTED;
+    }
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const bool reuse_prep = (algo & C2V_FLAG_REUSE_PREP) != 0;
+    g_pdl_this_call = (algo & C2V_FLAG_NO_PDL) == 0;
+    int rc = launch_row_inv_norm(code_vector, B, d->encode, inv_norms, st);
+    if (rc == C2V_OK) rc = launch_row_inv_norm(p->output_weight, d->label_count, d->encode, inv_norms + B, st);
+    if (rc != C2V_OK) return rc;
+    LabelLossArgs la;
+    memset(&la, 0, sizeof(la));
+    la.label = reinterpret_cast<const long long *>(label); la.loss = loss; la.lse_out = lse;
+    la.inv_norms = inv_norms; la.cos_m = cosf(margin); la.sin_m = sinf(margin); la.inverse_temp = inverse_temp;
+    return launch_label_tcgen05_ex(d, code_vector, B, p->output_weight, nullptr, outputs, reinterpret_cast<long long *>(argmax),
+                                   maxval, workspace, workspace_bytes, reuse_prep, st, &la);
+}
+
+int c2v_angular_dlogits(const c2v_dims *d, const c2v_params *p, const float *code_vector, const int64_t *label,
+                        const float *lse, const float *inv_norms, int32_t B, float margin, float inverse_temp, float scale,
+                        const float *scale_device, float *d_dot, void *workspace, size_t workspace_bytes, int32_t algo,
+                        void *stream)
+{
+    if (!dims_ok(d)) return C2V_EINVAL;
+    if (!p || !p->output_weight || !code_vector || !label || !lse || !inv_norms || !d_dot || B < 1 || d->label_count < 1) {
+        set_error("c2v_angular_dlogits: bad argument (NULL pointer or B < 1)");
+        return C2V_EINVAL;
+    }
+    if (!label_tcgen05_shape_ok(d)) {
+        set_error("c2v_angular_dlogits: needs encode_size %% 4 == 0 and <= 256 (got %d)", d->encode);
+        return C2V_EUNSUPPORTED;
+    }
+    const bool reuse_prep = (algo & C2V_FLAG_REUSE_PREP) != 0;
+    g_pdl_this_call = false;
+    LabelLossArgs la;
+    memset(&la, 0, sizeof(la));
+    la.label = reinterpret_cast<const long long *>(label); la.dlogits_lse = lse; la.dscale = scale; la.dscale_ptr = scale_device;
+    la.inv_norms = inv_norms; la.cos_m = cosf(margin); la.sin_m = sinf(margin); la.inverse_temp = inverse_temp;
+    return launch_label_tcgen05_ex(d, code_vector, B, p->output_weight, nullptr, d_dot, nullptr, nullptr, workspace,
+                                   workspace_bytes, reuse_prep, static_cast<cudaStream_t>(stream), &la);
+}
+
+int c2v_angular_backward_ws(const c2v_dims *d, const c2v_params *p, const float *code_vector, const float *d_dot,
+                            const float *inv_norms, int32_t B, float *d_code_vector, float *d_output_weight, void *workspace,
+                            size_t workspace_bytes, int32_t algo, void *stream)
+{
+    if (!dims_ok(d)) return C2V_EINVAL;
+    if (!p || !p->output_weight || !code_vector || !d_dot || !inv_norms || B < 1 || d->label_count < 1) {
+        set_error("c2v_angular_backward_ws: bad argument (NULL pointer or B < 1)");
+        return C2V_EINVAL;
+    }
+    // d_cv_raw = G . W, dW_raw = G^T . cv (the plain label backward, no bias), then the radial projection of F.normalize
+    int rc = c2v_label_backward_ws(d, p, code_vector, d_dot, B, d_code_vector, d_output_weight, nullptr, workspace,
+                                   workspace_bytes, algo, stream);
+    if (rc != C2V_OK) return rc;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (d_code_vector) rc = launch_angular_project(d_code_vector, code_vector, inv_norms, B, d->encode, st);
+    if (rc == C2V_OK && d_output_weight)
+        rc = launch_angular_project(d_output_weight, p->output_weight, inv_norms + B, d->label_count, d->encode, st);
+    return rc;
 }
 
 int c2v_angular_logits(const c2v_dims *d, const c2v_params *p, const float *code_vector,

@@ -124,6 +124,10 @@ struct LabelLossArgs {
     const float *dlogits_lse;    // in: [B] -> `out` receives d loss / d logits instead of the logits (or NULL)
     float dscale;                // dlogits scale: 1 / B (mean) ...
     const float *dscale_ptr;     // ... times *dscale_ptr when not NULL (the upstream gradient of the scalar loss, on the device)
+    // angular-margin head (model.py:71-80) when not NULL: [B + C] = 1 / max(|cv_b|, 1e-12) then 1 / max(|W_c|, 1e-12).
+    // The logits are s cos (s phi(cos) at the label), the bias is ignored, and dlogits mode writes d loss / d (cv . W^T).
+    const float *inv_norms;
+    float cos_m, sin_m, inverse_temp;
 };
 int launch_label_tcgen05_ex(const c2v_dims *d, const float *cv, int B, const float *Wout, const float *bias,
                             float *out, long long *argmax, float *maxval, void *ws, size_t ws_bytes, bool reuse_prep,

@@ -112,6 +112,41 @@ __global__ void row_inv_norm_kernel(const float *__restrict__ X, long long rows,
     if (lane == 0) inv[r] = 1.0f / fmaxf(sqrtf(s), 1e-12f);   // F.normalize eps
 }
 
+// inv[r] = 1 / max(|X[r]|, 1e-12) for the rows of X [rows, H]
+int launch_row_inv_norm(const float *X, long long rows, int H, float *inv, cudaStream_t st)
+{
+    if (rows <= 0) return C2V_OK;
+    row_inv_norm_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(X, rows, H, inv);
+    C2V_LAUNCH_OK("row_inv_norm_kernel");
+    return C2V_OK;
+}
+
+// d[r] -= inv[r]^2 (x[r] . d[r]) x[r]: the gradient through F.normalize, given d = the gradient w.r.t. the unnormalised
+// dot's operand (one warp per row of [rows, H]).  Exact for the angular head: sum_c dcos cos = sum_c G dot = x_r . (G W)_r.
+__global__ void __launch_bounds__(256)
+angular_project_rows_kernel(float *__restrict__ d, const float *__restrict__ x, const float *__restrict__ inv, long long rows,
+                            int H)
+{
+    const long long r = (long long)blockIdx.x * (blockDim.x / 32) + (threadIdx.x >> 5);
+    if (r >= rows) return;
+    const int lane = threadIdx.x & 31;
+    const float *xr = x + r * H;
+    float *dr = d + r * H;
+    float s = 0.0f;
+    for (int c = lane; c < H; c += 32) s = fmaf(xr[c], dr[c], s);
+    s = warp_sum(s);
+    const float f = -inv[r] * inv[r] * s;
+    for (int c = lane; c < H; c += 32) dr[c] = fmaf(f, xr[c], dr[c]);
+}
+
+int launch_angular_project(float *d, const float *x, const float *inv, long long rows, int H, cudaStream_t st)
+{
+    if (rows <= 0) return C2V_OK;
+    angular_project_rows_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(d, x, inv, rows, H);
+    C2V_LAUNCH_OK("angular_project_rows_kernel");
+    return C2V_OK;
+}
+
 __global__ void angular_epilogue_kernel(float *__restrict__ out, const float *__restrict__ inv_cv,
                                         const float *__restrict__ inv_w,
                                         const long long *__restrict__ label, int B, long long C,
@@ -136,11 +171,11 @@ int launch_angular(const c2v_dims *d, const c2v_params *p, const float *cv, cons
     const int H = d->encode;
     const long long C = d->label_count;
     float *inv_cv = scratch, *inv_w = scratch + B;
-    row_inv_norm_kernel<<<(B + 7) / 8, 256, 0, st>>>(cv, B, H, inv_cv);
-    C2V_LAUNCH_OK("row_inv_norm_kernel");
-    row_inv_norm_kernel<<<(unsigned)((C + 7) / 8), 256, 0, st>>>(p->output_weight, C, H, inv_w);
-    C2V_LAUNCH_OK("row_inv_norm_kernel");
-    int rc = launch_sgemm(B, (int)C, H, cv, H, 1, p->output_weight, 1, H, nullptr, out, C, false, st);
+    int rc = launch_row_inv_norm(cv, B, H, inv_cv, st);
+    if (rc != C2V_OK) return rc;
+    rc = launch_row_inv_norm(p->output_weight, C, H, inv_w, st);
+    if (rc != C2V_OK) return rc;
+    rc = launch_sgemm(B, (int)C, H, cv, H, 1, p->output_weight, 1, H, nullptr, out, C, false, st);
     if (rc != C2V_OK) return rc;
     const long long n = (long long)B * C;
     angular_epilogue_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(

@@ -152,9 +152,14 @@ __device__ __forceinline__ LtTile lt_tile(long long t, int n_mt, long long n_nt,
 //                  and the target logit v[row, label[row]] -> tgt[row]; merged by loss_partials_reduce / loss_finalize.
 //   lse  != NULL : dlogits mode (backward): the value stored is (exp(v - lse[row]) - [col == label[row]]) * dscale
 //                  instead of the logit (main.py:174 through log_softmax + NLLLoss, weights == 1).
+// Angular head (model.py:71-80, the label_gemm_v2_kernel<true> instantiation): the GEMM gives dot = cv . W^T (no bias) and
+// the epilogue's value becomes  s cos,  s phi(cos) at col == label[row],  cos = dot icv[row] iw[col]  (c2v_head.cu's
+// semantics).  The loss / arg-max modes then run on those logits; dlogits mode stores G = d loss / d dot instead.
 struct LtLoss {
     float2 *part; float *tgt; const long long *label; const float *lse; const float *dscale_ptr; float dscale; int Mpad;
     unsigned *gmax_bits;      // dlogits mode: bits of max |value stored| over the launch (what the label backward's fp16 split scales by)
+    const float *icv, *iw;    // angular: 1 / max(|cv_b|, 1e-12) [M], 1 / max(|W_c|, 1e-12) [N]
+    float cos_m, sin_m, s;    // angular: cos(margin), sin(margin), inverse_temp
 };
 constexpr float LT_LOG2E = 1.4426950408889634f;
 __device__ __forceinline__ float lt_ex2(float x) {
@@ -190,6 +195,8 @@ constexpr int SMEM_BYTES = SMEM_BAR_OFF + 128 + 1024;
 // registers), turns the fragments into one row per thread through shared memory, then each warp (32 rows x 32 columns)
 // does *1/scale + bias -> running arg-max (smem table, 64-bit atomicMax) -> padded smem tile -> row-contiguous stores.
 // Bound: the logits write (B*C*4 bytes); the arg-max costs no extra pass over them.
+// ANG: the angular-margin epilogue (see LtLoss); a template parameter so that the plain head compiles without it.
+template <bool ANG>
 __global__ void __launch_bounds__(lt2::THREADS, 1)
 label_gemm_v2_kernel(const uint8_t *__restrict__ imgA, const uint8_t *__restrict__ imgB,
                      const float *__restrict__ bias, const float *__restrict__ hdr, float *__restrict__ out,
@@ -263,12 +270,13 @@ label_gemm_v2_kernel(const uint8_t *__restrict__ imgA, const uint8_t *__restrict
         const int w4 = warp & 3, m4 = lane & 3;
         int it = 0;
         // bias of the NEXT tile's 32 columns is fetched one tile ahead (a dependent global load at the top of every tile
-        // otherwise sits on each warp's critical path)
+        // otherwise sits on each warp's critical path); the angular head fetches iw[col] the same way
         auto bias_of = [&](int i) {
-            if (!bias || i >= my_tiles) return 0.0f;
+            const float *colv = ANG ? ls.iw : bias;
+            if (!colv || i >= my_tiles) return 0.0f;
             const LtTile t2 = tile_of(i);
             const long long c2 = t2.nt * lt::TN + cq * 32 + lane;
-            return c2 < N ? __ldg(bias + c2) : 0.0f;
+            return c2 < N ? __ldg(colv + c2) : 0.0f;
         };
         float bias_next = bias_of(0);
         for (int i = 0; i < my_tiles; ++i) {
@@ -282,6 +290,8 @@ label_gemm_v2_kernel(const uint8_t *__restrict__ imgA, const uint8_t *__restrict
             sbias[lane] = bias_next;
             __syncwarp();
             bias_next = bias_of(i + 1);
+            float icv_r = 0.0f;                                        // angular: 1 / |cv| of this thread's row (thread = row)
+            if constexpr (ANG) icv_r = row0 + lane < M ? __ldg(ls.icv + row0 + lane) : 0.0f;
             float d[2][16];
             for (int kb = 0; kb < nkb; ++kb, ++it) {
                 const int st = it & 1;
@@ -325,11 +335,36 @@ label_gemm_v2_kernel(const uint8_t *__restrict__ imgA, const uint8_t *__restrict
                 for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4 *>(r + j) = *reinterpret_cast<const float4 *>(src + j);
             }
             float v[32];
+            float cos_t = 0.0f;                  // angular: cosine at this row's target column, when it lies in this block
+            if constexpr (!ANG) {
 #pragma unroll
-            for (int j = 0; j < 32; j += 4) {                                                       // model.py:83
-                const float4 b4 = *reinterpret_cast<const float4 *>(sbias + j);
-                v[j] = fmaf(r[j], inv_scale, b4.x); v[j + 1] = fmaf(r[j + 1], inv_scale, b4.y);
-                v[j + 2] = fmaf(r[j + 2], inv_scale, b4.z); v[j + 3] = fmaf(r[j + 3], inv_scale, b4.w);
+                for (int j = 0; j < 32; j += 4) {                                                   // model.py:83
+                    const float4 b4 = *reinterpret_cast<const float4 *>(sbias + j);
+                    v[j] = fmaf(r[j], inv_scale, b4.x); v[j + 1] = fmaf(r[j + 1], inv_scale, b4.y);
+                    v[j + 2] = fmaf(r[j + 2], inv_scale, b4.z); v[j + 3] = fmaf(r[j + 3], inv_scale, b4.w);
+                }
+            } else {                                                                                // model.py:71-80
+#pragma unroll
+                for (int j = 0; j < 32; j += 4) {                   // cos = dot icv iw (sbias holds iw of these columns)
+                    const float4 w4 = *reinterpret_cast<const float4 *>(sbias + j);
+                    v[j] = r[j] * inv_scale * icv_r * w4.x; v[j + 1] = r[j + 1] * inv_scale * icv_r * w4.y;
+                    v[j + 2] = r[j + 2] * inv_scale * icv_r * w4.z; v[j + 3] = r[j + 3] * inv_scale * icv_r * w4.w;
+                }
+                const long long grow = row0 + lane;
+                const long long tj = (grow < M ? ls.label[grow] : -1) - col0;
+                const int tji = (tj >= 0 && tj < n_cols) ? (int)tj : -1;
+                float phi = 0.0f;
+                if (__any_sync(0xffffffffu, tji >= 0)) {
+                    // the PTX select chain of the loss partials below: a dynamic v[tj] would put v[] in local memory
+#pragma unroll
+                    for (int j = 0; j < 32; ++j)
+                        asm volatile("{\n\t.reg .pred p;\n\tsetp.eq.s32 p, %2, %3;\n\tselp.f32 %0, %1, %0, p;\n\t}"
+                                     : "+f"(cos_t) : "f"(v[j]), "r"(tji), "r"(j));
+                    // phi(c) = c > 0 ? c cos_m - sqrt(1 - c^2) sin_m : c, for the target element only
+                    phi = cos_t > 0.0f ? cos_t * ls.cos_m - sqrtf(1.0f - cos_t * cos_t) * ls.sin_m : cos_t;
+                }
+#pragma unroll
+                for (int j = 0; j < 32; ++j) v[j] = (j == tji ? phi : v[j]) * ls.s;
             }
             if (ls.part || ls.lse) {
                 const long long grow = row0 + lane;                                     // this thread's output row
@@ -359,8 +394,25 @@ label_gemm_v2_kernel(const uint8_t *__restrict__ imgA, const uint8_t *__restrict
                 if (ls.lse) {                                                           // dlogits (overwrites v)
                     const float lb = (grow < M ? ls.lse[grow] : 0.0f) * LT_LOG2E;
                     const float sc = ls.dscale_ptr ? ls.dscale * *ls.dscale_ptr : ls.dscale;
+                    if constexpr (!ANG) {
 #pragma unroll
-                    for (int j = 0; j < 32; ++j) v[j] = (lt_ex2(fmaf(v[j], LT_LOG2E, -lb)) - ((j == (int)tj) ? 1.0f : 0.0f)) * sc;
+                        for (int j = 0; j < 32; ++j) v[j] = (lt_ex2(fmaf(v[j], LT_LOG2E, -lb)) - ((j == (int)tj) ? 1.0f : 0.0f)) * sc;
+                    } else {
+                        // G = d loss / d dot: dcos = s d_logit (x phi'(cos) at the target when cos > 0), G = dcos icv iw
+                        const float tf = cos_t > 0.0f ? ls.cos_m + ls.sin_m * cos_t / sqrtf(1.0f - cos_t * cos_t) : 1.0f;
+#pragma unroll
+                        for (int j = 0; j < 32; j += 4) {
+                            const float4 w4 = *reinterpret_cast<const float4 *>(sbias + j);
+                            const float iwj[4] = {w4.x, w4.y, w4.z, w4.w};
+#pragma unroll
+                            for (int u = 0; u < 4; ++u) {
+                                const bool t = j + u == (int)tj;
+                                float dcos = (lt_ex2(fmaf(v[j + u], LT_LOG2E, -lb)) - (t ? 1.0f : 0.0f)) * sc * ls.s;
+                                if (t) dcos *= tf;
+                                v[j + u] = dcos * icv_r * iwj[u];
+                            }
+                        }
+                    }
                     if (ls.gmax_bits && grow < M) {
 #pragma unroll
                         for (int j = 0; j < 32; ++j) gmax = fmaxf(gmax, j < n_cols ? fabsf(v[j]) : 0.0f);
@@ -655,6 +707,15 @@ int launch_label_tcgen05_ex(const c2v_dims *d, const float *cv, int B, const flo
         ls.gmax_bits = reinterpret_cast<unsigned *>(p + 768);
         C2V_CUDA_OK(cudaMemsetAsync(ls.gmax_bits, 0, 4, st));
     }
+    const bool angular = la && la->inv_norms;
+    if (angular) {
+        if (!la->label) { set_error("angular label head: label is NULL"); return C2V_EINVAL; }
+        ls.label = la->label;
+        ls.icv = la->inv_norms; ls.iw = la->inv_norms + B;
+        ls.cos_m = la->cos_m; ls.sin_m = la->sin_m; ls.s = la->inverse_temp;
+        bias = nullptr;                                                 // the angular head has none
+    }
+    auto *kern = angular ? label_gemm_v2_kernel<true> : label_gemm_v2_kernel<false>;
     const bool want_arg = argmax || maxval;
     const bool fused_arg = want_arg && mt <= (size_t)lt2::MAX_MT;
     int dev = 0, sms = 0;
@@ -674,7 +735,7 @@ int launch_label_tcgen05_ex(const c2v_dims *d, const float *cv, int B, const flo
                            reinterpret_cast<unsigned long long *>(key_region), fused_arg ? 8 + B : 0));
     C2V_COUNT_LAUNCH();
 
-    C2V_CUDA_OK(cudaFuncSetAttribute(label_gemm_v2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, lt2::SMEM_BYTES));
+    C2V_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, lt2::SMEM_BYTES));
     const long long n_tiles = (long long)mt * (long long)nt;
     const int grid = (int)(n_tiles < sms ? n_tiles : sms);
     // tile order (see lt_range): lanes when that keeps >= 95 % of the CTAs busy, else groups; C2V_LABEL_ORDER=groups|lanes forces one
@@ -684,7 +745,7 @@ int launch_label_tcgen05_ex(const c2v_dims *d, const float *cv, int B, const flo
         if (!strcmp(ord, "groups")) per_m = 0;
         else if (!strcmp(ord, "lanes") && mt <= (size_t)grid) per_m = grid / (int)mt;
     }
-    C2V_CUDA_OK(launch_pdl(label_gemm_v2_kernel, dim3((unsigned)grid), dim3(lt2::THREADS), (size_t)lt2::SMEM_BYTES, st,
+    C2V_CUDA_OK(launch_pdl(kern, dim3((unsigned)grid), dim3(lt2::THREADS), (size_t)lt2::SMEM_BYTES, st,
                            (const uint8_t *)imgA, (const uint8_t *)imgB, bias, (const float *)hdr, out, B, C, nkb, (int)mt,
                            (long long)nt, n_tiles, fused_arg ? keys : (unsigned long long *)nullptr, ticket,
                            fused_arg ? argmax : (long long *)nullptr, fused_arg ? maxval : (float *)nullptr,

@@ -253,6 +253,88 @@ def label_dlogits(dims, params, cv, label, lse, scale, scale_device=None, algo=_
     return dout
 
 
+def _label_ws(lib, dims, B, dev, algo, cache, weight):
+    nbytes = lib.c2v_label_workspace_bytes(ctypes.byref(dims), B)
+    if cache is not None and weight is not None:
+        ws, reuse = cache.get(nbytes, dev, weight)
+        if reuse:
+            algo = int(algo) | REUSE_PREP
+    else:
+        ws = _empty((nbytes,), torch.uint8, dev)
+    return ws, algo
+
+
+def angular_loss(dims, params, cv, label, margin, inverse_temp, want_logits=False, algo=_lib.ALGO_AUTO, cache=None,
+                 weight=None):
+    """model.py:71-80 + main.py:251-264 + main.py:285 in one pass over the label GEMM's accumulators
+    -> (loss 0-d, lse [B], argmax int64 [B], maxval [B], inv_norms [B + C], outputs [B, C] or None).  inv_norms is what
+    angular_dlogits / angular_backward_ws need; with want_logits=False the [B, C] logits are never written."""
+    lib = _lib.load()
+    _need_cuda(cv, label)
+    B = cv.shape[0]
+    dev = cv.device
+    label = _idx(label, "label", (B,))
+    with torch.cuda.device(dev):
+        out = _empty((B, dims.label_count), torch.float32, dev) if want_logits else None
+        loss = _empty((), torch.float32, dev)
+        lse = _empty((B,), torch.float32, dev)
+        am = _empty((B,), torch.int64, dev)
+        mx = _empty((B,), torch.float32, dev)
+        inv = _empty((B + dims.label_count,), torch.float32, dev)
+        ws, algo = _label_ws(lib, dims, B, dev, algo, cache, weight)
+        cv = _f32c(cv, "code_vector")
+        rc = lib.c2v_angular_loss_argmax(ctypes.byref(dims), ctypes.byref(params), _ptr(cv), _ptr(label), B, float(margin),
+                                         float(inverse_temp), _ptr(out), _ptr(loss), _ptr(lse), _ptr(am), _ptr(mx), _ptr(inv),
+                                         _ptr(ws), ws.numel(), int(algo), _stream(dev))
+        _lib.check(rc, "c2v_angular_loss_argmax")
+    return loss, lse, am, mx, inv, out
+
+
+def angular_dlogits(dims, params, cv, label, lse, inv_norms, margin, inverse_temp, scale, scale_device=None,
+                    algo=_lib.ALGO_AUTO, cache=None, weight=None):
+    """d(mean NLL)/d(cv . W^T) [B, C] of the angular head (scale and scale_device as in label_dlogits), recomputed from
+    cv and W_out"""
+    lib = _lib.load()
+    B = cv.shape[0]
+    dev = cv.device
+    label = _idx(label, "label", (B,))
+    with torch.cuda.device(dev):
+        g = _empty((B, dims.label_count), torch.float32, dev)
+        ws, algo = _label_ws(lib, dims, B, dev, algo, cache, weight)
+        cv = _f32c(cv, "code_vector"); lse = _f32c(lse, "lse"); inv = _f32c(inv_norms, "inv_norms")
+        sd = _f32c(scale_device, "scale_device") if scale_device is not None else None
+        rc = lib.c2v_angular_dlogits(ctypes.byref(dims), ctypes.byref(params), _ptr(cv), _ptr(label), _ptr(lse), _ptr(inv), B,
+                                     float(margin), float(inverse_temp), float(scale), _ptr(sd), _ptr(g), _ptr(ws), ws.numel(),
+                                     int(algo), _stream(dev))
+        _lib.check(rc, "c2v_angular_dlogits")
+    return g
+
+
+def angular_backward_ws(dims, params, cv, d_dot, inv_norms, need_cv=True, need_w=True, algo=_lib.ALGO_AUTO, cache=None,
+                        weight=None, absmax_ready=False):
+    """backward of the angular head from G = angular_dlogits(...) -> (d_code_vector, d_output_weight).  With the label
+    PrepCache of the forward (cache + weight) the contractions run on the tensor cores and stream the cached W_out image;
+    absmax_ready: d_dot is the tensor angular_dlogits just returned for the same cache."""
+    lib = _lib.load()
+    B = cv.shape[0]
+    dev = cv.device
+    with torch.cuda.device(dev):
+        d_cv = torch.empty_like(cv) if need_cv else None
+        d_w = _empty((dims.label_count, dims.encode), torch.float32, dev) if need_w else None
+        cv = _f32c(cv, "code_vector"); d_dot = _f32c(d_dot, "d_dot"); inv = _f32c(inv_norms, "inv_norms")
+        if cache is not None and weight is not None:
+            nbytes = lib.c2v_label_workspace_bytes(ctypes.byref(dims), B)
+            ws, reuse = cache.get(nbytes, dev, weight)
+            flags = int(algo) | (REUSE_PREP if reuse else 0) | (GRAD_ABSMAX_READY if absmax_ready else 0)
+        else:
+            ws, flags = None, int(algo)
+        rc = lib.c2v_angular_backward_ws(ctypes.byref(dims), ctypes.byref(params), _ptr(cv), _ptr(d_dot), _ptr(inv), B,
+                                         _ptr(d_cv), _ptr(d_w), _ptr(ws), ws.numel() if ws is not None else 0, flags,
+                                         _stream(dev))
+        _lib.check(rc, "c2v_angular_backward_ws")
+    return d_cv, d_w
+
+
 def angular_logits(dims, params, cv, label, margin, inverse_temp):
     """model.py:71-80"""
     lib = _lib.load()

@@ -155,6 +155,36 @@ class _LabelLossFn(torch.autograd.Function):
         return d_cv, d_w, d_b, None, None, None, None
 
 
+class _AngularLossFn(torch.autograd.Function):
+    """mean NLL of log_softmax over the angular-margin head (model.py:71-80 + main.py:251-264) without materialising the
+    logits: the label GEMM's angular epilogue produces loss / logsumexp / arg-max; the backward recomputes
+    G = d loss / d (cv . W^T) tile by tile, runs the plain label backward on it and projects through F.normalize."""
+
+    @staticmethod
+    def forward(ctx, cv, w_out, label, dims, margin, inverse_temp, algo, cache):
+        params = CF.make_params(None, None, None, None, None, None, w_out, None)
+        if any(ctx.needs_input_grad[:2]):
+            algo = int(algo) | CF.NO_PDL
+        loss, lse, am, mx, inv, _ = CF.angular_loss(dims, params, cv, label, margin, inverse_temp, want_logits=False,
+                                                    algo=algo, cache=cache, weight=w_out)
+        ctx.save_for_backward(cv, w_out, label, lse, inv)
+        ctx.dims, ctx.cache, ctx.algo, ctx.cfg = dims, cache, algo, (margin, inverse_temp)
+        ctx.mark_non_differentiable(am, mx)
+        return loss, am, mx
+
+    @staticmethod
+    def backward(ctx, d_loss, _d_am, _d_mx):
+        cv, w_out, label, lse, inv = ctx.saved_tensors
+        margin, inverse_temp = ctx.cfg
+        params = CF.make_params(None, None, None, None, None, None, w_out, None)
+        B = cv.shape[0]
+        g = CF.angular_dlogits(ctx.dims, params, cv, label, lse, inv, margin, inverse_temp, 1.0 / B,
+                               scale_device=d_loss.reshape(1), algo=ctx.algo, cache=ctx.cache, weight=w_out)
+        d_cv, d_w = CF.angular_backward_ws(ctx.dims, params, cv, g, inv, ctx.needs_input_grad[0], ctx.needs_input_grad[1],
+                                           algo=int(ctx.algo) & 0xff, cache=ctx.cache, weight=w_out, absmax_ready=True)
+        return d_cv, d_w, None, None, None, None, None, None
+
+
 class Code2Vec(nn.Module):
     """the code2vec model (H100-native drop-in for model.py:15-105)"""
 
@@ -210,6 +240,14 @@ class Code2Vec(nn.Module):
         self._dropout_calls += 1
         return int(torch.randint(0, 2 ** 62, (1,)).item())
 
+    def _angular_outputs(self, code_vector, label, dims):
+        """the angular-margin head's logits (model.py:71-80) on the CUDA cores"""
+        option = self.option
+        if torch.is_grad_enabled() and (code_vector.requires_grad or self.output_linear.requires_grad):
+            return _AngularFn.apply(code_vector, self.output_linear, label, dims, option.angular_margin, option.inverse_temp)
+        params = CF.make_params(None, None, None, None, None, None, self.output_linear, None)
+        return CF.angular_logits(dims, params, code_vector, label, option.angular_margin, option.inverse_temp)
+
     # -- the reference surface -------------------------------------------------------------
     def check_indices(self):
         """Synchronise and raise IndexError if any forward so far saw an index outside the embedding tables
@@ -232,12 +270,7 @@ class Code2Vec(nn.Module):
             starts, paths, ends, dims, drop_p, training, seed, self.algo, self._enc_cache)
 
         if option.angular_margin_loss:
-            if torch.is_grad_enabled() and (code_vector.requires_grad or self.output_linear.requires_grad):
-                outputs = _AngularFn.apply(code_vector, self.output_linear, label, dims, option.angular_margin,
-                                           option.inverse_temp)
-            else:
-                params = CF.make_params(None, None, None, None, None, None, self.output_linear, None)
-                outputs = CF.angular_logits(dims, params, code_vector, label, option.angular_margin, option.inverse_temp)
+            outputs = self._angular_outputs(code_vector, label, dims)
         else:
             outputs = _LabelFn.apply(code_vector, self.output_linear.weight, self.output_linear.bias, dims,
                                      _lib.ALGO_FFMA if self.algo == _lib.ALGO_FFMA else _lib.ALGO_AUTO,
@@ -249,10 +282,10 @@ class Code2Vec(nn.Module):
     def forward_loss(self, starts, paths, ends, label):
         """-> (loss, pred_label [b], pred_score [b], code_vector [b,H], attention [b,L]); loss is the mean NLL the
         reference's `calculate_loss(preds, label, criterion, option)` returns (criterion weights are all
-        1) and is autograd-connected; the [b, C] logits are never written.  Plain label head only; shapes the fused
-        kernel does not take fall back to forward() + c2v_loss_argmax."""
-        if self.option.angular_margin_loss:
-            raise NotImplementedError("forward_loss() needs the plain label head")
+        1) and is autograd-connected; the [b, C] logits are never written.  Both label heads: with
+        option.angular_margin_loss the loss, arg-max and max are those of the angular-margin logits (model.py:71-80).
+        Shapes the fused kernel does not take, and algo="ffma", fall back to forward()'s head + eager log_softmax / NLL +
+        torch.max."""
         self._enc_cache.raise_deferred()
         self._enc_cache.fuse_grad_accumulation = self.fuse_grad_accumulation
         self._enc_cache.on_path_grads_ready = self.on_path_grads_ready
@@ -264,7 +297,16 @@ class Code2Vec(nn.Module):
             self.terminal_embedding.weight, self.path_embedding.weight, self.input_linear.weight,
             self.input_layer_norm.weight, self.input_layer_norm.bias, self.attention_parameter,
             starts, paths, ends, dims, drop_p, training, seed, self.algo, self._enc_cache)
-        if self.algo != _lib.ALGO_FFMA and CF.label_loss_supported(dims, starts.shape[0]):
+        fused = self.algo != _lib.ALGO_FFMA and CF.label_loss_supported(dims, starts.shape[0])
+        if self.option.angular_margin_loss:
+            if fused:
+                loss, am, mx = _AngularLossFn.apply(code_vector, self.output_linear, label, dims, self.option.angular_margin,
+                                                    self.option.inverse_temp, _lib.ALGO_AUTO, self._lab_cache)
+            else:
+                outputs = self._angular_outputs(code_vector, label, dims)
+                loss = F.nll_loss(F.log_softmax(outputs, dim=1), label)
+                mx, am = torch.max(outputs.detach(), dim=1)
+        elif fused:
             loss, am, mx = _LabelLossFn.apply(code_vector, self.output_linear.weight, self.output_linear.bias, label, dims,
                                               _lib.ALGO_AUTO, self._lab_cache)
         else:

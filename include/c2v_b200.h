@@ -199,6 +199,32 @@ int c2v_label_loss_argmax(const c2v_dims *d, const c2v_params *p, const float *c
 int c2v_label_dlogits(const c2v_dims *d, const c2v_params *p, const float *code_vector, const int64_t *label,
                       const float *lse, int32_t B, float scale, const float *scale_device, float *d_outputs,
                       void *workspace, size_t workspace_bytes, int32_t algo, void *stream);
+/* The same trio for the angular-margin head: model.py:71-80 + main.py:251-264 + main.py:285 fused into the tensor-core
+ * label GEMM.  The epilogue turns dot = cv . W^T into cos = dot icv[b] iw[c] and the logit s cos -- s phi(cos) at
+ * c == label[b], phi(c) = c > 0 ? c cos(margin) - sqrt(1 - c^2) sin(margin) : c, s = inverse_temp -- exactly as
+ * c2v_angular_logits does; output_bias is not read.
+ * c2v_angular_loss_argmax: loss / lse / argmax / maxval as in c2v_label_loss_argmax, over the angular logits (the [B, C]
+ * logits are written only if outputs != NULL).  inv_norms [B + C] (out, not NULL): 1 / max(|cv_b|, 1e-12) then
+ * 1 / max(|W_c|, 1e-12), kept for the two calls below.  Same label workspace, same support rule
+ * (c2v_label_loss_supported). */
+int c2v_angular_loss_argmax(const c2v_dims *d, const c2v_params *p, const float *code_vector, const int64_t *label,
+                            int32_t B, float margin, float inverse_temp, float *outputs, float *loss, float *lse,
+                            int64_t *argmax, float *maxval, float *inv_norms, void *workspace, size_t workspace_bytes,
+                            int32_t algo, void *stream);
+/* Backward companion: G = d loss / d (cv . W^T) [B, C], recomputed tile by tile from the GEMM's accumulators
+ * (scale, scale_device as in c2v_label_dlogits; lse and inv_norms from c2v_angular_loss_argmax); feed it to
+ * c2v_angular_backward_ws (C2V_FLAG_GRAD_ABSMAX_READY applies as after c2v_label_dlogits). */
+int c2v_angular_dlogits(const c2v_dims *d, const c2v_params *p, const float *code_vector, const int64_t *label,
+                        const float *lse, const float *inv_norms, int32_t B, float margin, float inverse_temp, float scale,
+                        const float *scale_device, float *d_dot, void *workspace, size_t workspace_bytes, int32_t algo,
+                        void *stream);
+/* c2v_label_backward_ws on G (no bias), then the radial projection of F.normalize:
+ *   d_code_vector[b] = (G . W)[b] - icv[b]^2 (cv[b] . (G . W)[b]) cv[b]   [B, H]
+ *   d_output_weight[c] = (G^T . cv)[c] - iw[c]^2 (W[c] . (G^T . cv)[c]) W[c]   [C, H]   (either may be NULL).
+ * Same workspace / algo rules (and CUDA-core fallback) as c2v_label_backward_ws. */
+int c2v_angular_backward_ws(const c2v_dims *d, const c2v_params *p, const float *code_vector, const float *d_dot,
+                            const float *inv_norms, int32_t B, float *d_code_vector, float *d_output_weight, void *workspace,
+                            size_t workspace_bytes, int32_t algo, void *stream);
 /* Label logits + the prediction the reference takes from them (`torch.max(preds, dim=1)`,
  * main.py:285; first maximum wins) in one call: the argmax pass runs right behind the GEMM while the
  * [B,C] logits are still in L2.  argmax int64 [B], maxval fp32 [B] (either may be NULL).
