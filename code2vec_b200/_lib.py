@@ -12,6 +12,7 @@ LIB_PATH = os.environ.get("C2V_LIB", os.path.join(_HERE, "libc2v_b200.so"))   # 
 C2V_OK, C2V_EINVAL, C2V_ECUDA, C2V_EWORKSPACE, C2V_EINDEX, C2V_EUNSUPPORTED = 0, -1, -2, -3, -4, -5
 ALGO_AUTO, ALGO_FFMA, ALGO_TCGEN05 = 0, 1, 2
 ABI_VERSION = 1
+TOPK_MAX = 16                # C2V_TOPK_MAX: the largest k of the fused top-k (c2v_label_topk / c2v_angular_topk)
 
 c_i32, c_i64, c_f32, c_vp, c_sz = ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_void_p, ctypes.c_size_t
 
@@ -76,6 +77,11 @@ SYMBOLS = {
     "c2v_angular_backward_ws": (ctypes.c_int, [_P(Dims), _P(Params), c_vp, c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_sz, c_i32,
                                                c_vp]),
     "c2v_angular_logits": (ctypes.c_int, [_P(Dims), _P(Params), c_vp, c_vp, c_i32, c_f32, c_f32, c_vp, c_vp]),
+    "c2v_label_topk_supported": (ctypes.c_int, [_P(Dims), c_i32, c_i32]),
+    "c2v_label_topk_workspace_bytes": (c_sz, [_P(Dims), c_i32, c_i32]),
+    "c2v_label_topk": (ctypes.c_int, [_P(Dims), _P(Params), c_vp, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp, c_sz, c_i32, c_vp]),
+    "c2v_angular_topk": (ctypes.c_int, [_P(Dims), _P(Params), c_vp, c_i32, c_i32, c_f32, c_vp, c_vp, c_vp, c_vp, c_sz, c_i32,
+                                        c_vp]),
     "c2v_angular_forward_train": (ctypes.c_int, [_P(Dims), _P(Params), c_vp, c_vp, c_i32, c_f32, c_f32, c_vp, c_vp, c_vp, c_vp]),
     "c2v_angular_backward": (ctypes.c_int, [_P(Dims), _P(Params), c_vp, c_vp, c_i32, c_f32, c_f32, c_vp, c_vp, c_vp, c_vp,
                                             c_vp, c_vp, c_vp]),

@@ -515,6 +515,88 @@ int c2v_angular_logits(const c2v_dims *d, const c2v_params *p, const float *code
     return rc;
 }
 
+int c2v_label_topk_supported(const c2v_dims *d, int32_t B, int32_t k)
+{
+    if (!dims_ok(d) || k < 1 || k > C2V_TOPK_MAX || k > d->label_count) return 0;
+    return c2v_label_loss_supported(d, B);
+}
+
+size_t c2v_label_topk_workspace_bytes(const c2v_dims *d, int32_t B, int32_t k)
+{
+    if (!dims_ok(d) || B < 1 || k < 1 || k > C2V_TOPK_MAX || k > d->label_count) return 0;
+    return align_up(label_topk_workspace_bytes(d, B, k), 1024);
+}
+
+// argument checks shared by c2v_label_topk / c2v_angular_topk, all before any CUDA call
+static int topk_args_ok(const char *fn, const c2v_dims *d, const c2v_params *p, const float *code_vector, int32_t B,
+                        int32_t k, const int64_t *indices, const float *values, const void *workspace, size_t workspace_bytes,
+                        int32_t algo)
+{
+    if (!d) { set_error("%s: dims is NULL", fn); return C2V_EINVAL; }
+    if (!dims_ok(d)) return C2V_EINVAL;
+    if (!p || !p->output_weight || !code_vector || !indices || !values) {
+        set_error("%s: NULL pointer argument", fn);
+        return C2V_EINVAL;
+    }
+    if (B < 1 || k < 1 || k > d->label_count) {
+        set_error("%s: B=%d, k=%d: needs B >= 1 and 1 <= k <= label_count (%lld)", fn, B, k, (long long)d->label_count);
+        return C2V_EINVAL;
+    }
+    const int base_algo = algo & 0xff;
+    if (base_algo != C2V_ALGO_AUTO && base_algo != C2V_ALGO_FFMA && base_algo != C2V_ALGO_TCGEN05) {
+        set_error("%s: unknown algo %d", fn, base_algo);
+        return C2V_EINVAL;
+    }
+    if (!c2v_label_topk_supported(d, B, k) || base_algo == C2V_ALGO_FFMA) {
+        set_error("%s: the fused top-k runs on the tensor cores and needs encode_size %% 4 == 0 and <= 256, B <= 2048 and "
+                  "k <= %d (got encode_size %d, B %d, k %d, algo %d); take the top k of c2v_label_logits' output instead",
+                  fn, C2V_TOPK_MAX, d->encode, B, k, base_algo);
+        return C2V_EUNSUPPORTED;
+    }
+    const size_t need = label_topk_workspace_bytes(d, B, k);
+    if (!workspace || workspace_bytes < need) {
+        set_error("%s: workspace too small: %zu < %zu", fn, workspace ? workspace_bytes : (size_t)0, need);
+        return C2V_EWORKSPACE;
+    }
+    return C2V_OK;
+}
+
+int c2v_label_topk(const c2v_dims *d, const c2v_params *p, const float *code_vector, int32_t B, int32_t k,
+                   int64_t *indices, float *values, float *probs, void *workspace, size_t workspace_bytes, int32_t algo,
+                   void *stream)
+{
+    const int rc = topk_args_ok("c2v_label_topk", d, p, code_vector, B, k, indices, values, workspace, workspace_bytes, algo);
+    if (rc != C2V_OK) return rc;
+    const bool reuse_prep = (algo & C2V_FLAG_REUSE_PREP) != 0;
+    g_pdl_this_call = (algo & C2V_FLAG_NO_PDL) == 0;
+    LabelLossArgs la;
+    memset(&la, 0, sizeof(la));
+    la.topk_k = k; la.topk_idx = reinterpret_cast<long long *>(indices); la.topk_val = values; la.topk_prob = probs;
+    return launch_label_tcgen05_ex(d, code_vector, B, p->output_weight, p->output_bias, nullptr, nullptr, nullptr, workspace,
+                                   workspace_bytes, reuse_prep, static_cast<cudaStream_t>(stream), &la);
+}
+
+int c2v_angular_topk(const c2v_dims *d, const c2v_params *p, const float *code_vector, int32_t B, int32_t k,
+                     float inverse_temp, int64_t *indices, float *values, float *probs, void *workspace,
+                     size_t workspace_bytes, int32_t algo, void *stream)
+{
+    int rc = topk_args_ok("c2v_angular_topk", d, p, code_vector, B, k, indices, values, workspace, workspace_bytes, algo);
+    if (rc != C2V_OK) return rc;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const bool reuse_prep = (algo & C2V_FLAG_REUSE_PREP) != 0;
+    g_pdl_this_call = (algo & C2V_FLAG_NO_PDL) == 0;
+    float *inv = label_topk_inv_norms(d, B, k, workspace);
+    rc = launch_row_inv_norm(code_vector, B, d->encode, inv, st);
+    if (rc == C2V_OK) rc = launch_row_inv_norm(p->output_weight, d->label_count, d->encode, inv + B, st);
+    if (rc != C2V_OK) return rc;
+    LabelLossArgs la;
+    memset(&la, 0, sizeof(la));
+    la.inv_norms = inv; la.inverse_temp = inverse_temp;
+    la.topk_k = k; la.topk_idx = reinterpret_cast<long long *>(indices); la.topk_val = values; la.topk_prob = probs;
+    return launch_label_tcgen05_ex(d, code_vector, B, p->output_weight, nullptr, nullptr, nullptr, nullptr, workspace,
+                                   workspace_bytes, reuse_prep, st, &la);
+}
+
 int c2v_angular_forward_train(const c2v_dims *d, const c2v_params *p, const float *code_vector, const int64_t *label,
                               int32_t B, float margin, float inverse_temp, float *outputs, float *cosine,
                               float *inv_norms, void *stream)

@@ -128,7 +128,15 @@ struct LabelLossArgs {
     // The logits are s cos (s phi(cos) at the label), the bias is ignored, and dlogits mode writes d loss / d (cv . W^T).
     const float *inv_norms;
     float cos_m, sin_m, inverse_temp;
+    // top-k mode when topk_k > 0 (label_topk_workspace_bytes of workspace, no other output, label not read): the topk_k
+    // largest logits of every row, value descending then column ascending -> topk_idx / topk_val [B, topk_k], and
+    // topk_prob (or NULL) = their softmax probabilities.  With inv_norms the logits are s cos without the margin.
+    int topk_k;
+    long long *topk_idx;
+    float *topk_val, *topk_prob;
 };
+size_t label_topk_workspace_bytes(const c2v_dims *d, int B, int k);
+float *label_topk_inv_norms(const c2v_dims *d, int B, int k, void *ws);     // where the angular head's inv_norms go
 int launch_label_tcgen05_ex(const c2v_dims *d, const float *cv, int B, const float *Wout, const float *bias,
                             float *out, long long *argmax, float *maxval, void *ws, size_t ws_bytes, bool reuse_prep,
                             cudaStream_t st, const LabelLossArgs *la);

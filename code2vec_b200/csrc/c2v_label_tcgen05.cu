@@ -160,7 +160,30 @@ struct LtLoss {
     unsigned *gmax_bits;      // dlogits mode: bits of max |value stored| over the launch (what the label backward's fp16 split scales by)
     const float *icv, *iw;    // angular: 1 / max(|cv_b|, 1e-12) [M], 1 / max(|W_c|, 1e-12) [N]
     float cos_m, sin_m, s;    // angular: cos(margin), sin(margin), inverse_temp
+    unsigned long long *topk; // top-k mode: per CTA 512 lists (column quarter x 128 rows) of topk_k keys, see lt_topk_insert
+    int topk_k;
 };
+
+// Top-k mode (the label_gemm_v2_kernel<*, true> instantiations): a thread of the epilogue (one row, one column quarter of
+// its CTA's m-tile) keeps the topk_k largest keys  lt_orderable(v) << 32 | ~col  it has seen, sorted descending, in its
+// own slot of the workspace (too big for shared memory, which is full); only the upper word of the k-th key stays in a
+// register.  Key order is value descending, then column ascending: torch.sort(descending=True, stable=True).
+// Inserts key into lst[0..k) (empty slots hold 0, below every key) and returns the upper word of the new k-th key:
+// slot i becomes max(old[i], min(key, old[i - 1])), so the loads do not wait for each other.
+__device__ __forceinline__ uint32_t lt_topk_insert(unsigned long long *lst, int k, unsigned long long key) {
+    unsigned long long prev = ~0ull, n = 0ull;
+#pragma unroll
+    for (int i = 0; i < C2V_TOPK_MAX; ++i) {
+        if (i < k) {
+            const unsigned long long o = lst[i];
+            const unsigned long long c = key < prev ? key : prev;
+            n = o > c ? o : c;
+            if (n != o) lst[i] = n;
+            prev = o;
+        }
+    }
+    return (uint32_t)(n >> 32);
+}
 constexpr float LT_LOG2E = 1.4426950408889634f;
 __device__ __forceinline__ float lt_ex2(float x) {
     float r;
@@ -196,7 +219,9 @@ constexpr int SMEM_BYTES = SMEM_BAR_OFF + 128 + 1024;
 // does *1/scale + bias -> running arg-max (smem table, 64-bit atomicMax) -> padded smem tile -> row-contiguous stores.
 // Bound: the logits write (B*C*4 bytes); the arg-max costs no extra pass over them.
 // ANG: the angular-margin epilogue (see LtLoss); a template parameter so that the plain head compiles without it.
-template <bool ANG>
+// TOPK: the running top-k epilogue (lt_topk_insert) instead of logits / arg-max / dlogits; needs lane order (per_m > 0,
+// a CTA sees every column of its slice for its rows).  With ANG the logits are s cos without the margin: no label is read.
+template <bool ANG, bool TOPK>
 __global__ void __launch_bounds__(lt2::THREADS, 1)
 label_gemm_v2_kernel(const uint8_t *__restrict__ imgA, const uint8_t *__restrict__ imgB,
                      const float *__restrict__ bias, const float *__restrict__ hdr, float *__restrict__ out,
@@ -279,6 +304,12 @@ label_gemm_v2_kernel(const uint8_t *__restrict__ imgA, const uint8_t *__restrict
             return c2 < N ? __ldg(colv + c2) : 0.0f;
         };
         float bias_next = bias_of(0);
+        unsigned long long *tk_list = nullptr;                // top-k: this thread's list and the upper word of its k-th key
+        uint32_t tk_thr = 0;
+        if constexpr (TOPK) {
+            tk_list = ls.topk + ((size_t)blockIdx.x * 512 + cq * 128 + q * 32 + lane) * ls.topk_k;
+            for (int j = 0; j < ls.topk_k; ++j) tk_list[j] = 0ull;
+        }
         for (int i = 0; i < my_tiles; ++i) {
             const LtTile tt = tile_of(i);
             const long long nt = tt.nt; const int mt = tt.mt;
@@ -350,21 +381,26 @@ label_gemm_v2_kernel(const uint8_t *__restrict__ imgA, const uint8_t *__restrict
                     v[j] = r[j] * inv_scale * icv_r * w4.x; v[j + 1] = r[j + 1] * inv_scale * icv_r * w4.y;
                     v[j + 2] = r[j + 2] * inv_scale * icv_r * w4.z; v[j + 3] = r[j + 3] * inv_scale * icv_r * w4.w;
                 }
-                const long long grow = row0 + lane;
-                const long long tj = (grow < M ? ls.label[grow] : -1) - col0;
-                const int tji = (tj >= 0 && tj < n_cols) ? (int)tj : -1;
-                float phi = 0.0f;
-                if (__any_sync(0xffffffffu, tji >= 0)) {
-                    // the PTX select chain of the loss partials below: a dynamic v[tj] would put v[] in local memory
+                if constexpr (TOPK) {                                               // label-free: s cos, no margin
 #pragma unroll
-                    for (int j = 0; j < 32; ++j)
-                        asm volatile("{\n\t.reg .pred p;\n\tsetp.eq.s32 p, %2, %3;\n\tselp.f32 %0, %1, %0, p;\n\t}"
-                                     : "+f"(cos_t) : "f"(v[j]), "r"(tji), "r"(j));
-                    // phi(c) = c > 0 ? c cos_m - sqrt(1 - c^2) sin_m : c, for the target element only
-                    phi = cos_t > 0.0f ? cos_t * ls.cos_m - sqrtf(1.0f - cos_t * cos_t) * ls.sin_m : cos_t;
+                    for (int j = 0; j < 32; ++j) v[j] *= ls.s;
+                } else {
+                    const long long grow = row0 + lane;
+                    const long long tj = (grow < M ? ls.label[grow] : -1) - col0;
+                    const int tji = (tj >= 0 && tj < n_cols) ? (int)tj : -1;
+                    float phi = 0.0f;
+                    if (__any_sync(0xffffffffu, tji >= 0)) {
+                        // the PTX select chain of the loss partials below: a dynamic v[tj] would put v[] in local memory
+#pragma unroll
+                        for (int j = 0; j < 32; ++j)
+                            asm volatile("{\n\t.reg .pred p;\n\tsetp.eq.s32 p, %2, %3;\n\tselp.f32 %0, %1, %0, p;\n\t}"
+                                         : "+f"(cos_t) : "f"(v[j]), "r"(tji), "r"(j));
+                        // phi(c) = c > 0 ? c cos_m - sqrt(1 - c^2) sin_m : c, for the target element only
+                        phi = cos_t > 0.0f ? cos_t * ls.cos_m - sqrtf(1.0f - cos_t * cos_t) * ls.sin_m : cos_t;
+                    }
+#pragma unroll
+                    for (int j = 0; j < 32; ++j) v[j] = (j == tji ? phi : v[j]) * ls.s;
                 }
-#pragma unroll
-                for (int j = 0; j < 32; ++j) v[j] = (j == tji ? phi : v[j]) * ls.s;
             }
             if (ls.part || ls.lse) {
                 const long long grow = row0 + lane;                                     // this thread's output row
@@ -391,7 +427,7 @@ label_gemm_v2_kernel(const uint8_t *__restrict__ imgA, const uint8_t *__restrict
                         if (tj >= 0 && tj < n_cols) ls.tgt[grow] = t;
                     }
                 }
-                if (ls.lse) {                                                           // dlogits (overwrites v)
+                if (!TOPK && ls.lse) {                                                  // dlogits (overwrites v)
                     const float lb = (grow < M ? ls.lse[grow] : 0.0f) * LT_LOG2E;
                     const float sc = ls.dscale_ptr ? ls.dscale * *ls.dscale_ptr : ls.dscale;
                     if constexpr (!ANG) {
@@ -418,6 +454,38 @@ label_gemm_v2_kernel(const uint8_t *__restrict__ imgA, const uint8_t *__restrict
                         for (int j = 0; j < 32; ++j) gmax = fmaxf(gmax, j < n_cols ? fabsf(v[j]) : 0.0f);
                     }
                 }
+            }
+            if constexpr (TOPK) {
+                // candidates: keys above the k-th one (columns arrive in increasing order, so an equal value never
+                // displaces an earlier column).  v + 0: -0 ranks as +0, as torch compares them equal.
+                uint32_t cand = 0;
+                if (lane < n_rows) {
+#pragma unroll
+                    for (int j = 0; j < 32; ++j) {
+                        const uint32_t h = lt_orderable(v[j] + 0.0f);
+                        v[j] = __uint_as_float(h);
+                        cand |= (j < n_cols && h > tk_thr) ? (1u << j) : 0u;
+                    }
+                }
+                if (cand) {
+                    // this row's keys go back to its own staging slot (read above; the warpgroup barrier at the top of the
+                    // next tile orders the reuse), so that the insert loop can index them
+                    uint32_t *ks = reinterpret_cast<uint32_t *>(stage_all + (q * 32 + lane) * xld + xcol);
+#pragma unroll
+                    for (int j = 0; j < 32; j += 4)
+                        *reinterpret_cast<uint4 *>(ks + j) = make_uint4(__float_as_uint(v[j]), __float_as_uint(v[j + 1]),
+                                                                        __float_as_uint(v[j + 2]), __float_as_uint(v[j + 3]));
+                    do {
+                        const int j = __ffs(cand) - 1;
+                        cand &= cand - 1;
+                        const uint32_t h = ks[j];
+                        if (h > tk_thr)
+                            tk_thr = lt_topk_insert(tk_list, ls.topk_k, ((unsigned long long)h << 32) |
+                                                                            (unsigned long long)(0xFFFFFFFFu - (uint32_t)(col0 + j)));
+                    } while (cand);
+                }
+                __syncwarp();
+                continue;
             }
             if (want_arg && lane < n_rows && n_cols > 0 && !C2V_EXPT(dbg, 2)) {
                 float m = -INFINITY;
@@ -580,6 +648,64 @@ loss_finalize_kernel(const float2 *__restrict__ part2, int nsplit, int Mpad, con
     }
 }
 
+// ---- top-k: merging the per-thread lists of label_gemm_v2_kernel<*, true> --------------------------------------------
+constexpr int LT_TOPK_MAX_CTAS = 256;               // grid cap of the top-k GEMM: bounds its workspace independently of the device
+// one warp per row b: the row's 4 per_m sorted lists (list l = 4 slice + column quarter, written by CTA slice * n_mt + mt)
+// are merged k-way -- every lane holds the best head of its lists l = lane, lane + 32, ...; k rounds of a warp maximum.
+// part2 != NULL: lse from the row's (max, sum exp) partials and prob = exp(v - lse).
+__global__ void __launch_bounds__(256)
+topk_merge_kernel(const unsigned long long *__restrict__ lists, int k, int M, int n_mt, int per_m,
+                  const float2 *__restrict__ part2, int Mpad, long long *__restrict__ idx, float *__restrict__ val,
+                  float *__restrict__ prob)
+{
+    __shared__ unsigned char heads[8][4 * LT_TOPK_MAX_CTAS];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const int b = blockIdx.x * 8 + w;
+    if (b >= M) return;
+    const int L = 4 * per_m, mt = b >> 7, r = b & 127;
+    unsigned char *hd = heads[w];
+    for (int l = lane; l < L; l += 32) hd[l] = 0;
+    unsigned long long best = 0ull;
+    int bl = -1;
+    auto rescan = [&]() {
+        best = 0ull; bl = -1;
+        for (int l = lane; l < L; l += 32) {
+            const int h = hd[l];
+            const unsigned long long key = h < k ? lists[((size_t)((l >> 2) * n_mt + mt) * 512 + (l & 3) * 128 + r) * k + h] : 0ull;
+            if (key > best) { best = key; bl = l; }
+        }
+    };
+    rescan();
+    float lse = 0.0f;
+    if (prob) {
+        float Mx = -INFINITY, S = 0.0f;
+        if (lane < LT_PSPLIT) { const float2 pr = part2[(size_t)lane * Mpad + b]; Mx = pr.x; S = pr.y; }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const float m2 = __shfl_xor_sync(0xffffffffu, Mx, o), s2 = __shfl_xor_sync(0xffffffffu, S, o);
+            lt_merge(Mx, S, m2, s2);
+        }
+        lse = __shfl_sync(0xffffffffu, Mx + logf(S), 0);
+    }
+    for (int i = 0; i < k; ++i) {
+        unsigned long long top = best;
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const unsigned long long t = __shfl_xor_sync(0xffffffffu, top, o);
+            top = t > top ? t : top;
+        }
+        if (lane == 0) {
+            const float v = lt_from_orderable((uint32_t)(top >> 32));
+            const size_t o = (size_t)b * k + i;
+            idx[o] = (long long)(0xFFFFFFFFu - (uint32_t)(top & 0xFFFFFFFFull));
+            val[o] = v;
+            if (prob) prob[o] = expf(v - lse);
+        }
+        if (bl >= 0 && best == top) { hd[bl] += 1; rescan(); }          // keys are unique (one column each): one winner
+        __syncwarp();
+    }
+}
+
 // K (= encode_size) is zero-padded to a multiple of 64 inside the operand images
 bool label_tcgen05_shape_ok(const c2v_dims *d) { return d->encode >= 4 && d->encode <= 256 && (d->encode & 3) == 0; }
 
@@ -599,6 +725,25 @@ size_t label_tcgen05_workspace_bytes(const c2v_dims *d, int B)
     const size_t nkb = (size_t)(d->encode + 63) / 64;
     const size_t mt = (size_t)(B + 127) / 128, nt = (size_t)(d->label_count + 127) / 128;
     return 1024 + lt_keys_bytes(B) + (mt + nt) * nkb * 2 * lt::TILE_BYTES + lt_loss_bytes(B, d->label_count);
+}
+
+// top-k region, behind the label workspace (whose layout it leaves alone): the GEMM's lists, 512 x k keys per CTA |
+// inv_norms [B + C] of the angular head
+static size_t lt_topk_lists_bytes(const c2v_dims *d, int B, int k)
+{
+    const long long n_tiles = (long long)((B + 127) / 128) * ((d->label_count + 127) / 128);
+    const long long ctas = n_tiles < LT_TOPK_MAX_CTAS ? n_tiles : LT_TOPK_MAX_CTAS;
+    return align_up((size_t)ctas * 512 * (size_t)k * 8, 1024);
+}
+size_t label_topk_workspace_bytes(const c2v_dims *d, int B, int k)
+{
+    return align_up(label_tcgen05_workspace_bytes(d, B), 1024) + lt_topk_lists_bytes(d, B, k) +
+           align_up((size_t)(B + d->label_count) * sizeof(float), 1024);
+}
+float *label_topk_inv_norms(const c2v_dims *d, int B, int k, void *ws)
+{
+    return reinterpret_cast<float *>(static_cast<uint8_t *>(ws) + align_up(label_tcgen05_workspace_bytes(d, B), 1024) +
+                                     lt_topk_lists_bytes(d, B, k));
 }
 
 int launch_loss_argmax(const float *out, const long long *label, int B, long long C, float *loss,
@@ -668,8 +813,10 @@ int launch_label_tcgen05_ex(const c2v_dims *d, const float *cv, int B, const flo
     }
     const int H = d->encode, nkb = (H + 63) / 64;
     const long long C = d->label_count;
-    if (!ws || ws_bytes < label_tcgen05_workspace_bytes(d, B)) {
-        set_error("label workspace too small: %zu < %zu", ws_bytes, label_tcgen05_workspace_bytes(d, B));
+    const bool topk = la && la->topk_k > 0;
+    const size_t ws_need = topk ? label_topk_workspace_bytes(d, B, la->topk_k) : label_tcgen05_workspace_bytes(d, B);
+    if (!ws || ws_bytes < ws_need) {
+        set_error("label workspace too small: %zu < %zu", ws_bytes, ws_need);
         return C2V_EWORKSPACE;
     }
     g_label_last.ws = ws; g_label_last.cv = cv; g_label_last.B = B; g_label_last.dlogits = la && la->dlogits_lse;
@@ -709,13 +856,23 @@ int launch_label_tcgen05_ex(const c2v_dims *d, const float *cv, int B, const flo
     }
     const bool angular = la && la->inv_norms;
     if (angular) {
-        if (!la->label) { set_error("angular label head: label is NULL"); return C2V_EINVAL; }
-        ls.label = la->label;
+        if (!la->label && !topk) { set_error("angular label head: label is NULL"); return C2V_EINVAL; }
+        ls.label = topk ? nullptr : la->label;
         ls.icv = la->inv_norms; ls.iw = la->inv_norms + B;
         ls.cos_m = la->cos_m; ls.sin_m = la->sin_m; ls.s = la->inverse_temp;
         bias = nullptr;                                                 // the angular head has none
     }
-    auto *kern = angular ? label_gemm_v2_kernel<true> : label_gemm_v2_kernel<false>;
+    if (topk) {
+        if (!la->topk_idx || !la->topk_val || out || argmax || maxval || want_loss || la->dlogits_lse) {
+            set_error("label top-k: indices / values missing, or combined with another output");
+            return C2V_EINVAL;
+        }
+        ls.topk = reinterpret_cast<unsigned long long *>(p + align_up(label_tcgen05_workspace_bytes(d, B), 1024));
+        ls.topk_k = la->topk_k;
+        if (la->topk_prob) ls.part = part;                              // (max, sum exp) partials, no label / target
+    }
+    auto *kern = topk ? (angular ? label_gemm_v2_kernel<true, true> : label_gemm_v2_kernel<false, true>)
+                      : (angular ? label_gemm_v2_kernel<true, false> : label_gemm_v2_kernel<false, false>);
     const bool want_arg = argmax || maxval;
     const bool fused_arg = want_arg && mt <= (size_t)lt2::MAX_MT;
     int dev = 0, sms = 0;
@@ -737,13 +894,18 @@ int launch_label_tcgen05_ex(const c2v_dims *d, const float *cv, int B, const flo
 
     C2V_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, lt2::SMEM_BYTES));
     const long long n_tiles = (long long)mt * (long long)nt;
-    const int grid = (int)(n_tiles < sms ? n_tiles : sms);
+    int grid = (int)(n_tiles < sms ? n_tiles : sms);
     // tile order (see lt_range): lanes when that keeps >= 95 % of the CTAs busy, else groups; C2V_LABEL_ORDER=groups|lanes forces one
     int per_m = (mt <= (size_t)grid) ? grid / (int)mt : 0;
     if (per_m > 0 && (long long)per_m * (long long)mt * 100 < 95ll * grid) per_m = 0;
     if (const char *ord = getenv("C2V_LABEL_ORDER")) {
         if (!strcmp(ord, "groups")) per_m = 0;
         else if (!strcmp(ord, "lanes") && mt <= (size_t)grid) per_m = grid / (int)mt;
+    }
+    if (topk) {                                   // always lane order: each list then sees every column of its slice
+        if (grid > LT_TOPK_MAX_CTAS) grid = LT_TOPK_MAX_CTAS;
+        per_m = grid / (int)mt;
+        if (per_m < 1) { set_error("label top-k: %d SMs for %zu m-tiles", sms, mt); return C2V_EUNSUPPORTED; }
     }
     C2V_CUDA_OK(launch_pdl(kern, dim3((unsigned)grid), dim3(lt2::THREADS), (size_t)lt2::SMEM_BYTES, st,
                            (const uint8_t *)imgA, (const uint8_t *)imgB, bias, (const float *)hdr, out, B, C, nkb, (int)mt,
@@ -756,6 +918,16 @@ int launch_label_tcgen05_ex(const c2v_dims *d, const float *cv, int B, const flo
         C2V_LAUNCH_OK("loss_partials_reduce_kernel");
         loss_finalize_kernel<<<1, 1024, 0, st>>>(part2, LT_PSPLIT, Mpad, tgt, B, la->lse_out, la->loss);
         C2V_LAUNCH_OK("loss_finalize_kernel");
+    }
+    if (topk) {
+        if (la->topk_prob) {
+            loss_partials_reduce_kernel<<<dim3((unsigned)(Mpad / 32), LT_PSPLIT), 256, 0, st>>>(part, (int)(nt * 4), Mpad, part2);
+            C2V_LAUNCH_OK("loss_partials_reduce_kernel");
+        }
+        topk_merge_kernel<<<(unsigned)((B + 7) / 8), 256, 0, st>>>(ls.topk, la->topk_k, B, (int)mt, per_m,
+                                                                  la->topk_prob ? part2 : nullptr, Mpad, la->topk_idx,
+                                                                  la->topk_val, la->topk_prob);
+        C2V_LAUNCH_OK("topk_merge_kernel");
     }
     if (want_arg && !fused_arg) {
         if (!out) { set_error("label loss without logits: arg-max needs B <= %d", lt2::MAX_MT * 128); return C2V_EUNSUPPORTED; }

@@ -253,8 +253,9 @@ def label_dlogits(dims, params, cv, label, lse, scale, scale_device=None, algo=_
     return dout
 
 
-def _label_ws(lib, dims, B, dev, algo, cache, weight):
-    nbytes = lib.c2v_label_workspace_bytes(ctypes.byref(dims), B)
+def _label_ws(lib, dims, B, dev, algo, cache, weight, nbytes=None):
+    if nbytes is None:
+        nbytes = lib.c2v_label_workspace_bytes(ctypes.byref(dims), B)
     if cache is not None and weight is not None:
         ws, reuse = cache.get(nbytes, dev, weight)
         if reuse:
@@ -288,6 +289,42 @@ def angular_loss(dims, params, cv, label, margin, inverse_temp, want_logits=Fals
                                          _ptr(ws), ws.numel(), int(algo), _stream(dev))
         _lib.check(rc, "c2v_angular_loss_argmax")
     return loss, lse, am, mx, inv, out
+
+
+def label_topk_supported(dims, B, k):
+    return bool(_lib.load().c2v_label_topk_supported(ctypes.byref(dims), int(B), int(k)))
+
+
+def _topk(fn, dims, params, cv, k, want_probs, algo, cache, weight, *head_args):
+    lib = _lib.load()
+    _need_cuda(cv)
+    B, k = cv.shape[0], int(k)
+    dev = cv.device
+    with torch.cuda.device(dev):
+        idx = _empty((B, k), torch.int64, dev)
+        val = _empty((B, k), torch.float32, dev)
+        prob = _empty((B, k), torch.float32, dev) if want_probs else None
+        ws = None                    # a call the library will refuse must not mark the cache's weight image as current
+        if (int(algo) & 0xff) != _lib.ALGO_FFMA and label_topk_supported(dims, B, k):
+            nbytes = lib.c2v_label_topk_workspace_bytes(ctypes.byref(dims), B, k)
+            ws, algo = _label_ws(lib, dims, B, dev, algo, cache, weight, nbytes=nbytes)
+        cv = _f32c(cv, "code_vector")
+        rc = getattr(lib, fn)(ctypes.byref(dims), ctypes.byref(params), _ptr(cv), B, k, *head_args, _ptr(idx), _ptr(val),
+                              _ptr(prob), _ptr(ws), ws.numel() if ws is not None else 0, int(algo), _stream(dev))
+        _lib.check(rc, fn)
+    return idx, val, prob
+
+
+def label_topk(dims, params, cv, k, want_probs=True, algo=_lib.ALGO_AUTO, cache=None, weight=None):
+    """the k largest logits of model.py:83 per row, ranked as torch.sort(descending=True, stable=True) ranks them, from
+    the label GEMM's epilogue (the [B, C] logits are never written) -> (indices int64 [B, k], values [B, k],
+    softmax probabilities [B, k] or None).  B <= 2048 and k <= _lib.TOPK_MAX (label_topk_supported)."""
+    return _topk("c2v_label_topk", dims, params, cv, k, want_probs, algo, cache, weight)
+
+
+def angular_topk(dims, params, cv, k, inverse_temp, want_probs=True, algo=_lib.ALGO_AUTO, cache=None, weight=None):
+    """label_topk for the angular head (model.py:71-80) without its margin: logits inverse_temp * cos(cv, W_c), no label"""
+    return _topk("c2v_angular_topk", dims, params, cv, k, want_probs, algo, cache, weight, ctypes.c_float(inverse_temp))
 
 
 def angular_dlogits(dims, params, cv, label, lse, inv_norms, margin, inverse_temp, scale, scale_device=None,

@@ -333,3 +333,51 @@ class Code2Vec(nn.Module):
                                            _lib.ALGO_FFMA if self.algo == _lib.ALGO_FFMA else _lib.ALGO_AUTO,
                                            cache=self._lab_cache, weight=self.output_linear.weight, want_logits=False)
         return am, mx, code_vector, attention
+
+    _TOPK_ROWS = 2048                   # rows per fused top-k call (c2v_label_topk_supported)
+
+    @torch.no_grad()
+    def predict_topk(self, starts, paths, ends, k=10, probs=True):
+        """-> (pred_labels int64 [b, k], pred_scores [b, k], pred_probs [b, k] or None, code_vector [b,H], attention [b,L]):
+        the k best labels of every method, best first, ranked as torch.sort(logits, 1, descending=True, stable=True) ranks
+        them (equal scores: the lower label index first; k=1 is predict()), their scores and, with probs=True, their softmax
+        probabilities.  Plain head: the logits of forward().  Angular-margin head: inverse_temp * cos(code_vector, W_c),
+        without the margin, so no label is needed (predict_topk(k=1) is that head's prediction).
+        The label GEMM keeps a running top-k in its epilogue and never writes the [b, C] logits (b is cut into chunks of
+        2048 rows).  k > _lib.TOPK_MAX, encode sizes the fused kernel does not take and algo="ffma" materialise the
+        logits and sort them instead."""
+        k = int(k)
+        C = self.option.label_count
+        if not 1 <= k <= C:
+            raise ValueError(f"predict_topk: k = {k} is outside [1, label_count = {C}]")
+        self._enc_cache.raise_deferred()
+        dims = self._dims()
+        angular = self.option.angular_margin_loss
+        w_out = self.output_linear if angular else self.output_linear.weight
+        params = CF.make_params(self.terminal_embedding.weight, self.path_embedding.weight, self.input_linear.weight,
+                                self.input_layer_norm.weight, self.input_layer_norm.bias, self.attention_parameter,
+                                w_out, None if angular else self.output_linear.bias)
+        code_vector, attention = CF.encode_forward(dims, params, starts, paths, ends, algo=self.algo,
+                                                   cache=self._enc_cache, weight=self.input_linear.weight)
+        b = code_vector.shape[0]
+        if self.algo != _lib.ALGO_FFMA and CF.label_topk_supported(dims, min(b, self._TOPK_ROWS), k):
+            parts = []
+            for i in range(0, b, self._TOPK_ROWS):
+                cv = code_vector[i:i + self._TOPK_ROWS]
+                if angular:
+                    parts.append(CF.angular_topk(dims, params, cv, k, self.option.inverse_temp, want_probs=probs,
+                                                 cache=self._lab_cache, weight=w_out))
+                else:
+                    parts.append(CF.label_topk(dims, params, cv, k, want_probs=probs, cache=self._lab_cache, weight=w_out))
+            idx, val, prob = (torch.cat(t) if t[0] is not None else None for t in zip(*parts))
+            return idx, val, prob, code_vector, attention
+        if angular:
+            logits = self.option.inverse_temp * F.linear(F.normalize(code_vector), F.normalize(w_out))
+        else:
+            logits = CF.label_logits(dims, params, code_vector,
+                                     _lib.ALGO_FFMA if self.algo == _lib.ALGO_FFMA else _lib.ALGO_AUTO,
+                                     cache=self._lab_cache, weight=w_out)
+        val, idx = torch.sort(logits, dim=1, descending=True, stable=True)
+        val, idx = val[:, :k].contiguous(), idx[:, :k].contiguous()
+        prob = torch.softmax(logits, dim=1).gather(1, idx) if probs else None
+        return idx, val, prob, code_vector, attention

@@ -237,6 +237,27 @@ int c2v_angular_logits(const c2v_dims *d, const c2v_params *p, const float *code
                        const int64_t *label, int32_t B, float margin, float inverse_temp,
                        float *outputs, void *stream);
 
+/* Top-k prediction fused into the tensor-core label GEMM: the k largest logits of every row, ranked as
+ * torch.sort(logits, 1, descending=True, stable=True) ranks them (value descending, equal values by column ascending; k = 1
+ * is torch.max(dim=1)).  The [B, C] logits are never written.
+ *   indices int64 [B, k], values fp32 [B, k] (the logits at those columns), probs fp32 [B, k] or NULL (their softmax
+ *   probabilities, exp(value - logsumexp of the row)).
+ * c2v_label_topk: logits cv . W_out^T + b (model.py:83), the same numbers c2v_label_logits writes on the tensor cores.
+ * c2v_angular_topk: the angular head's logits without the margin, inverse_temp * cos(cv_b, W_c): no label is needed, and
+ * output_bias is not read.  This is how an unlabelled method is ranked under the angular-margin head.
+ * 1 <= k <= min(C2V_TOPK_MAX, label_count); c2v_label_topk_supported: additionally encode_size % 4 == 0, <= 256, B <= 2048.
+ * workspace: c2v_label_topk_workspace_bytes (at least c2v_label_workspace_bytes; the W_out image sits where the other label
+ * calls keep it, so C2V_FLAG_REUSE_PREP carries over between them).  algo: AUTO or TCGEN05 (FFMA is C2V_EUNSUPPORTED). */
+#define C2V_TOPK_MAX 16
+int c2v_label_topk_supported(const c2v_dims *d, int32_t B, int32_t k);
+size_t c2v_label_topk_workspace_bytes(const c2v_dims *d, int32_t B, int32_t k);
+int c2v_label_topk(const c2v_dims *d, const c2v_params *p, const float *code_vector, int32_t B, int32_t k,
+                   int64_t *indices, float *values, float *probs, void *workspace, size_t workspace_bytes, int32_t algo,
+                   void *stream);
+int c2v_angular_topk(const c2v_dims *d, const c2v_params *p, const float *code_vector, int32_t B, int32_t k,
+                     float inverse_temp, int64_t *indices, float *values, float *probs, void *workspace,
+                     size_t workspace_bytes, int32_t algo, void *stream);
+
 /* ---- loss / predict next to the path ----------------------------------------------
  * main.py:251-264: mean over the batch of -log_softmax(outputs)[label] (NLLLoss
  * weights are identically 1); main.py:285: torch.max(dim=1).
