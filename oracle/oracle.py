@@ -165,7 +165,14 @@ def num_threads():
 # bench.py times as the CPU baseline (kind="port"): the C file above is the
 # arithmetic checker, this is the fastest faithful CPU path (MKL sgemm, oneDNN LN).
 # --------------------------------------------------------------------------------------
-def torch_forward(p, starts, paths, ends, label=None, angular=None, drop_p=0.0, training=False):
+def torch_forward(p, starts, paths, ends, label=None, angular=None, drop_p=0.0, training=False, dropmask=None,
+                  taps=None):
+    """-> (outputs, code_vector, attention) in the dtype and on the device of `p`.
+    dropmask: a given multiplicative mask [B, L, encode] applied to the tanh output instead of a random F.dropout (what
+    `forward(..., dropmask=)` does), e.g. the kernels' Philox mask rebuilt by tests/philox_ref.py.
+    taps: a dict that receives the intermediates "x" (input_linear output, before the LayerNorm), "ln" (LayerNorm
+    output), "z" (masked attention scores), "cv", "logits" and, angular head only, "cos", so that a caller can
+    retain_grad() them and read the gradient at every stage."""
     import math
     import torch
     import torch.nn.functional as F
@@ -174,11 +181,17 @@ def torch_forward(p, starts, paths, ends, label=None, angular=None, drop_p=0.0, 
     ee = F.embedding(ends, p["terminal_embedding.weight"])              # model.py:50
     c = torch.cat((es, ep, ee), dim=2)                                  # model.py:51
     x = F.linear(c, p["input_linear.weight"])                           # model.py:54
+    if taps is not None:
+        taps["x"] = x
     H = x.shape[-1]
     x = F.layer_norm(x.view(-1, H), (H,), p["input_layer_norm.weight"],
                      p["input_layer_norm.bias"], 1e-5).view(x.shape)    # model.py:55-56
+    if taps is not None:
+        taps["ln"] = x
     h = torch.tanh(x)                                                   # model.py:57
-    if training and 0.0 < drop_p < 1.0:
+    if dropmask is not None:
+        h = h * dropmask                                                # model.py:60-61 with a given mask
+    elif training and 0.0 < drop_p < 1.0:
         h = F.dropout(h, drop_p, True)                                  # model.py:60-61
     mask = (starts > 0).float()                                         # model.py:64
     z = (h * p["attention_parameter"]).sum(2) * mask + (1 - mask) * (-3.4e38)   # model.py:92-93
@@ -193,4 +206,8 @@ def torch_forward(p, starts, paths, ends, label=None, angular=None, drop_p=0.0, 
         out = (oh * phi + (1.0 - oh) * cos) * angular["inverse_temp"]
     else:
         out = F.linear(cv, p["output_linear.weight"], p["output_linear.bias"])  # model.py:83
+    if taps is not None:
+        taps.update(z=z, cv=cv, logits=out)
+        if angular is not None:
+            taps["cos"] = cos
     return out, cv, att
