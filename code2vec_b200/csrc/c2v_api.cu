@@ -321,6 +321,28 @@ size_t c2v_label_workspace_bytes(const c2v_dims *d, int32_t B)
     return align_up(label_tcgen05_workspace_bytes(d, B), 1024);
 }
 
+// What every tensor-core label entry point does once its own argument checks have passed: apply the flags of `algo`
+// (C2V_FLAG_REUSE_PREP, C2V_FLAG_NO_PDL) and launch the label GEMM in the mode `la` selects (NULL: the logits, with the
+// fused arg-max when argmax / maxval are given).  The angular head ignores output_bias.
+static int label_gemm(const c2v_dims *d, const c2v_params *p, const float *code_vector, int32_t B, float *out,
+                      int64_t *argmax, float *maxval, void *workspace, size_t workspace_bytes, int32_t algo, void *stream,
+                      const LabelLossArgs *la)
+{
+    g_pdl_this_call = (algo & C2V_FLAG_NO_PDL) == 0;
+    return launch_label_tcgen05_ex(d, code_vector, B, p->output_weight, p->output_bias, out,
+                                   reinterpret_cast<long long *>(argmax), maxval, workspace, workspace_bytes,
+                                   (algo & C2V_FLAG_REUSE_PREP) != 0, static_cast<cudaStream_t>(stream), la);
+}
+
+// the angular head's inverse row norms: inv[0, B) of the code vectors, then inv[B, B + C) of the W_out rows
+static int angular_inv_norms(const c2v_dims *d, const c2v_params *p, const float *code_vector, int32_t B, float *inv,
+                             void *stream)
+{
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int rc = launch_row_inv_norm(code_vector, B, d->encode, inv, st);
+    return rc != C2V_OK ? rc : launch_row_inv_norm(p->output_weight, d->label_count, d->encode, inv + B, st);
+}
+
 int c2v_label_logits(const c2v_dims *d, const c2v_params *p, const float *code_vector, int32_t B,
                      float *outputs, void *workspace, size_t workspace_bytes, int32_t algo,
                      void *stream)
@@ -330,19 +352,7 @@ int c2v_label_logits(const c2v_dims *d, const c2v_params *p, const float *code_v
         set_error("c2v_label_logits: bad argument");
         return C2V_EINVAL;
     }
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int H = d->encode;
-    const long long C = d->label_count;
-    const bool reuse_prep = (algo & C2V_FLAG_REUSE_PREP) != 0;
-    g_pdl_this_call = (algo & C2V_FLAG_NO_PDL) == 0;
-    algo &= 0xff;
-    if (algo == C2V_ALGO_TCGEN05 || (algo == C2V_ALGO_AUTO && label_tcgen05_shape_ok(d))) {
-        return launch_label_tcgen05(d, code_vector, B, p->output_weight, p->output_bias, outputs, nullptr,
-                                    nullptr, workspace, workspace_bytes, reuse_prep, st);
-    }
-    // outputs[b,c] = sum_h cv[b,h] * W_out[c,h] + bias[c]   (model.py:83)
-    return launch_sgemm(B, (int)C, H, code_vector, H, 1, p->output_weight, 1, H, p->output_bias,
-                        outputs, C, false, st);
+    return c2v_label_logits_argmax(d, p, code_vector, B, outputs, nullptr, nullptr, workspace, workspace_bytes, algo, stream);
 }
 
 int c2v_label_logits_argmax(const c2v_dims *d, const c2v_params *p, const float *code_vector, int32_t B,
@@ -358,18 +368,20 @@ int c2v_label_logits_argmax(const c2v_dims *d, const c2v_params *p, const float 
         set_error("c2v_label_logits_argmax: outputs == NULL needs encode_size %% 4 == 0, <= 256 and B <= 2048");
         return C2V_EUNSUPPORTED;
     }
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const bool reuse_prep = (algo & C2V_FLAG_REUSE_PREP) != 0;
-    g_pdl_this_call = (algo & C2V_FLAG_NO_PDL) == 0;
     const int base_algo = algo & 0xff;
     if (base_algo == C2V_ALGO_TCGEN05 || (base_algo == C2V_ALGO_AUTO && label_tcgen05_shape_ok(d)))
-        return launch_label_tcgen05(d, code_vector, B, p->output_weight, p->output_bias, outputs,
-                                    reinterpret_cast<long long *>(argmax), maxval, workspace, workspace_bytes,
-                                    reuse_prep, st);
-    int rc = c2v_label_logits(d, p, code_vector, B, outputs, workspace, workspace_bytes, algo, stream);
+        return label_gemm(d, p, code_vector, B, outputs, argmax, maxval, workspace, workspace_bytes, algo, stream, nullptr);
+    if (!outputs) {
+        set_error("c2v_label_logits_argmax: outputs == NULL needs the tensor-core label GEMM (got algo %d)", base_algo);
+        return C2V_EINVAL;
+    }
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int H = d->encode;
+    const long long C = d->label_count;
+    // outputs[b,c] = sum_h cv[b,h] * W_out[c,h] + bias[c]   (model.py:83)
+    int rc = launch_sgemm(B, (int)C, H, code_vector, H, 1, p->output_weight, 1, H, p->output_bias, outputs, C, false, st);
     if (rc != C2V_OK || (!argmax && !maxval)) return rc;
-    return launch_loss_argmax(outputs, nullptr, B, d->label_count, nullptr,
-                              reinterpret_cast<long long *>(argmax), maxval, nullptr, st);
+    return launch_loss_argmax(outputs, nullptr, B, C, nullptr, reinterpret_cast<long long *>(argmax), maxval, nullptr, st);
 }
 
 int c2v_label_loss_supported(const c2v_dims *d, int32_t B)
@@ -392,14 +404,9 @@ int c2v_label_loss_argmax(const c2v_dims *d, const c2v_params *p, const float *c
                   "c2v_label_logits + c2v_loss_argmax", d->encode, B);
         return C2V_EUNSUPPORTED;
     }
-    const bool reuse_prep = (algo & C2V_FLAG_REUSE_PREP) != 0;
-    g_pdl_this_call = (algo & C2V_FLAG_NO_PDL) == 0;
-    LabelLossArgs la;
-    memset(&la, 0, sizeof(la));
+    LabelLossArgs la = {};
     la.label = reinterpret_cast<const long long *>(label); la.loss = loss; la.lse_out = lse;
-    return launch_label_tcgen05_ex(d, code_vector, B, p->output_weight, p->output_bias, outputs,
-                                   reinterpret_cast<long long *>(argmax), maxval, workspace, workspace_bytes, reuse_prep,
-                                   static_cast<cudaStream_t>(stream), &la);
+    return label_gemm(d, p, code_vector, B, outputs, argmax, maxval, workspace, workspace_bytes, algo, stream, &la);
 }
 
 int c2v_label_dlogits(const c2v_dims *d, const c2v_params *p, const float *code_vector, const int64_t *label,
@@ -415,13 +422,10 @@ int c2v_label_dlogits(const c2v_dims *d, const c2v_params *p, const float *code_
         set_error("c2v_label_dlogits: needs encode_size %% 4 == 0 and <= 256 (got %d)", d->encode);
         return C2V_EUNSUPPORTED;
     }
-    const bool reuse_prep = (algo & C2V_FLAG_REUSE_PREP) != 0;
-    g_pdl_this_call = false;
-    LabelLossArgs la;
-    memset(&la, 0, sizeof(la));
+    LabelLossArgs la = {};
     la.label = reinterpret_cast<const long long *>(label); la.dlogits_lse = lse; la.dscale = scale; la.dscale_ptr = scale_device;
-    return launch_label_tcgen05_ex(d, code_vector, B, p->output_weight, p->output_bias, d_outputs, nullptr, nullptr,
-                                   workspace, workspace_bytes, reuse_prep, static_cast<cudaStream_t>(stream), &la);
+    return label_gemm(d, p, code_vector, B, d_outputs, nullptr, nullptr, workspace, workspace_bytes, algo | C2V_FLAG_NO_PDL,
+                      stream, &la);
 }
 
 int c2v_angular_loss_argmax(const c2v_dims *d, const c2v_params *p, const float *code_vector, const int64_t *label,
@@ -439,18 +443,12 @@ int c2v_angular_loss_argmax(const c2v_dims *d, const c2v_params *p, const float 
                   "c2v_angular_forward_train + c2v_loss_argmax", d->encode, B);
         return C2V_EUNSUPPORTED;
     }
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const bool reuse_prep = (algo & C2V_FLAG_REUSE_PREP) != 0;
-    g_pdl_this_call = (algo & C2V_FLAG_NO_PDL) == 0;
-    int rc = launch_row_inv_norm(code_vector, B, d->encode, inv_norms, st);
-    if (rc == C2V_OK) rc = launch_row_inv_norm(p->output_weight, d->label_count, d->encode, inv_norms + B, st);
+    const int rc = angular_inv_norms(d, p, code_vector, B, inv_norms, stream);
     if (rc != C2V_OK) return rc;
-    LabelLossArgs la;
-    memset(&la, 0, sizeof(la));
+    LabelLossArgs la = {};
     la.label = reinterpret_cast<const long long *>(label); la.loss = loss; la.lse_out = lse;
     la.inv_norms = inv_norms; la.cos_m = cosf(margin); la.sin_m = sinf(margin); la.inverse_temp = inverse_temp;
-    return launch_label_tcgen05_ex(d, code_vector, B, p->output_weight, nullptr, outputs, reinterpret_cast<long long *>(argmax),
-                                   maxval, workspace, workspace_bytes, reuse_prep, st, &la);
+    return label_gemm(d, p, code_vector, B, outputs, argmax, maxval, workspace, workspace_bytes, algo, stream, &la);
 }
 
 int c2v_angular_dlogits(const c2v_dims *d, const c2v_params *p, const float *code_vector, const int64_t *label,
@@ -467,14 +465,11 @@ int c2v_angular_dlogits(const c2v_dims *d, const c2v_params *p, const float *cod
         set_error("c2v_angular_dlogits: needs encode_size %% 4 == 0 and <= 256 (got %d)", d->encode);
         return C2V_EUNSUPPORTED;
     }
-    const bool reuse_prep = (algo & C2V_FLAG_REUSE_PREP) != 0;
-    g_pdl_this_call = false;
-    LabelLossArgs la;
-    memset(&la, 0, sizeof(la));
+    LabelLossArgs la = {};
     la.label = reinterpret_cast<const long long *>(label); la.dlogits_lse = lse; la.dscale = scale; la.dscale_ptr = scale_device;
     la.inv_norms = inv_norms; la.cos_m = cosf(margin); la.sin_m = sinf(margin); la.inverse_temp = inverse_temp;
-    return launch_label_tcgen05_ex(d, code_vector, B, p->output_weight, nullptr, d_dot, nullptr, nullptr, workspace,
-                                   workspace_bytes, reuse_prep, static_cast<cudaStream_t>(stream), &la);
+    return label_gemm(d, p, code_vector, B, d_dot, nullptr, nullptr, workspace, workspace_bytes, algo | C2V_FLAG_NO_PDL, stream,
+                      &la);
 }
 
 int c2v_angular_backward_ws(const c2v_dims *d, const c2v_params *p, const float *code_vector, const float *d_dot,
@@ -567,13 +562,9 @@ int c2v_label_topk(const c2v_dims *d, const c2v_params *p, const float *code_vec
 {
     const int rc = topk_args_ok("c2v_label_topk", d, p, code_vector, B, k, indices, values, workspace, workspace_bytes, algo);
     if (rc != C2V_OK) return rc;
-    const bool reuse_prep = (algo & C2V_FLAG_REUSE_PREP) != 0;
-    g_pdl_this_call = (algo & C2V_FLAG_NO_PDL) == 0;
-    LabelLossArgs la;
-    memset(&la, 0, sizeof(la));
+    LabelLossArgs la = {};
     la.topk_k = k; la.topk_idx = reinterpret_cast<long long *>(indices); la.topk_val = values; la.topk_prob = probs;
-    return launch_label_tcgen05_ex(d, code_vector, B, p->output_weight, p->output_bias, nullptr, nullptr, nullptr, workspace,
-                                   workspace_bytes, reuse_prep, static_cast<cudaStream_t>(stream), &la);
+    return label_gemm(d, p, code_vector, B, nullptr, nullptr, nullptr, workspace, workspace_bytes, algo, stream, &la);
 }
 
 int c2v_angular_topk(const c2v_dims *d, const c2v_params *p, const float *code_vector, int32_t B, int32_t k,
@@ -582,19 +573,13 @@ int c2v_angular_topk(const c2v_dims *d, const c2v_params *p, const float *code_v
 {
     int rc = topk_args_ok("c2v_angular_topk", d, p, code_vector, B, k, indices, values, workspace, workspace_bytes, algo);
     if (rc != C2V_OK) return rc;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const bool reuse_prep = (algo & C2V_FLAG_REUSE_PREP) != 0;
-    g_pdl_this_call = (algo & C2V_FLAG_NO_PDL) == 0;
     float *inv = label_topk_inv_norms(d, B, k, workspace);
-    rc = launch_row_inv_norm(code_vector, B, d->encode, inv, st);
-    if (rc == C2V_OK) rc = launch_row_inv_norm(p->output_weight, d->label_count, d->encode, inv + B, st);
+    rc = angular_inv_norms(d, p, code_vector, B, inv, stream);
     if (rc != C2V_OK) return rc;
-    LabelLossArgs la;
-    memset(&la, 0, sizeof(la));
+    LabelLossArgs la = {};
     la.inv_norms = inv; la.inverse_temp = inverse_temp;
     la.topk_k = k; la.topk_idx = reinterpret_cast<long long *>(indices); la.topk_val = values; la.topk_prob = probs;
-    return launch_label_tcgen05_ex(d, code_vector, B, p->output_weight, nullptr, nullptr, nullptr, nullptr, workspace,
-                                   workspace_bytes, reuse_prep, st, &la);
+    return label_gemm(d, p, code_vector, B, nullptr, nullptr, nullptr, workspace, workspace_bytes, algo, stream, &la);
 }
 
 int c2v_angular_forward_train(const c2v_dims *d, const c2v_params *p, const float *code_vector, const int64_t *label,
@@ -672,9 +657,8 @@ int c2v_label_backward_ws(const c2v_dims *d, const c2v_params *p, const float *c
         return C2V_EINVAL;
     }
     const int base_algo = algo & 0xff;
-    const char *env = getenv("C2V_LABEL_BACKWARD");
     const bool tc = base_algo != C2V_ALGO_FFMA && workspace != nullptr && label_backward_tc_ok(d) &&
-                    (d_output_weight != nullptr || d_output_bias == nullptr) && !(env && !strcmp(env, "ffma"));
+                    (d_output_weight != nullptr || d_output_bias == nullptr);
     if (!tc) {
         if (base_algo == C2V_ALGO_TCGEN05) {
             set_error("tensor-core label backward needs a label workspace, encode_size %% 4 == 0 and <= 256");

@@ -140,9 +140,6 @@ float *label_topk_inv_norms(const c2v_dims *d, int B, int k, void *ws);     // w
 int launch_label_tcgen05_ex(const c2v_dims *d, const float *cv, int B, const float *Wout, const float *bias,
                             float *out, long long *argmax, float *maxval, void *ws, size_t ws_bytes, bool reuse_prep,
                             cudaStream_t st, const LabelLossArgs *la);
-int launch_label_tcgen05(const c2v_dims *d, const float *cv, int B, const float *Wout,
-                         const float *bias, float *out, long long *argmax, float *maxval, void *ws,
-                         size_t ws_bytes, bool reuse_prep, cudaStream_t st);
 
 // ---------------------------------------------------------------------------------
 // device helpers

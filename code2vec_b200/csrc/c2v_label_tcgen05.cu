@@ -785,13 +785,6 @@ int label_w_image(const c2v_dims *d, const float *Wout, int B, void *ws, size_t 
     return C2V_OK;
 }
 
-int launch_label_tcgen05(const c2v_dims *d, const float *cv, int B, const float *Wout, const float *bias,
-                         float *out, long long *argmax, float *maxval, void *ws, size_t ws_bytes, bool reuse_prep,
-                         cudaStream_t st)
-{
-    return launch_label_tcgen05_ex(d, cv, B, Wout, bias, out, argmax, maxval, ws, ws_bytes, reuse_prep, st, nullptr);
-}
-
 // What the last label GEMM launched from this host thread left in its workspace: the fp16 image of `cv` (every call) and, in
 // dlogits mode, max |d logit|.  c2v_label_backward_ws only believes C2V_FLAG_GRAD_ABSMAX_READY when this record matches its
 // own workspace / code_vector / B -- a wrong flag then costs the skipped shortcuts, not the result.

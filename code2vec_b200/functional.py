@@ -58,7 +58,7 @@ def make_dims(T, P, C, Et, Ep, H):
     return Dims(int(T), int(P), int(C), int(Et), int(Ep), int(H), 0)
 
 
-def make_params(emb_t, emb_p, W, ln_g, ln_b, attn, w_out=None, b_out=None):
+def make_params(emb_t=None, emb_p=None, W=None, ln_g=None, ln_b=None, attn=None, w_out=None, b_out=None):
     for t in (emb_t, emb_p, W, ln_g, ln_b, attn, w_out, b_out):
         if t is not None and (t.dtype != torch.float32 or not t.is_contiguous()):
             raise TypeError("parameters must be contiguous fp32")
@@ -149,6 +149,18 @@ def encode_forward(dims, params, starts, paths, ends, drop_p=0.0, training=False
     return cv, att
 
 
+def _label_ws(dims, B, dev, algo, cache, weight, nbytes=None, absmax_ready=False, fresh=True):
+    """-> (workspace, algo with its flags) of a label-head call.  With a cache (and its weight, W_out) the cache's persistent
+    workspace, plus REUSE_PREP while its W_out image is current and GRAD_ABSMAX_READY if absmax_ready.  Without one a fresh
+    workspace, or None if not fresh (the backward calls then run on the CUDA cores)."""
+    if nbytes is None:
+        nbytes = _lib.load().c2v_label_workspace_bytes(ctypes.byref(dims), B)
+    if cache is not None and weight is not None:
+        ws, reuse = cache.get(nbytes, dev, weight)
+        return ws, int(algo) | (REUSE_PREP if reuse else 0) | (GRAD_ABSMAX_READY if absmax_ready else 0)
+    return (_empty((nbytes,), torch.uint8, dev) if fresh else None), int(algo)
+
+
 def label_logits(dims, params, cv, algo=_lib.ALGO_AUTO, cache=None, weight=None):
     """model.py:83"""
     lib = _lib.load()
@@ -157,13 +169,7 @@ def label_logits(dims, params, cv, algo=_lib.ALGO_AUTO, cache=None, weight=None)
     dev = cv.device
     with torch.cuda.device(dev):
         out = _empty((B, dims.label_count), torch.float32, dev)
-        nbytes = lib.c2v_label_workspace_bytes(ctypes.byref(dims), B)
-        if cache is not None and weight is not None:
-            ws, reuse = cache.get(nbytes, dev, weight)
-            if reuse:
-                algo = int(algo) | REUSE_PREP
-        else:
-            ws = _empty((nbytes,), torch.uint8, dev)
+        ws, algo = _label_ws(dims, B, dev, algo, cache, weight)
         cv = _f32c(cv, "code_vector")          # bound to a local: the pointer must outlive the launch
         rc = lib.c2v_label_logits(ctypes.byref(dims), ctypes.byref(params), _ptr(cv), B, _ptr(out),
                                   _ptr(ws), ws.numel(), int(algo), _stream(dev))
@@ -183,13 +189,7 @@ def label_logits_argmax(dims, params, cv, algo=_lib.ALGO_AUTO, cache=None, weigh
         out = _empty((B, dims.label_count), torch.float32, dev) if want_logits else None
         am = _empty((B,), torch.int64, dev)
         mx = _empty((B,), torch.float32, dev)
-        nbytes = lib.c2v_label_workspace_bytes(ctypes.byref(dims), B)
-        if cache is not None and weight is not None:
-            ws, reuse = cache.get(nbytes, dev, weight)
-            if reuse:
-                algo = int(algo) | REUSE_PREP
-        else:
-            ws = _empty((nbytes,), torch.uint8, dev)
+        ws, algo = _label_ws(dims, B, dev, algo, cache, weight)
         cv = _f32c(cv, "code_vector")
         rc = lib.c2v_label_logits_argmax(ctypes.byref(dims), ctypes.byref(params), _ptr(cv), B, _ptr(out),
                                          _ptr(am), _ptr(mx), _ptr(ws), ws.numel(), int(algo), _stream(dev))
@@ -216,13 +216,7 @@ def label_loss(dims, params, cv, label, want_logits=False, algo=_lib.ALGO_AUTO, 
         lse = _empty((B,), torch.float32, dev)
         am = _empty((B,), torch.int64, dev)
         mx = _empty((B,), torch.float32, dev)
-        nbytes = lib.c2v_label_workspace_bytes(ctypes.byref(dims), B)
-        if cache is not None and weight is not None:
-            ws, reuse = cache.get(nbytes, dev, weight)
-            if reuse:
-                algo = int(algo) | REUSE_PREP
-        else:
-            ws = _empty((nbytes,), torch.uint8, dev)
+        ws, algo = _label_ws(dims, B, dev, algo, cache, weight)
         cv = _f32c(cv, "code_vector")
         rc = lib.c2v_label_loss_argmax(ctypes.byref(dims), ctypes.byref(params), _ptr(cv), _ptr(label), B, _ptr(out),
                                        _ptr(loss), _ptr(lse), _ptr(am), _ptr(mx), _ptr(ws), ws.numel(), int(algo),
@@ -238,31 +232,13 @@ def label_dlogits(dims, params, cv, label, lse, scale, scale_device=None, algo=_
     dev = cv.device
     with torch.cuda.device(dev):
         dout = _empty((B, dims.label_count), torch.float32, dev)
-        nbytes = lib.c2v_label_workspace_bytes(ctypes.byref(dims), B)
-        if cache is not None and weight is not None:
-            ws, reuse = cache.get(nbytes, dev, weight)
-            if reuse:
-                algo = int(algo) | REUSE_PREP
-        else:
-            ws = _empty((nbytes,), torch.uint8, dev)
+        ws, algo = _label_ws(dims, B, dev, algo, cache, weight)
         cv = _f32c(cv, "code_vector"); lse = _f32c(lse, "lse")
         sd = _f32c(scale_device, "scale_device") if scale_device is not None else None
         rc = lib.c2v_label_dlogits(ctypes.byref(dims), ctypes.byref(params), _ptr(cv), _ptr(label), _ptr(lse), B,
                                    float(scale), _ptr(sd), _ptr(dout), _ptr(ws), ws.numel(), int(algo), _stream(dev))
         _lib.check(rc, "c2v_label_dlogits")
     return dout
-
-
-def _label_ws(lib, dims, B, dev, algo, cache, weight, nbytes=None):
-    if nbytes is None:
-        nbytes = lib.c2v_label_workspace_bytes(ctypes.byref(dims), B)
-    if cache is not None and weight is not None:
-        ws, reuse = cache.get(nbytes, dev, weight)
-        if reuse:
-            algo = int(algo) | REUSE_PREP
-    else:
-        ws = _empty((nbytes,), torch.uint8, dev)
-    return ws, algo
 
 
 def angular_loss(dims, params, cv, label, margin, inverse_temp, want_logits=False, algo=_lib.ALGO_AUTO, cache=None,
@@ -282,7 +258,7 @@ def angular_loss(dims, params, cv, label, margin, inverse_temp, want_logits=Fals
         am = _empty((B,), torch.int64, dev)
         mx = _empty((B,), torch.float32, dev)
         inv = _empty((B + dims.label_count,), torch.float32, dev)
-        ws, algo = _label_ws(lib, dims, B, dev, algo, cache, weight)
+        ws, algo = _label_ws(dims, B, dev, algo, cache, weight)
         cv = _f32c(cv, "code_vector")
         rc = lib.c2v_angular_loss_argmax(ctypes.byref(dims), ctypes.byref(params), _ptr(cv), _ptr(label), B, float(margin),
                                          float(inverse_temp), _ptr(out), _ptr(loss), _ptr(lse), _ptr(am), _ptr(mx), _ptr(inv),
@@ -307,7 +283,7 @@ def _topk(fn, dims, params, cv, k, want_probs, algo, cache, weight, *head_args):
         ws = None                    # a call the library will refuse must not mark the cache's weight image as current
         if (int(algo) & 0xff) != _lib.ALGO_FFMA and label_topk_supported(dims, B, k):
             nbytes = lib.c2v_label_topk_workspace_bytes(ctypes.byref(dims), B, k)
-            ws, algo = _label_ws(lib, dims, B, dev, algo, cache, weight, nbytes=nbytes)
+            ws, algo = _label_ws(dims, B, dev, algo, cache, weight, nbytes=nbytes)
         cv = _f32c(cv, "code_vector")
         rc = getattr(lib, fn)(ctypes.byref(dims), ctypes.byref(params), _ptr(cv), B, k, *head_args, _ptr(idx), _ptr(val),
                               _ptr(prob), _ptr(ws), ws.numel() if ws is not None else 0, int(algo), _stream(dev))
@@ -337,7 +313,7 @@ def angular_dlogits(dims, params, cv, label, lse, inv_norms, margin, inverse_tem
     label = _idx(label, "label", (B,))
     with torch.cuda.device(dev):
         g = _empty((B, dims.label_count), torch.float32, dev)
-        ws, algo = _label_ws(lib, dims, B, dev, algo, cache, weight)
+        ws, algo = _label_ws(dims, B, dev, algo, cache, weight)
         cv = _f32c(cv, "code_vector"); lse = _f32c(lse, "lse"); inv = _f32c(inv_norms, "inv_norms")
         sd = _f32c(scale_device, "scale_device") if scale_device is not None else None
         rc = lib.c2v_angular_dlogits(ctypes.byref(dims), ctypes.byref(params), _ptr(cv), _ptr(label), _ptr(lse), _ptr(inv), B,
@@ -359,12 +335,7 @@ def angular_backward_ws(dims, params, cv, d_dot, inv_norms, need_cv=True, need_w
         d_cv = torch.empty_like(cv) if need_cv else None
         d_w = _empty((dims.label_count, dims.encode), torch.float32, dev) if need_w else None
         cv = _f32c(cv, "code_vector"); d_dot = _f32c(d_dot, "d_dot"); inv = _f32c(inv_norms, "inv_norms")
-        if cache is not None and weight is not None:
-            nbytes = lib.c2v_label_workspace_bytes(ctypes.byref(dims), B)
-            ws, reuse = cache.get(nbytes, dev, weight)
-            flags = int(algo) | (REUSE_PREP if reuse else 0) | (GRAD_ABSMAX_READY if absmax_ready else 0)
-        else:
-            ws, flags = None, int(algo)
+        ws, flags = _label_ws(dims, B, dev, algo, cache, weight, absmax_ready=absmax_ready, fresh=False)
         rc = lib.c2v_angular_backward_ws(ctypes.byref(dims), ctypes.byref(params), _ptr(cv), _ptr(d_dot), _ptr(inv), B,
                                          _ptr(d_cv), _ptr(d_w), _ptr(ws), ws.numel() if ws is not None else 0, flags,
                                          _stream(dev))
@@ -457,10 +428,8 @@ def label_backward(dims, params, cv, d_out, need_cv=True, need_w=True, need_b=Tr
         d_w = _empty((dims.label_count, dims.encode), torch.float32, dev) if (need_w or need_b) else None
         d_b = _empty((dims.label_count,), torch.float32, dev) if need_b else None
         cv = _f32c(cv, "code_vector"); d_out = _f32c(d_out, "d_outputs")
-        if cache is not None and weight is not None:
-            nbytes = lib.c2v_label_workspace_bytes(ctypes.byref(dims), B)
-            ws, reuse = cache.get(nbytes, dev, weight)
-            flags = int(algo) | (REUSE_PREP if reuse else 0) | (GRAD_ABSMAX_READY if absmax_ready else 0)
+        ws, flags = _label_ws(dims, B, dev, algo, cache, weight, absmax_ready=absmax_ready, fresh=False)
+        if ws is not None:
             rc = lib.c2v_label_backward_ws(ctypes.byref(dims), ctypes.byref(params), _ptr(cv), _ptr(d_out), B, _ptr(d_cv),
                                            _ptr(d_w), _ptr(d_b), _ptr(ws), ws.numel(), flags, _stream(dev))
             _lib.check(rc, "c2v_label_backward_ws")

@@ -88,7 +88,7 @@ class _LabelFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, cv, w_out, b_out, dims, algo, cache):
-        params = CF.make_params(None, None, None, None, None, None, w_out, b_out)
+        params = CF.make_params(w_out=w_out, b_out=b_out)
         if any(ctx.needs_input_grad[:3]):
             algo = int(algo) | CF.NO_PDL            # the calls that feed autograd use plain stream-ordered launches
         out = CF.label_logits(dims, params, cv, algo, cache=cache, weight=w_out)
@@ -99,7 +99,7 @@ class _LabelFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, d_out):
         cv, w_out = ctx.saved_tensors
-        params = CF.make_params(None, None, None, None, None, None, w_out, None)
+        params = CF.make_params(w_out=w_out)
         d_cv, d_w, d_b = CF.label_backward(ctx.dims, params, cv, d_out, ctx.needs_input_grad[0],
                                            ctx.needs_input_grad[1], ctx.needs_input_grad[2], algo=ctx.algo, cache=ctx.cache,
                                            weight=w_out)
@@ -111,7 +111,7 @@ class _AngularFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, cv, w_out, label, dims, margin, inverse_temp):
-        params = CF.make_params(None, None, None, None, None, None, w_out, None)
+        params = CF.make_params(w_out=w_out)
         out, cos, inv = CF.angular_forward_train(dims, params, cv, label, margin, inverse_temp)
         ctx.save_for_backward(cv, w_out, label, cos, inv)
         ctx.cfg = (dims, margin, inverse_temp)
@@ -121,68 +121,49 @@ class _AngularFn(torch.autograd.Function):
     def backward(ctx, d_out):
         cv, w_out, label, cos, inv = ctx.saved_tensors
         dims, margin, inverse_temp = ctx.cfg
-        params = CF.make_params(None, None, None, None, None, None, w_out, None)
+        params = CF.make_params(w_out=w_out)
         d_cv, d_w = CF.angular_backward(dims, params, cv, label, margin, inverse_temp, cos, inv, d_out,
                                         ctx.needs_input_grad[0], ctx.needs_input_grad[1])
         return d_cv, d_w, None, None, None, None
 
 
 class _LabelLossFn(torch.autograd.Function):
-    """mean NLL of log_softmax(cv . W_out^T + b) (model.py:83 + main.py:251-264) without materialising the logits:
-    the label GEMM's epilogue produces loss / logsumexp / arg-max; the backward recomputes the tile-wise softmax."""
+    """mean NLL of log_softmax over the label head's logits (+ main.py:251-264) without materialising them: the label
+    GEMM's epilogue produces loss / logsumexp / arg-max; the backward recomputes G = d loss / d logits tile by tile and
+    runs the label backward on it.  angular=None: the plain head cv . W_out^T + b (model.py:83).
+    angular=(margin, inverse_temp), b_out=None: the angular-margin head (model.py:71-80), whose G is d loss / d (cv . W^T)
+    and whose backward then projects through F.normalize."""
 
     @staticmethod
-    def forward(ctx, cv, w_out, b_out, label, dims, algo, cache):
-        params = CF.make_params(None, None, None, None, None, None, w_out, b_out)
+    def forward(ctx, cv, w_out, b_out, label, dims, algo, cache, angular):
+        params = CF.make_params(w_out=w_out, b_out=b_out)
         if any(ctx.needs_input_grad[:3]):
-            algo = int(algo) | CF.NO_PDL
-        loss, lse, am, mx, _ = CF.label_loss(dims, params, cv, label, want_logits=False, algo=algo, cache=cache, weight=w_out)
-        ctx.save_for_backward(cv, w_out, b_out, label, lse)
-        ctx.dims, ctx.cache, ctx.algo = dims, cache, algo
+            algo = int(algo) | CF.NO_PDL            # the calls that feed autograd use plain stream-ordered launches
+        if angular is None:
+            loss, lse, am, mx, _ = CF.label_loss(dims, params, cv, label, algo=algo, cache=cache, weight=w_out)
+            inv = None
+        else:
+            loss, lse, am, mx, inv, _ = CF.angular_loss(dims, params, cv, label, *angular, algo=algo, cache=cache, weight=w_out)
+        ctx.save_for_backward(cv, w_out, b_out, label, lse, inv)
+        ctx.dims, ctx.cache, ctx.algo, ctx.angular = dims, cache, algo, angular
         ctx.mark_non_differentiable(am, mx)
         return loss, am, mx
 
     @staticmethod
     def backward(ctx, d_loss, _d_am, _d_mx):
-        cv, w_out, b_out, label, lse = ctx.saved_tensors
-        params = CF.make_params(None, None, None, None, None, None, w_out, b_out)
-        B = cv.shape[0]
-        d_out = CF.label_dlogits(ctx.dims, params, cv, label, lse, 1.0 / B, scale_device=d_loss.reshape(1),
-                                 algo=ctx.algo, cache=ctx.cache, weight=w_out)
-        d_cv, d_w, d_b = CF.label_backward(ctx.dims, params, cv, d_out, ctx.needs_input_grad[0], ctx.needs_input_grad[1],
-                                           ctx.needs_input_grad[2], algo=int(ctx.algo) & 0xff, cache=ctx.cache, weight=w_out,
-                                           absmax_ready=True)
-        return d_cv, d_w, d_b, None, None, None, None
-
-
-class _AngularLossFn(torch.autograd.Function):
-    """mean NLL of log_softmax over the angular-margin head (model.py:71-80 + main.py:251-264) without materialising the
-    logits: the label GEMM's angular epilogue produces loss / logsumexp / arg-max; the backward recomputes
-    G = d loss / d (cv . W^T) tile by tile, runs the plain label backward on it and projects through F.normalize."""
-
-    @staticmethod
-    def forward(ctx, cv, w_out, label, dims, margin, inverse_temp, algo, cache):
-        params = CF.make_params(None, None, None, None, None, None, w_out, None)
-        if any(ctx.needs_input_grad[:2]):
-            algo = int(algo) | CF.NO_PDL
-        loss, lse, am, mx, inv, _ = CF.angular_loss(dims, params, cv, label, margin, inverse_temp, want_logits=False,
-                                                    algo=algo, cache=cache, weight=w_out)
-        ctx.save_for_backward(cv, w_out, label, lse, inv)
-        ctx.dims, ctx.cache, ctx.algo, ctx.cfg = dims, cache, algo, (margin, inverse_temp)
-        ctx.mark_non_differentiable(am, mx)
-        return loss, am, mx
-
-    @staticmethod
-    def backward(ctx, d_loss, _d_am, _d_mx):
-        cv, w_out, label, lse, inv = ctx.saved_tensors
-        margin, inverse_temp = ctx.cfg
-        params = CF.make_params(None, None, None, None, None, None, w_out, None)
-        B = cv.shape[0]
-        g = CF.angular_dlogits(ctx.dims, params, cv, label, lse, inv, margin, inverse_temp, 1.0 / B,
-                               scale_device=d_loss.reshape(1), algo=ctx.algo, cache=ctx.cache, weight=w_out)
-        d_cv, d_w = CF.angular_backward_ws(ctx.dims, params, cv, g, inv, ctx.needs_input_grad[0], ctx.needs_input_grad[1],
-                                           algo=int(ctx.algo) & 0xff, cache=ctx.cache, weight=w_out, absmax_ready=True)
-        return d_cv, d_w, None, None, None, None, None, None
+        cv, w_out, b_out, label, lse, inv = ctx.saved_tensors
+        params = CF.make_params(w_out=w_out, b_out=b_out)
+        dlogits = dict(scale_device=d_loss.reshape(1), algo=ctx.algo, cache=ctx.cache, weight=w_out)
+        bw = dict(algo=int(ctx.algo) & 0xff, cache=ctx.cache, weight=w_out, absmax_ready=True)
+        need, scale = ctx.needs_input_grad, 1.0 / cv.shape[0]
+        if ctx.angular is None:
+            g = CF.label_dlogits(ctx.dims, params, cv, label, lse, scale, **dlogits)
+            d_cv, d_w, d_b = CF.label_backward(ctx.dims, params, cv, g, need[0], need[1], need[2], **bw)
+        else:
+            g = CF.angular_dlogits(ctx.dims, params, cv, label, lse, inv, *ctx.angular, scale, **dlogits)
+            d_cv, d_w = CF.angular_backward_ws(ctx.dims, params, cv, g, inv, need[0], need[1], **bw)
+            d_b = None
+        return d_cv, d_w, d_b, None, None, None, None, None
 
 
 class Code2Vec(nn.Module):
@@ -216,6 +197,8 @@ class Code2Vec(nn.Module):
             self.output_linear.bias.data.fill_(0.0)
 
         self.algo = {"auto": _lib.ALGO_AUTO, "ffma": _lib.ALGO_FFMA, "tcgen05": _lib.ALGO_TCGEN05}[algo]
+        # the label head takes the tensor cores wherever its shape allows them, unless algo="ffma"
+        self._label_algo = _lib.ALGO_FFMA if self.algo == _lib.ALGO_FFMA else _lib.ALGO_AUTO
         self._dropout_calls = 0
         # persistent workspaces: the hi/lo split images of input_linear / output_linear are rebuilt
         # only when the optimizer changed the weights (tracked by the tensors' version counters)
@@ -240,52 +223,14 @@ class Code2Vec(nn.Module):
         self._dropout_calls += 1
         return int(torch.randint(0, 2 ** 62, (1,)).item())
 
-    def _angular_outputs(self, code_vector, label, dims):
-        """the angular-margin head's logits (model.py:71-80) on the CUDA cores"""
-        option = self.option
-        if torch.is_grad_enabled() and (code_vector.requires_grad or self.output_linear.requires_grad):
-            return _AngularFn.apply(code_vector, self.output_linear, label, dims, option.angular_margin, option.inverse_temp)
-        params = CF.make_params(None, None, None, None, None, None, self.output_linear, None)
-        return CF.angular_logits(dims, params, code_vector, label, option.angular_margin, option.inverse_temp)
+    def _head(self):
+        """-> (W_out, b_out) of the label head; the angular-margin head has no bias"""
+        if self.option.angular_margin_loss:
+            return self.output_linear, None
+        return self.output_linear.weight, self.output_linear.bias
 
-    # -- the reference surface -------------------------------------------------------------
-    def check_indices(self):
-        """Synchronise and raise IndexError if any forward so far saw an index outside the embedding tables
-        (`forward` itself raises it one call late, without synchronising: see functional.PrepCache.raise_deferred)."""
-        self._enc_cache.raise_deferred(synchronize=True)
-
-    def forward(self, starts, paths, ends, label):
-        self._enc_cache.raise_deferred()
-        self._enc_cache.fuse_grad_accumulation = self.fuse_grad_accumulation
-        self._enc_cache.on_path_grads_ready = self.on_path_grads_ready
-        option = self.option
-        dims = self._dims()
-        training = self.training and self.input_dropout is not None
-        drop_p = float(option.dropout_prob) if training else 0.0
-        seed = self._next_seed() if training else 0
-
-        code_vector, attention = _EncodeFn.apply(
-            self.terminal_embedding.weight, self.path_embedding.weight, self.input_linear.weight,
-            self.input_layer_norm.weight, self.input_layer_norm.bias, self.attention_parameter,
-            starts, paths, ends, dims, drop_p, training, seed, self.algo, self._enc_cache)
-
-        if option.angular_margin_loss:
-            outputs = self._angular_outputs(code_vector, label, dims)
-        else:
-            outputs = _LabelFn.apply(code_vector, self.output_linear.weight, self.output_linear.bias, dims,
-                                     _lib.ALGO_FFMA if self.algo == _lib.ALGO_FFMA else _lib.ALGO_AUTO,
-                                     self._lab_cache)
-
-        return outputs, code_vector, attention
-
-    # -- additive fast path: forward + calculate_loss (main.py:251-264) + torch.max (main.py:285) -----
-    def forward_loss(self, starts, paths, ends, label):
-        """-> (loss, pred_label [b], pred_score [b], code_vector [b,H], attention [b,L]); loss is the mean NLL the
-        reference's `calculate_loss(preds, label, criterion, option)` returns (criterion weights are all
-        1) and is autograd-connected; the [b, C] logits are never written.  Both label heads: with
-        option.angular_margin_loss the loss, arg-max and max are those of the angular-margin logits (model.py:71-80).
-        Shapes the fused kernel does not take, and algo="ffma", fall back to forward()'s head + eager log_softmax / NLL +
-        torch.max."""
+    def _encode(self, starts, paths, ends):
+        """the encode of forward() / forward_loss(), autograd-connected -> (code_vector, attention, dims)"""
         self._enc_cache.raise_deferred()
         self._enc_cache.fuse_grad_accumulation = self.fuse_grad_accumulation
         self._enc_cache.on_path_grads_ready = self.on_path_grads_ready
@@ -297,23 +242,61 @@ class Code2Vec(nn.Module):
             self.terminal_embedding.weight, self.path_embedding.weight, self.input_linear.weight,
             self.input_layer_norm.weight, self.input_layer_norm.bias, self.attention_parameter,
             starts, paths, ends, dims, drop_p, training, seed, self.algo, self._enc_cache)
-        fused = self.algo != _lib.ALGO_FFMA and CF.label_loss_supported(dims, starts.shape[0])
-        if self.option.angular_margin_loss:
-            if fused:
-                loss, am, mx = _AngularLossFn.apply(code_vector, self.output_linear, label, dims, self.option.angular_margin,
-                                                    self.option.inverse_temp, _lib.ALGO_AUTO, self._lab_cache)
-            else:
-                outputs = self._angular_outputs(code_vector, label, dims)
-                loss = F.nll_loss(F.log_softmax(outputs, dim=1), label)
-                mx, am = torch.max(outputs.detach(), dim=1)
-        elif fused:
-            loss, am, mx = _LabelLossFn.apply(code_vector, self.output_linear.weight, self.output_linear.bias, label, dims,
-                                              _lib.ALGO_AUTO, self._lab_cache)
+        return code_vector, attention, dims
+
+    def _encode_eval(self, starts, paths, ends):
+        """the encode of predict() / predict_topk(), without autograd or dropout -> (code_vector, attention, dims)"""
+        self._enc_cache.raise_deferred()
+        dims = self._dims()
+        params = CF.make_params(self.terminal_embedding.weight, self.path_embedding.weight, self.input_linear.weight,
+                                self.input_layer_norm.weight, self.input_layer_norm.bias, self.attention_parameter)
+        code_vector, attention = CF.encode_forward(dims, params, starts, paths, ends, algo=self.algo,
+                                                   cache=self._enc_cache, weight=self.input_linear.weight)
+        return code_vector, attention, dims
+
+    def _head_logits(self, code_vector, label, dims):
+        """forward()'s logits: model.py:83, or the angular-margin head (model.py:71-80) on the CUDA cores"""
+        option = self.option
+        if not option.angular_margin_loss:
+            return _LabelFn.apply(code_vector, *self._head(), dims, self._label_algo, self._lab_cache)
+        if torch.is_grad_enabled() and (code_vector.requires_grad or self.output_linear.requires_grad):
+            return _AngularFn.apply(code_vector, self.output_linear, label, dims, option.angular_margin, option.inverse_temp)
+        params = CF.make_params(w_out=self.output_linear)
+        return CF.angular_logits(dims, params, code_vector, label, option.angular_margin, option.inverse_temp)
+
+    @staticmethod
+    def _eager_loss(outputs, label):
+        """forward_loss() from materialised logits: eager log_softmax / NLL (main.py:251-264) + torch.max (main.py:285)"""
+        loss = F.nll_loss(F.log_softmax(outputs, dim=1), label)
+        mx, am = torch.max(outputs.detach(), dim=1)
+        return loss, am, mx
+
+    # -- the reference surface -------------------------------------------------------------
+    def check_indices(self):
+        """Synchronise and raise IndexError if any forward so far saw an index outside the embedding tables
+        (`forward` itself raises it one call late, without synchronising: see functional.PrepCache.raise_deferred)."""
+        self._enc_cache.raise_deferred(synchronize=True)
+
+    def forward(self, starts, paths, ends, label):
+        code_vector, attention, dims = self._encode(starts, paths, ends)
+        return self._head_logits(code_vector, label, dims), code_vector, attention
+
+    # -- additive fast path: forward + calculate_loss (main.py:251-264) + torch.max (main.py:285) -----
+    def forward_loss(self, starts, paths, ends, label):
+        """-> (loss, pred_label [b], pred_score [b], code_vector [b,H], attention [b,L]); loss is the mean NLL the
+        reference's `calculate_loss(preds, label, criterion, option)` returns (criterion weights are all
+        1) and is autograd-connected; the [b, C] logits are never written.  Both label heads: with
+        option.angular_margin_loss the loss, arg-max and max are those of the angular-margin logits (model.py:71-80).
+        Shapes the fused kernel does not take, and algo="ffma", fall back to forward()'s head + eager log_softmax / NLL +
+        torch.max."""
+        code_vector, attention, dims = self._encode(starts, paths, ends)
+        if self.algo != _lib.ALGO_FFMA and CF.label_loss_supported(dims, starts.shape[0]):
+            o = self.option
+            angular = (o.angular_margin, o.inverse_temp) if o.angular_margin_loss else None
+            loss, am, mx = _LabelLossFn.apply(code_vector, *self._head(), label, dims, self._label_algo, self._lab_cache,
+                                              angular)
         else:
-            outputs = _LabelFn.apply(code_vector, self.output_linear.weight, self.output_linear.bias, dims,
-                                     _lib.ALGO_FFMA if self.algo == _lib.ALGO_FFMA else _lib.ALGO_AUTO, self._lab_cache)
-            loss = F.nll_loss(F.log_softmax(outputs, dim=1), label)
-            mx, am = torch.max(outputs.detach(), dim=1)
+            loss, am, mx = self._eager_loss(self._head_logits(code_vector, label, dims), label)
         return loss, am, mx, code_vector, attention
 
     # -- additive convenience (the reference does torch.max(preds, dim=1) at main.py:285) ----
@@ -322,16 +305,10 @@ class Code2Vec(nn.Module):
         """-> (pred_label [b], pred_score [b], code_vector [b,H], attention [b,L])"""
         if self.option.angular_margin_loss:
             raise NotImplementedError("predict() needs the plain label head (the angular head needs labels)")
-        self._enc_cache.raise_deferred()
-        dims = self._dims()
-        params = CF.make_params(self.terminal_embedding.weight, self.path_embedding.weight, self.input_linear.weight,
-                                self.input_layer_norm.weight, self.input_layer_norm.bias, self.attention_parameter,
-                                self.output_linear.weight, self.output_linear.bias)
-        code_vector, attention = CF.encode_forward(dims, params, starts, paths, ends, algo=self.algo,
-                                                   cache=self._enc_cache, weight=self.input_linear.weight)
-        _, am, mx = CF.label_logits_argmax(dims, params, code_vector,
-                                           _lib.ALGO_FFMA if self.algo == _lib.ALGO_FFMA else _lib.ALGO_AUTO,
-                                           cache=self._lab_cache, weight=self.output_linear.weight, want_logits=False)
+        code_vector, attention, dims = self._encode_eval(starts, paths, ends)
+        w_out, b_out = self._head()
+        _, am, mx = CF.label_logits_argmax(dims, CF.make_params(w_out=w_out, b_out=b_out), code_vector, self._label_algo,
+                                           cache=self._lab_cache, weight=w_out, want_logits=False)
         return am, mx, code_vector, attention
 
     _TOPK_ROWS = 2048                   # rows per fused top-k call (c2v_label_topk_supported)
@@ -350,15 +327,10 @@ class Code2Vec(nn.Module):
         C = self.option.label_count
         if not 1 <= k <= C:
             raise ValueError(f"predict_topk: k = {k} is outside [1, label_count = {C}]")
-        self._enc_cache.raise_deferred()
-        dims = self._dims()
+        code_vector, attention, dims = self._encode_eval(starts, paths, ends)
         angular = self.option.angular_margin_loss
-        w_out = self.output_linear if angular else self.output_linear.weight
-        params = CF.make_params(self.terminal_embedding.weight, self.path_embedding.weight, self.input_linear.weight,
-                                self.input_layer_norm.weight, self.input_layer_norm.bias, self.attention_parameter,
-                                w_out, None if angular else self.output_linear.bias)
-        code_vector, attention = CF.encode_forward(dims, params, starts, paths, ends, algo=self.algo,
-                                                   cache=self._enc_cache, weight=self.input_linear.weight)
+        w_out, b_out = self._head()
+        params = CF.make_params(w_out=w_out, b_out=b_out)
         b = code_vector.shape[0]
         if self.algo != _lib.ALGO_FFMA and CF.label_topk_supported(dims, min(b, self._TOPK_ROWS), k):
             parts = []
@@ -374,9 +346,7 @@ class Code2Vec(nn.Module):
         if angular:
             logits = self.option.inverse_temp * F.linear(F.normalize(code_vector), F.normalize(w_out))
         else:
-            logits = CF.label_logits(dims, params, code_vector,
-                                     _lib.ALGO_FFMA if self.algo == _lib.ALGO_FFMA else _lib.ALGO_AUTO,
-                                     cache=self._lab_cache, weight=w_out)
+            logits = CF.label_logits(dims, params, code_vector, self._label_algo, cache=self._lab_cache, weight=w_out)
         val, idx = torch.sort(logits, dim=1, descending=True, stable=True)
         val, idx = val[:, :k].contiguous(), idx[:, :k].contiguous()
         prob = torch.softmax(logits, dim=1).gather(1, idx) if probs else None
