@@ -59,6 +59,15 @@ SYMBOLS = {
                                           c_vp, c_vp, c_vp, c_sz, c_i32, c_vp]),
     "c2v_encode_forward_stash": (ctypes.c_int, [_P(Dims), _P(Params), c_vp, c_vp, c_vp, c_i32, c_i32, _P(Dropout),
                                                 c_vp, c_vp, c_vp, c_vp, c_sz, c_i32, c_vp]),
+    "c2v_encode_packed_workspace_bytes": (c_sz, [_P(Dims), c_i32, c_i64]),
+    "c2v_encode_forward_packed": (ctypes.c_int, [_P(Dims), _P(Params), c_vp, c_vp, c_vp, c_vp, c_i32, c_i64, c_i32,
+                                                 _P(Dropout), c_vp, c_vp, c_vp, c_vp, c_sz, c_i32, c_vp]),
+    "c2v_encode_backward_packed_workspace_bytes": (c_sz, [_P(Dims), c_i32, c_i64]),
+    "c2v_encode_backward_packed": (ctypes.c_int, [_P(Dims), _P(Params), c_vp, c_vp, c_vp, c_vp, c_i32, c_i64, c_i32,
+                                                  _P(Dropout), c_vp, c_vp, c_vp, c_vp, c_vp, _P(Grads), c_vp, c_sz, c_i32,
+                                                  c_vp]),
+    "c2v_build_batch_packed": (ctypes.c_int, [c_vp, c_vp, c_i64, c_vp, c_vp, c_i32, c_i32, ctypes.c_uint64, c_i64, c_i64,
+                                              c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "c2v_workspace_status": (c_i64, [c_vp, c_vp]),
     "c2v_workspace_set_status_mirror": (ctypes.c_int, [c_vp, c_vp, c_vp]),
     "c2v_label_workspace_bytes": (c_sz, [_P(Dims), c_i32]),

@@ -9,13 +9,34 @@ CPU fallback.
 """
 import ctypes
 
+import numpy as np
 import torch
 
 from . import _lib
+from .functional import PackedBags
 
 
 def _ptr(t):
     return ctypes.c_void_p(t.data_ptr()) if t is not None else None
+
+
+def packed_offsets(counts, item_ids, max_path_length):
+    """Bag offsets (numpy int64 [B + 1]) of the packed batch of items `item_ids` (host int array [B]) over a corpus whose
+    item i holds counts[i] contexts: bag b holds min(counts[id], L) contexts, and one (a pad context) when the item has
+    none or the id is outside [0, len(counts)).  A pure host function: no device copy."""
+    counts = np.asarray(counts, dtype=np.int64)
+    ids = np.asarray(item_ids, dtype=np.int64).reshape(-1)
+    ok = (ids >= 0) & (ids < counts.size)
+    n = np.zeros(ids.size, np.int64)
+    n[ok] = counts[ids[ok]]
+    off = np.zeros(ids.size + 1, np.int64)
+    np.cumsum(np.clip(n, 1, int(max_path_length)), out=off[1:])
+    return off
+
+
+def _upload(a, device):
+    """host int64 array -> device tensor through pinned memory, without blocking the host"""
+    return torch.from_numpy(np.ascontiguousarray(a, dtype=np.int64)).pin_memory().to(device, non_blocking=True)
 
 
 class DeviceCorpus:
@@ -25,6 +46,8 @@ class DeviceCorpus:
         dev = torch.device(device)
         if dev.type != "cuda":
             raise _lib.C2VError("DeviceCorpus lives on a CUDA device (sm_100a); there is no CPU path")
+        host_offsets = (offsets.cpu().numpy() if isinstance(offsets, torch.Tensor) else np.asarray(offsets)).astype(np.int64).reshape(-1)
+        self.counts = np.diff(host_offsets)           # contexts per item, on the host: packed bag offsets need no copy
         self.offsets = torch.as_tensor(offsets, dtype=torch.int64).contiguous().to(dev)
         self.contexts = torch.as_tensor(contexts, dtype=torch.int32).reshape(-1, 3).contiguous().to(dev)
         self.labels = None if labels is None else torch.as_tensor(labels, dtype=torch.int64).contiguous().to(dev)
@@ -130,6 +153,59 @@ class DeviceCorpus:
         order = order[rank::world]
         for lo in range(0, order.numel(), batch_size):          # last batch ragged (drop_last unset, main.py:162)
             yield self.build(order[lo:lo + batch_size], max_path_length, seed)
+
+    def build_packed(self, item_ids, max_path_length, seed):
+        """-> (PackedBags, label [B]): the bags `build` returns for the same ids and seed, without the zero suffix.  Bag b
+        holds min(n, L) contexts of its item (n = the item's context count); an empty item or an id outside the corpus is a
+        bag of one pad context (0, 0, 0).  item_ids: host ints (a list, numpy array or CPU tensor: ids and bag offsets go to
+        the device in one pinned, asynchronous copy) or a CUDA tensor (one device-to-host copy of the ids, because the bag
+        offsets are computed on the host)."""
+        L = int(max_path_length)
+        if isinstance(item_ids, torch.Tensor) and item_ids.is_cuda:
+            ids = item_ids.to(dtype=torch.int64).reshape(-1).contiguous()
+            off = packed_offsets(self.counts, ids.cpu().numpy(), L)
+            off_dev = _upload(off, self.device)
+        else:
+            host_ids = (item_ids.numpy() if isinstance(item_ids, torch.Tensor) else np.asarray(item_ids)).astype(np.int64).reshape(-1)
+            off = packed_offsets(self.counts, host_ids, L)
+            staged = _upload(np.concatenate([host_ids, off]), self.device)
+            ids, off_dev = staged[:host_ids.size], staged[host_ids.size:]
+        return self._build_packed(ids, off, off_dev, L, seed)
+
+    def _build_packed(self, ids, off, off_dev, L, seed):
+        """c2v_build_batch_packed for device ids [B] and bag offsets given on the host (off) and on the device (off_dev)"""
+        lib = _lib.load()
+        B, N = int(ids.numel()), int(off[-1])
+        with torch.cuda.device(self.device):
+            starts = torch.empty((N,), dtype=torch.int64, device=self.device)
+            bags = PackedBags(starts, torch.empty_like(starts), torch.empty_like(starts), off, L,
+                              device_offsets=off_dev)                                  # filled below
+            label = torch.empty((B,), dtype=torch.int64, device=self.device)
+            rc = lib.c2v_build_batch_packed(_ptr(self.offsets), _ptr(self.contexts), self.n_items, _ptr(ids), _ptr(self.labels),
+                                            B, L, int(seed) & 0xFFFFFFFFFFFFFFFF, self.method_token, self.question_token,
+                                            _ptr(bags.offsets), _ptr(bags.starts), _ptr(bags.paths), _ptr(bags.ends),
+                                            _ptr(label), ctypes.c_void_p(torch.cuda.current_stream(self.device).cuda_stream))
+            _lib.check(rc, "c2v_build_batch_packed")
+        return bags, label
+
+    def epoch_packed(self, batch_size, max_path_length, seed, shuffle=True, rank=0, world=1):
+        """`epoch` with packed batches: the same permutation, the same items in the same order -> (PackedBags, label) per
+        batch, as build_packed makes them.  Per epoch, not per batch: one device-to-host copy of the permutation (the bag
+        offsets are computed on the host) and one pinned, asynchronous copy of every batch's offsets to the device; each
+        batch takes its ids and offsets as slices of device tensors."""
+        L = int(max_path_length)
+        g = torch.Generator(device=self.device).manual_seed(int(seed))
+        order = torch.randperm(self.n_items, generator=g, device=self.device) if shuffle else \
+            torch.arange(self.n_items, device=self.device)
+        order = order[rank::world].contiguous()
+        host = order.cpu().numpy()
+        spans = [(lo, min(lo + batch_size, host.size)) for lo in range(0, host.size, batch_size)]
+        offs = [packed_offsets(self.counts, host[lo:hi], L) for lo, hi in spans]
+        if not offs:
+            return
+        all_dev = _upload(np.concatenate(offs), self.device)        # batch i's B + 1 offsets start at lo + i
+        for i, ((lo, hi), off) in enumerate(zip(spans, offs)):
+            yield self._build_packed(order[lo:hi], off, all_dev[lo + i:hi + i + 1], L, seed)
 
     def epoch_vars(self, batch_size, max_path_length, seed, shuffle=True, rank=0, world=1):
         """the same pass over the variable-name units (dataset_builder.py:152-204)"""

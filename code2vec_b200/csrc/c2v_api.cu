@@ -45,6 +45,7 @@ int launch_encode_backward(const c2v_dims *d, const c2v_params *p, const EncodeA
                            const float *d_att, const c2v_grads *g, void *ws, size_t ws_bytes,
                            cudaStream_t st, const float *x_stash, int phase);
 size_t encode_backward_workspace_bytes(const c2v_dims *d, int B, int L);
+size_t encode_backward_workspace_bytes_n(const c2v_dims *d, int B, long long N, bool packed);
 bool label_tcgen05_shape_ok(const c2v_dims *d);
 bool label_backward_tc_ok(const c2v_dims *d);
 int label_w_image(const c2v_dims *d, const float *Wout, int B, void *ws, size_t ws_bytes, bool reuse_prep, cudaStream_t st,
@@ -94,13 +95,13 @@ static bool dims_ok(const c2v_dims *d)
 // tile rows used for sizing: the smallest tile any algorithm uses (64) gives the most slots
 static const int kMinTileRows = 16;   // tensor-core path: one partial per 16-row consumer warp
 
-EncodeWorkspace carve_encode_workspace(const c2v_dims *d, int B, int L, void *base)
+// N context rows; a packed batch (row_bag != NULL) gets its row -> bag map (int32 [N]) behind everything else
+EncodeWorkspace carve_encode_workspace_n(const c2v_dims *d, int B, long long N, void *base, int **row_bag)
 {
     EncodeWorkspace w;
     memset(&w, 0, sizeof(w));
     const int H = d->encode, D = 2 * d->terminal_embed + d->path_embed;
     const int Hs = (H + 3) / 4 * 4;
-    const long long N = (long long)B * L;
     const size_t n_tiles = (size_t)((N + kMinTileRows - 1) / kMinTileRows);
     const size_t slots = n_tiles + (size_t)B + 1;
     // tcgen05 split weights: K padded to 64-element blocks, N padded to 128 rows... sized generously
@@ -120,8 +121,14 @@ EncodeWorkspace carve_encode_workspace(const c2v_dims *d, int B, int L, void *ba
     w.part_m = reinterpret_cast<float *>(take(slots * sizeof(float)));
     w.part_s = reinterpret_cast<float *>(take(slots * sizeof(float)));
     w.part_v = reinterpret_cast<float *>(take(slots * (size_t)H * sizeof(float)));
+    if (row_bag) *row_bag = reinterpret_cast<int *>(take((size_t)N * sizeof(int)));
     w.bytes = o;
     return w;
+}
+
+EncodeWorkspace carve_encode_workspace(const c2v_dims *d, int B, int L, void *base)
+{
+    return carve_encode_workspace_n(d, B, (long long)B * L, base, nullptr);
 }
 
 }  // namespace c2v
@@ -167,24 +174,21 @@ int c2v_encode_forward(const c2v_dims *d, const c2v_params *p, const int64_t *st
                                     workspace_bytes, algo, stream);
 }
 
-int c2v_encode_forward_stash(const c2v_dims *d, const c2v_params *p, const int64_t *starts,
-                             const int64_t *paths, const int64_t *ends, int32_t B, int32_t L,
-                             const c2v_dropout *drop, float *code_vector, float *attention, float *x_stash,
-                             void *workspace, size_t workspace_bytes, int32_t algo, void *stream)
+// The encode of both layouts once the caller's argument checks have passed: [B, L] (offsets == NULL, N = B * L) or
+// packed (bag b = rows offsets[b] .. offsets[b+1]-1, N rows in all).
+static int encode_forward_impl(const char *fn, const c2v_dims *d, const c2v_params *p, const int64_t *starts,
+                               const int64_t *paths, const int64_t *ends, const int64_t *offsets, int32_t B, long long N,
+                               int32_t L, const c2v_dropout *drop, float *code_vector, float *attention, float *x_stash,
+                               void *workspace, size_t workspace_bytes, int32_t algo, void *stream)
 {
-    if (!dims_ok(d)) return C2V_EINVAL;
-    if (!p || !starts || !paths || !ends || !code_vector || !attention || !workspace) {
-        set_error("c2v_encode_forward: NULL pointer argument");
-        return C2V_EINVAL;
-    }
     if (!p->terminal_embedding || !p->path_embedding || !p->input_linear || !p->ln_weight ||
         !p->ln_bias || !p->attention) {
-        set_error("c2v_encode_forward: NULL parameter pointer");
+        set_error("%s: NULL parameter pointer", fn);
         return C2V_EINVAL;
     }
-    if (B < 1 || L < 1) { set_error("c2v_encode_forward: B=%d L=%d", B, L); return C2V_EINVAL; }
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    EncodeWorkspace ws = carve_encode_workspace(d, B, L, workspace);
+    int *row_bag = nullptr;
+    EncodeWorkspace ws = carve_encode_workspace_n(d, B, N, workspace, offsets ? &row_bag : nullptr);
     if (ws.bytes > workspace_bytes) {
         set_error("workspace too small: %zu < %zu", workspace_bytes, ws.bytes);
         return C2V_EWORKSPACE;
@@ -205,7 +209,7 @@ int c2v_encode_forward_stash(const c2v_dims *d, const c2v_params *p, const int64
     } else if (algo == C2V_ALGO_AUTO) {
         use_tc = tcgen05_shape_ok(d);
     } else {
-        set_error("unknown algo %d", algo);
+        set_error("%s: unknown algo %d", fn, algo);
         return C2V_EINVAL;
     }
 
@@ -219,7 +223,7 @@ int c2v_encode_forward_stash(const c2v_dims *d, const c2v_params *p, const int64
     a.T = d->terminal_count; a.P = d->path_count;
     a.Et = d->terminal_embed; a.Ep = d->path_embed; a.H = d->encode;
     a.D = 2 * a.Et + a.Ep;
-    a.L = L; a.N = (long long)B * L;
+    a.L = L; a.N = N;
     a.drop_p = 0.0f; a.drop_scale = 1.0f; a.seed = 0;
     if (drop && drop->training && drop->p > 0.0f && drop->p < 1.0f) {   // model.py:26-29
         a.drop_p = drop->p; a.drop_scale = 1.0f / (1.0f - drop->p); a.seed = drop->seed;
@@ -227,6 +231,9 @@ int c2v_encode_forward_stash(const c2v_dims *d, const c2v_params *p, const int64
     a.attention = attention;
     a.stash_x = x_stash;
     a.flags = 0;
+    a.bag_off = reinterpret_cast<const long long *>(offsets);
+    a.row_bag = row_bag;
+    a.n_bags = B;
     // rows per softmax partial: 64-row CTA tiles (FFMA) or 16-row consumer warps (tensor cores)
     ws.tile_rows = use_tc ? 16 : 64;
     const int cta_rows = use_tc ? 128 : 64;
@@ -246,6 +253,10 @@ int c2v_encode_forward_stash(const c2v_dims *d, const c2v_params *p, const int64
         rc = use_tc ? launch_split_w_tcgen05(d, p->input_linear, a.ws, st)
                     : launch_transpose_w(p->input_linear, ws.w_t, a.H, a.D, (a.H + 3) / 4 * 4, st);
     if (rc != C2V_OK) return rc;
+    if (row_bag) {
+        rc = launch_row_bag(a.bag_off, B, N, row_bag, st);
+        if (rc != C2V_OK) return rc;
+    }
     int slot = -1;
     if (g_prof_on && (g_prof_calls++ % g_prof_stride) == 0) {
         if (g_prof_pending == kProfRing) { rc = prof_drain(); if (rc != C2V_OK) return rc; }
@@ -259,6 +270,54 @@ int c2v_encode_forward_stash(const c2v_dims *d, const c2v_params *p, const int64
         g_prof_pending = slot + 1;
     }
     return launch_encode_finalize(a, B, code_vector, st);
+}
+
+int c2v_encode_forward_stash(const c2v_dims *d, const c2v_params *p, const int64_t *starts,
+                             const int64_t *paths, const int64_t *ends, int32_t B, int32_t L,
+                             const c2v_dropout *drop, float *code_vector, float *attention, float *x_stash,
+                             void *workspace, size_t workspace_bytes, int32_t algo, void *stream)
+{
+    if (!dims_ok(d)) return C2V_EINVAL;
+    if (!p || !starts || !paths || !ends || !code_vector || !attention || !workspace) {
+        set_error("c2v_encode_forward: NULL pointer argument");
+        return C2V_EINVAL;
+    }
+    if (B < 1 || L < 1) { set_error("c2v_encode_forward: B=%d L=%d", B, L); return C2V_EINVAL; }
+    return encode_forward_impl("c2v_encode_forward", d, p, starts, paths, ends, nullptr, B, (long long)B * L, L, drop,
+                               code_vector, attention, x_stash, workspace, workspace_bytes, algo, stream);
+}
+
+// shape checks of the packed entry points
+static bool packed_shape_ok(const char *fn, int32_t B, int64_t N, int32_t L)
+{
+    if (B < 1 || L < 1 || N < B || N > (int64_t)B * L) {
+        set_error("%s: B=%d N=%lld L=%d: needs B >= 1, L >= 1 and B <= N <= B * L (every bag holds 1 .. L contexts)", fn, B,
+                  (long long)N, L);
+        return false;
+    }
+    return true;
+}
+
+size_t c2v_encode_packed_workspace_bytes(const c2v_dims *d, int32_t B, int64_t N)
+{
+    if (!dims_ok(d) || B < 1 || N < B) return 0;
+    int *row_bag = nullptr;
+    return carve_encode_workspace_n(d, B, N, nullptr, &row_bag).bytes;
+}
+
+int c2v_encode_forward_packed(const c2v_dims *d, const c2v_params *p, const int64_t *starts, const int64_t *paths,
+                              const int64_t *ends, const int64_t *offsets, int32_t B, int64_t N, int32_t L,
+                              const c2v_dropout *drop, float *code_vector, float *attention, float *x_stash,
+                              void *workspace, size_t workspace_bytes, int32_t algo, void *stream)
+{
+    if (!dims_ok(d)) return C2V_EINVAL;
+    if (!p || !starts || !paths || !ends || !offsets || !code_vector || !attention || !workspace) {
+        set_error("c2v_encode_forward_packed: NULL pointer argument");
+        return C2V_EINVAL;
+    }
+    if (!packed_shape_ok("c2v_encode_forward_packed", B, N, L)) return C2V_EINVAL;
+    return encode_forward_impl("c2v_encode_forward_packed", d, p, starts, paths, ends, offsets, B, N, L, drop, code_vector,
+                               attention, x_stash, workspace, workspace_bytes, algo, stream);
 }
 
 int c2v_profile_enable(int32_t on)
@@ -704,19 +763,13 @@ int c2v_encode_backward_stashed(const c2v_dims *d, const c2v_params *p, const in
                                       d_attention, grads, workspace, workspace_bytes, 0, stream);
 }
 
-int c2v_encode_backward_phased(const c2v_dims *d, const c2v_params *p, const int64_t *starts,
-                               const int64_t *paths, const int64_t *ends, int32_t B, int32_t L,
-                               const c2v_dropout *drop, const float *code_vector, const float *attention,
-                               const float *x_stash, const float *d_code_vector, const float *d_attention,
-                               const c2v_grads *grads, void *workspace, size_t workspace_bytes, int32_t phase, void *stream)
+// the backward of both layouts (offsets == NULL: [B, L], N = B * L) once the caller's argument checks have passed
+static int encode_backward_impl(const c2v_dims *d, const c2v_params *p, const int64_t *starts, const int64_t *paths,
+                                const int64_t *ends, const int64_t *offsets, int32_t B, long long N, int32_t L,
+                                const c2v_dropout *drop, const float *code_vector, const float *attention,
+                                const float *x_stash, const float *d_code_vector, const float *d_attention,
+                                const c2v_grads *grads, void *workspace, size_t workspace_bytes, int32_t phase, void *stream)
 {
-    if (phase < 0 || phase > 2) { set_error("c2v_encode_backward_phased: phase %d", phase); return C2V_EINVAL; }
-    if (!dims_ok(d)) return C2V_EINVAL;
-    if (!p || !starts || !paths || !ends || !code_vector || !attention || !d_code_vector || !grads ||
-        !workspace || B < 1 || L < 1) {
-        set_error("c2v_encode_backward: bad argument");
-        return C2V_EINVAL;
-    }
     if (!grads->terminal_embedding || !grads->path_embedding || !grads->input_linear ||
         !grads->ln_weight || !grads->ln_bias || !grads->attention) {
         set_error("c2v_encode_backward: NULL gradient pointer");
@@ -732,14 +785,57 @@ int c2v_encode_backward_phased(const c2v_dims *d, const c2v_params *p, const int
     a.T = d->terminal_count; a.P = d->path_count;
     a.Et = d->terminal_embed; a.Ep = d->path_embed; a.H = d->encode;
     a.D = 2 * a.Et + a.Ep;
-    a.L = L; a.N = (long long)B * L;
+    a.L = L; a.N = N;
     a.drop_p = 0.0f; a.drop_scale = 1.0f;
     if (drop && drop->training && drop->p > 0.0f && drop->p < 1.0f) {
         a.drop_p = drop->p; a.drop_scale = 1.0f / (1.0f - drop->p); a.seed = drop->seed;
     }
+    a.bag_off = reinterpret_cast<const long long *>(offsets);
+    a.n_bags = B;
     return launch_encode_backward(d, p, a, B, code_vector, attention, d_code_vector, d_attention,
                                   grads, workspace, workspace_bytes,
                                   static_cast<cudaStream_t>(stream), x_stash, phase);
+}
+
+int c2v_encode_backward_phased(const c2v_dims *d, const c2v_params *p, const int64_t *starts,
+                               const int64_t *paths, const int64_t *ends, int32_t B, int32_t L,
+                               const c2v_dropout *drop, const float *code_vector, const float *attention,
+                               const float *x_stash, const float *d_code_vector, const float *d_attention,
+                               const c2v_grads *grads, void *workspace, size_t workspace_bytes, int32_t phase, void *stream)
+{
+    if (phase < 0 || phase > 2) { set_error("c2v_encode_backward_phased: phase %d", phase); return C2V_EINVAL; }
+    if (!dims_ok(d)) return C2V_EINVAL;
+    if (!p || !starts || !paths || !ends || !code_vector || !attention || !d_code_vector || !grads ||
+        !workspace || B < 1 || L < 1) {
+        set_error("c2v_encode_backward: bad argument");
+        return C2V_EINVAL;
+    }
+    return encode_backward_impl(d, p, starts, paths, ends, nullptr, B, (long long)B * L, L, drop, code_vector, attention,
+                                x_stash, d_code_vector, d_attention, grads, workspace, workspace_bytes, phase, stream);
+}
+
+size_t c2v_encode_backward_packed_workspace_bytes(const c2v_dims *d, int32_t B, int64_t N)
+{
+    if (!dims_ok(d) || B < 1 || N < B) return 0;
+    return encode_backward_workspace_bytes_n(d, B, N, true);
+}
+
+int c2v_encode_backward_packed(const c2v_dims *d, const c2v_params *p, const int64_t *starts, const int64_t *paths,
+                               const int64_t *ends, const int64_t *offsets, int32_t B, int64_t N, int32_t L,
+                               const c2v_dropout *drop, const float *code_vector, const float *attention,
+                               const float *x_stash, const float *d_code_vector, const float *d_attention,
+                               const c2v_grads *grads, void *workspace, size_t workspace_bytes, int32_t phase, void *stream)
+{
+    if (phase < 0 || phase > 2) { set_error("c2v_encode_backward_packed: phase %d", phase); return C2V_EINVAL; }
+    if (!dims_ok(d)) return C2V_EINVAL;
+    if (!p || !starts || !paths || !ends || !offsets || !code_vector || !attention || !d_code_vector || !grads ||
+        !workspace) {
+        set_error("c2v_encode_backward_packed: NULL pointer argument");
+        return C2V_EINVAL;
+    }
+    if (!packed_shape_ok("c2v_encode_backward_packed", B, N, L)) return C2V_EINVAL;
+    return encode_backward_impl(d, p, starts, paths, ends, offsets, B, N, L, drop, code_vector, attention, x_stash,
+                                d_code_vector, d_attention, grads, workspace, workspace_bytes, phase, stream);
 }
 
 }  // extern "C"

@@ -58,6 +58,20 @@ __global__ void bag_dot_kernel(const float *__restrict__ att, const float *__res
     if (lane == 0) sb[b] = s;
 }
 
+// bag_dot_kernel of a packed batch: bag b is rows off[b] .. off[b+1]-1
+__global__ void bag_dot_packed_kernel(const float *__restrict__ att, const float *__restrict__ d_att,
+                                      const long long *__restrict__ off, long long N, float *__restrict__ sb)
+{
+    const int b = blockIdx.x, lane = threadIdx.x;
+    long long lo = off[b], hi = off[b + 1];
+    lo = lo < 0 ? 0 : (lo > N ? N : lo);
+    hi = hi < lo ? lo : (hi > N ? N : hi);
+    float s = 0.0f;
+    for (long long j = lo + lane; j < hi; j += 32) s = fmaf(att[j], d_att[j], s);
+    s = warp_sum(s);
+    if (lane == 0) sb[b] = s;
+}
+
 __device__ __forceinline__ void load_wrow_chunk(const float *__restrict__ W, int H, int D, float *Wc, int hc, int cb)
 {
     // KC rows (h) x NB columns (d) of W [H][D]
@@ -80,7 +94,7 @@ __device__ __forceinline__ void load_wrow_chunk(const float *__restrict__ W, int
     }
 }
 
-template <bool VEC>
+template <bool VEC, bool PACKED = false>
 __global__ void __launch_bounds__(THREADS)
 backward_rows_kernel(const EncodeArgs a, const BackwardArgs b, const int Hs)
 {
@@ -127,7 +141,8 @@ backward_rows_kernel(const EncodeArgs a, const BackwardArgs b, const int Hs)
                 for (int c = lane; c < Hs; c += 32) xr[c] = 0.0f;
                 continue;
             }
-            const long long bag = row / L;
+            const long long bag = PACKED ? bag_of_row<true>(a, row) : row / L;
+            const long long drow = dropout_row<PACKED>(a, row, bag);
             const float *gv = b.d_cv + bag * H, *cvb = b.cv + bag * H;
             const float alpha = b.att[row];
             float s = 0.0f;
@@ -147,7 +162,7 @@ backward_rows_kernel(const EncodeArgs a, const BackwardArgs b, const int Hs)
                     xh[k] = (xr[c] - mean) * rstd;
                     tt[k] = tanh_accurate(fmaf(xh[k], a.ln_g[c], a.ln_b[c]));
                     if (a.drop_p > 0.0f) {
-                        if ((k & 3) == 0) dbits = dropout_bits(a.seed, row, c >> 2);       // columns c .. c+3
+                        if ((k & 3) == 0) dbits = dropout_bits(a.seed, drow, c >> 2);      // columns c .. c+3
                         const unsigned w = (k & 3) == 0 ? dbits.x : (k & 3) == 1 ? dbits.y : (k & 3) == 2 ? dbits.z : dbits.w;
                         dm[k] = dropout_mul(w, a.drop_p, a.drop_scale);
                     }
@@ -301,7 +316,7 @@ backward_rows_kernel(const EncodeArgs a, const BackwardArgs b, const int Hs)
 // in registers for the whole launch, one Philox block serves four columns, and padded contexts (attention weight
 // exactly 0) cost one zero store.  encode_size % 4 == 0, <= 256.
 // ------------------------------------------------------------------------------------
-template <int NG>                                             // 128-column groups: 1 (encode_size <= 128) or 2
+template <int NG, bool PACKED = false>                        // 128-column groups: 1 (encode_size <= 128) or 2
 __global__ void __launch_bounds__(256, NG == 1 ? 4 : 2)
 backward_rows_lite_kernel(const EncodeArgs a, const BackwardArgs b)
 {
@@ -345,7 +360,8 @@ backward_rows_lite_kernel(const EncodeArgs a, const BackwardArgs b)
             for (int g = 0; g < NG; ++g) if (on[g]) dxr[g * 32 + lane] = make_float4(0.f, 0.f, 0.f, 0.f);
             continue;
         }
-        const long long bag = row / L;
+        const long long bag = PACKED ? bag_of_row<true>(a, row) : row / L;
+        const long long drow = dropout_row<PACKED>(a, row, bag);
         const float4 *xr = reinterpret_cast<const float4 *>(b.x_stash + row * H);
         const float4 *gvp = reinterpret_cast<const float4 *>(b.d_cv + bag * H), *cvp = reinterpret_cast<const float4 *>(b.cv + bag * H);
         float x[MAXC], gv[MAXC], cvv[MAXC];
@@ -369,7 +385,7 @@ backward_rows_lite_kernel(const EncodeArgs a, const BackwardArgs b)
 #pragma unroll
         for (int g = 0; g < NG; ++g) {
             uint4 bits = make_uint4(0u, 0u, 0u, 0u);
-            if (on[g] && a.drop_p > 0.0f) bits = dropout_bits(a.seed, row, g * 32 + lane);
+            if (on[g] && a.drop_p > 0.0f) bits = dropout_bits(a.seed, drow, g * 32 + lane);
             const float gam[4] = {g4[g].x, g4[g].y, g4[g].z, g4[g].w}, bet[4] = {b4[g].x, b4[g].y, b4[g].z, b4[g].w};
             const unsigned bw[4] = {bits.x, bits.y, bits.z, bits.w};
 #pragma unroll
@@ -513,12 +529,18 @@ backward_dw_kernel(const EncodeArgs a, const float *__restrict__ dx, float *__re
     }
 }
 
+// N context rows; a packed batch adds its row -> bag map (int32 [N]) at the end
+size_t encode_backward_workspace_bytes_n(const c2v_dims *d, int B, long long N, bool packed)
+{
+    const size_t H = d->encode, D = 2 * (size_t)d->terminal_embed + d->path_embed;
+    const size_t Hs = (H + 3) / 4 * 4;
+    return align_up((size_t)N * H * 4, 1024) + align_up((size_t)B * 4, 1024) + align_up(D * Hs * 4, 1024) + 1024 +   // 1 KB: dx absmax word
+           align_up(backward_dc_tc_workspace_bytes(), 1024) + (packed ? align_up((size_t)N * 4, 1024) : 0);
+}
+
 size_t encode_backward_workspace_bytes(const c2v_dims *d, int B, int L)
 {
-    const size_t N = (size_t)B * L, H = d->encode, D = 2 * (size_t)d->terminal_embed + d->path_embed;
-    const size_t Hs = (H + 3) / 4 * 4;
-    return align_up(N * H * 4, 1024) + align_up((size_t)B * 4, 1024) + align_up(D * Hs * 4, 1024) + 1024 +   // 1 KB: dx absmax word
-           align_up(backward_dc_tc_workspace_bytes(), 1024);
+    return encode_backward_workspace_bytes_n(d, B, (long long)B * L, false);
 }
 
 int launch_encode_backward(const c2v_dims *d, const c2v_params *p, const EncodeArgs &a_in, int B,
@@ -535,8 +557,10 @@ int launch_encode_backward(const c2v_dims *d, const c2v_params *p, const EncodeA
         set_error("encode backward supports encode_size <= %d (got %d)", 32 * MAXC, a.H);
         return C2V_EUNSUPPORTED;
     }
-    if (ws_bytes < encode_backward_workspace_bytes(d, B, a.L)) {
-        set_error("backward workspace too small: %zu < %zu", ws_bytes, encode_backward_workspace_bytes(d, B, a.L));
+    const bool packed = a.bag_off != nullptr;
+    const size_t need = encode_backward_workspace_bytes_n(d, B, a.N, packed);
+    if (ws_bytes < need) {
+        set_error("backward workspace too small: %zu < %zu", ws_bytes, need);
         return C2V_EWORKSPACE;
     }
     const int Hs = (a.H + 3) / 4 * 4;
@@ -546,7 +570,8 @@ int launch_encode_backward(const c2v_dims *d, const c2v_params *p, const EncodeA
     float *sb = reinterpret_cast<float *>(base + o); o += align_up((size_t)B * 4, 1024);
     float *w_t = reinterpret_cast<float *>(base + o); o += align_up((size_t)a.D * Hs * 4, 1024);
     unsigned *dx_absmax = reinterpret_cast<unsigned *>(base + o); o += 1024;
-    void *dc_ws = base + o;
+    void *dc_ws = base + o; o += align_up(backward_dc_tc_workspace_bytes(), 1024);
+    int *row_bag = packed ? reinterpret_cast<int *>(base + o) : nullptr;
     {
         const char *dc_env0 = getenv("C2V_BACKWARD_DC"), *dw_env0 = getenv("C2V_BACKWARD_DW");
         const bool split_ok = x_stash && (a.H & 3) == 0 && backward_dc_tc_ok(a) && backward_dw_tc_ok(a) &&
@@ -567,6 +592,11 @@ int launch_encode_backward(const c2v_dims *d, const c2v_params *p, const EncodeA
 
     int rc = launch_transpose_w(p->input_linear, w_t, a.H, a.D, Hs, st);
     if (rc != C2V_OK) return rc;
+    if (packed) {
+        rc = launch_row_bag(a.bag_off, B, a.N, row_bag, st);
+        if (rc != C2V_OK) return rc;
+        a.row_bag = row_bag;
+    }
     BackwardArgs b;
     b.cv = cv; b.att = attention; b.d_cv = d_cv; b.d_att = d_att; b.sb = nullptr; b.x_stash = x_stash; b.dx_absmax = dx_absmax;
     // dC = dX . W and dW = dX^T . C run on the tensor cores when the shape allows; C2V_BACKWARD_DC / _DW = ffma force CUDA cores
@@ -576,7 +606,11 @@ int launch_encode_backward(const c2v_dims *d, const c2v_params *p, const EncodeA
     b.W = p->input_linear; b.dx = dx;
     b.g_emb_t = g->terminal_embedding; b.g_emb_p = g->path_embedding;
     b.g_attn = g->attention; b.g_ln_g = g->ln_weight; b.g_ln_b = g->ln_bias;
-    if (d_att) {
+    if (d_att && packed) {
+        bag_dot_packed_kernel<<<B, 32, 0, st>>>(attention, d_att, a.bag_off, a.N, sb);
+        C2V_LAUNCH_OK("bag_dot_packed_kernel");
+        b.sb = sb;
+    } else if (d_att) {
         bag_dot_kernel<<<B, 32, 0, st>>>(attention, d_att, a.L, sb);
         C2V_LAUNCH_OK("bag_dot_kernel");
         b.sb = sb;
@@ -597,8 +631,8 @@ int launch_encode_backward(const c2v_dims *d, const c2v_params *p, const EncodeA
     C2V_CUDA_OK(cudaGetDevice(&dev));
     C2V_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     if (x_stash && dc_tc && (a.H & 3) == 0) {                  // no GEMM left in this kernel: one warp per row
-        if (a.H <= 128) backward_rows_lite_kernel<1><<<sms * 16, 256, 0, st>>>(a, b);
-        else backward_rows_lite_kernel<2><<<sms * 8, 256, 0, st>>>(a, b);
+        if (a.H <= 128) (packed ? backward_rows_lite_kernel<1, true> : backward_rows_lite_kernel<1>)<<<sms * 16, 256, 0, st>>>(a, b);
+        else (packed ? backward_rows_lite_kernel<2, true> : backward_rows_lite_kernel<2>)<<<sms * 8, 256, 0, st>>>(a, b);
         C2V_LAUNCH_OK("backward_rows_lite_kernel");
         if (phase == 1) {                                       // path sub-vector + dW; start / end follow in phase 2
             rc = launch_backward_dc_tc(a, p->input_linear, dx, dx_absmax, dc_ws, g->terminal_embedding, g->path_embedding, st, 2, true);
@@ -614,7 +648,8 @@ int launch_encode_backward(const c2v_dims *d, const c2v_params *p, const EncodeA
         goto dw_ffma;
     }
     {
-    auto kern = vec ? backward_rows_kernel<true> : backward_rows_kernel<false>;
+    auto kern = packed ? (vec ? backward_rows_kernel<true, true> : backward_rows_kernel<false, true>)
+                       : (vec ? backward_rows_kernel<true> : backward_rows_kernel<false>);
     C2V_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     int occ = 1;
     C2V_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, THREADS, smem));

@@ -39,19 +39,27 @@ __device__ __forceinline__ int bb_block_scan(int flag, int *s_warp, int *total) 
     return before + in_warp;
 }
 
+// PACKED: bag b goes to rows bag_off[b] .. bag_off[b+1]-1 (its length: min(n, L), 1 for an empty or unknown item)
+// instead of row b of the [B, L] tensors; the same contexts, without the zero suffix.
+template <bool PACKED = false>
 __global__ void __launch_bounds__(256)
 build_batch_kernel(const long long *__restrict__ offsets, const int *__restrict__ ctx, long long n_items,
                    const long long *__restrict__ item_ids, const long long *__restrict__ item_labels, int L,
                    unsigned long long seed, long long method_token, long long question_token,
                    long long *__restrict__ starts, long long *__restrict__ paths, long long *__restrict__ ends,
-                   long long *__restrict__ label)
+                   long long *__restrict__ label, const long long *__restrict__ bag_off)
 {
     __shared__ unsigned hist[256];
     __shared__ int s_warp[8];
     __shared__ unsigned s_prefix, s_k;
     const int b = blockIdx.x, tid = threadIdx.x;
     const long long item = item_ids[b];
-    long long *rs = starts + (size_t)b * L, *rp = paths + (size_t)b * L, *re = ends + (size_t)b * L;
+    const long long row0 = PACKED ? bag_off[b] : (long long)b * L;
+    long long *rs = starts + row0, *rp = paths + row0, *re = ends + row0;
+    if (PACKED) {                                            // the host-computed length, clamped into [0, L]
+        const long long len = bag_off[b + 1] - row0;
+        L = len < 0 ? 0 : (len > L ? L : (int)len);
+    }
     if (item < 0 || item >= n_items) {                      // not a method of this corpus: an all-pad bag
         for (int j = tid; j < L; j += 256) { rs[j] = 0; rp[j] = 0; re[j] = 0; }
         if (label && tid == 0) label[b] = 0;
@@ -251,8 +259,26 @@ extern "C" int c2v_build_batch(const int64_t *offsets, const int32_t *contexts, 
         reinterpret_cast<const long long *>(offsets), contexts, n_items, reinterpret_cast<const long long *>(item_ids),
         reinterpret_cast<const long long *>(item_labels), L, seed, method_token, question_token,
         reinterpret_cast<long long *>(starts), reinterpret_cast<long long *>(paths), reinterpret_cast<long long *>(ends),
-        reinterpret_cast<long long *>(label));
+        reinterpret_cast<long long *>(label), nullptr);
     C2V_LAUNCH_OK("build_batch_kernel");
+    return C2V_OK;
+}
+
+extern "C" int c2v_build_batch_packed(const int64_t *offsets, const int32_t *contexts, int64_t n_items,
+                                      const int64_t *item_ids, const int64_t *item_labels, int32_t B, int32_t L,
+                                      uint64_t seed, int64_t method_token, int64_t question_token, const int64_t *bag_offsets,
+                                      int64_t *starts, int64_t *paths, int64_t *ends, int64_t *label, void *stream)
+{
+    if (!offsets || !contexts || !item_ids || !bag_offsets || !starts || !paths || !ends || n_items < 1 || B < 1 || L < 1) {
+        set_error("c2v_build_batch_packed: bad argument (NULL pointer, n_items < 1, B < 1 or L < 1)");
+        return C2V_EINVAL;
+    }
+    build_batch_kernel<true><<<(unsigned)B, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        reinterpret_cast<const long long *>(offsets), contexts, n_items, reinterpret_cast<const long long *>(item_ids),
+        reinterpret_cast<const long long *>(item_labels), L, seed, method_token, question_token,
+        reinterpret_cast<long long *>(starts), reinterpret_cast<long long *>(paths), reinterpret_cast<long long *>(ends),
+        reinterpret_cast<long long *>(label), reinterpret_cast<const long long *>(bag_offsets));
+    C2V_LAUNCH_OK("build_batch_kernel<packed>");
     return C2V_OK;
 }
 

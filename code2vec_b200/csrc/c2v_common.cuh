@@ -84,8 +84,10 @@ struct EncodeWorkspace {
     size_t bytes;
 };
 // Partial slot of (tile t, bag b): t + b.  Walking the context rows in order, each new
-// (tile, bag) pair increments t or b (or both), so t + b is unique; needs n_tiles + B slots.
+// (tile, bag) pair increments t or b (or both), so t + b is unique; needs n_tiles + B slots.  This holds for packed
+// batches as well (rows and bags still increase together), with n_tiles counted over their N rows.
 EncodeWorkspace carve_encode_workspace(const c2v_dims *d, int B, int L, void *base);
+EncodeWorkspace carve_encode_workspace_n(const c2v_dims *d, int B, long long N, void *base, int **row_bag);
 
 struct EncodeArgs {
     const long long *starts, *paths, *ends;
@@ -102,7 +104,39 @@ struct EncodeArgs {
     float *stash_x;         // optional [N, H]: x = c . W^T (model.py:54) of every row, kept for the backward
     int flags;              // debug switches
     EncodeWorkspace ws;
+    // packed (CSR) batches only, NULL for [B, L] ones: bag b owns rows bag_off[b] .. bag_off[b+1]-1 (1 <= length <= L),
+    // row_bag [N] maps a row to its bag (built by launch_row_bag).  Kept behind every other field so that the padded
+    // kernels see the same parameter layout.
+    const long long *bag_off;
+    const int *row_bag;
+    int n_bags;
 };
+
+#ifdef __CUDACC__
+// Row -> bag, first row of a bag, and the Philox row counter of the dropout mask.  A packed context j of bag b draws the
+// counter b * L + j: the counter the same context has in the [B, L] layout, so both layouts share one mask.
+template <bool PACKED>
+__device__ __forceinline__ long long bag_of_row(const EncodeArgs &a, long long row)
+{
+    if (!PACKED) return row / a.L;
+    long long b = a.row_bag[row];
+    return b < 0 ? 0 : (b >= a.n_bags ? a.n_bags - 1 : b);
+}
+template <bool PACKED>
+__device__ __forceinline__ long long bag_first_row(const EncodeArgs &a, long long bag)
+{
+    if (!PACKED) return bag * a.L;
+    bag = bag < 0 ? 0 : (bag > a.n_bags ? a.n_bags : bag);      // bag_off has n_bags + 1 entries
+    long long r = a.bag_off[bag];
+    return r < 0 ? 0 : (r > a.N ? a.N : r);
+}
+template <bool PACKED>
+__device__ __forceinline__ long long dropout_row(const EncodeArgs &a, long long row, long long bag)
+{
+    return PACKED ? bag * a.L + (row - bag_first_row<true>(a, bag)) : row;
+}
+#endif
+int launch_row_bag(const long long *bag_off, int B, long long N, int *row_bag, cudaStream_t st);
 
 int launch_prepare_weights(const c2v_dims *d, const float *W, EncodeWorkspace &ws, bool tcgen05,
                            cudaStream_t st);

@@ -42,7 +42,7 @@ int launch_transpose_w(const float *W, float *Wt, int H, int D, int Hs, cudaStre
 // ------------------------------------------------------------------------------------
 // K1a
 // ------------------------------------------------------------------------------------
-template <bool VEC>
+template <bool VEC, bool PACKED = false>
 __global__ void __launch_bounds__(THREADS)
 encode_ffma_kernel(const EncodeArgs a, const int Hs)
 {
@@ -57,7 +57,7 @@ encode_ffma_kernel(const EncodeArgs a, const int Hs)
     float *mbuf = reinterpret_cast<float *>(smem + lay.m);
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int H = a.H, L = a.L;
+    const int H = a.H;
 
     for (int tile = blockIdx.x; tile < a.n_tiles; tile += gridDim.x) {
         const long long row0 = (long long)tile * TM;
@@ -82,10 +82,11 @@ encode_ffma_kernel(const EncodeArgs a, const int Hs)
             float v = 0.0f;
             for (int c = lane; c < H; c += 32) { const float d = xr[c] - mean; v = fmaf(d, d, v); }
             const float rstd = 1.0f / sqrtf(warp_sum(v) / (float)H + C2V_LN_EPS);
+            const long long drow = (PACKED && row < a.N) ? dropout_row<true>(a, row, bag_of_row<true>(a, row)) : row;
             float u = 0.0f;
             for (int c = lane; c < H; c += 32) {
                 float y = tanh_accurate((xr[c] - mean) * rstd * a.ln_g[c] + a.ln_b[c]);
-                if (a.drop_p > 0.0f) y *= dropout_mask_at(a.seed, row, c, a.drop_p, a.drop_scale);
+                if (a.drop_p > 0.0f) y *= dropout_mask_at(a.seed, drow, c, a.drop_p, a.drop_scale);
                 xr[c] = y;
                 u = fmaf(y, a.attn[c], u);
             }
@@ -103,19 +104,19 @@ encode_ffma_kernel(const EncodeArgs a, const int Hs)
         const int rows_here = (int)((a.N - row0) < TM ? (a.N - row0) : TM);
         if (tid < rows_here) {
             const long long row = row0 + tid;
-            const long long bag = row / L;
-            long long lo = bag * L - row0; if (lo < 0) lo = 0;
-            long long hi = (bag + 1) * L - row0; if (hi > rows_here) hi = rows_here;
+            const long long bag = bag_of_row<PACKED>(a, row);
+            long long lo = bag_first_row<PACKED>(a, bag) - row0; if (lo < 0) lo = 0;
+            long long hi = bag_first_row<PACKED>(a, bag + 1) - row0; if (hi > rows_here) hi = rows_here;
             float m = C2V_NINF;
             for (int q = (int)lo; q < (int)hi; ++q) m = fmaxf(m, zbuf[q]);
             mbuf[tid] = m;
             ebuf[tid] = __expf(zbuf[tid] - m);
         }
         __syncthreads();
-        const long long bag_first = row0 / L, bag_last = (row0 + rows_here - 1) / L;
+        const long long bag_first = bag_of_row<PACKED>(a, row0), bag_last = bag_of_row<PACKED>(a, row0 + rows_here - 1);
         for (long long bag = bag_first; bag <= bag_last; ++bag) {
-            long long lo = bag * L - row0; if (lo < 0) lo = 0;
-            long long hi = (bag + 1) * L - row0; if (hi > rows_here) hi = rows_here;
+            long long lo = bag_first_row<PACKED>(a, bag) - row0; if (lo < 0) lo = 0;
+            long long hi = bag_first_row<PACKED>(a, bag + 1) - row0; if (hi > rows_here) hi = rows_here;
             const size_t slot = (size_t)tile + (size_t)bag;
             for (int h = tid; h < H; h += THREADS) {
                 float v = 0.0f;
@@ -145,7 +146,8 @@ int launch_encode_ffma(const EncodeArgs &a, cudaStream_t st)
         set_error("encode_ffma: encode_size %d needs %d B of shared memory (> 227 KB)", a.H, lay.total);
         return C2V_EUNSUPPORTED;
     }
-    auto kern = vec ? encode_ffma_kernel<true> : encode_ffma_kernel<false>;
+    auto kern = a.bag_off ? (vec ? encode_ffma_kernel<true, true> : encode_ffma_kernel<false, true>)
+                          : (vec ? encode_ffma_kernel<true> : encode_ffma_kernel<false>);
     C2V_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, lay.total));
     int occ = 1;
     C2V_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, THREADS, lay.total));
@@ -160,6 +162,7 @@ int launch_encode_ffma(const EncodeArgs &a, cudaStream_t st)
 // ------------------------------------------------------------------------------------
 // K1f: merge the (tile, bag) partials of every bag (model.py:96 softmax, :68-69 sum)
 // ------------------------------------------------------------------------------------
+template <bool PACKED = false>
 __global__ void __launch_bounds__(128)
 encode_finalize_kernel(const EncodeArgs a, const int tile_rows, float *__restrict__ code_vector)
 {
@@ -178,8 +181,9 @@ encode_finalize_kernel(const EncodeArgs a, const int tile_rows, float *__restric
             __threadfence_system();
         }
     }
-    const int L = a.L, H = a.H;
-    const long long r0 = bag * L;
+    // L: the rows of this bag (every row of it in a [B, L] batch)
+    const int L = PACKED ? (int)(bag_first_row<true>(a, bag + 1) - bag_first_row<true>(a, bag)) : a.L, H = a.H;
+    const long long r0 = bag_first_row<PACKED>(a, bag);
     const int t0 = (int)(r0 / tile_rows), t1 = (int)((r0 + L - 1) / tile_rows);
     const int np = t1 - t0 + 1;
     const size_t slot0 = (size_t)t0 + bag;
@@ -243,9 +247,31 @@ encode_finalize_kernel(const EncodeArgs a, const int tile_rows, float *__restric
     }
 }
 
+// ------------------------------------------------------------------------------------
+// packed batches: row_bag[r] = the bag of context row r (one warp per bag; offsets clamped into [0, N])
+// ------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+row_bag_kernel(const long long *__restrict__ off, int B, long long N, int *__restrict__ row_bag)
+{
+    const int bag = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (bag >= B) return;
+    long long lo = off[bag], hi = off[bag + 1];
+    lo = lo < 0 ? 0 : (lo > N ? N : lo);
+    hi = hi < lo ? lo : (hi > N ? N : hi);
+    for (long long r = lo + lane; r < hi; r += 32) row_bag[r] = bag;
+}
+
+int launch_row_bag(const long long *bag_off, int B, long long N, int *row_bag, cudaStream_t st)
+{
+    row_bag_kernel<<<(unsigned)((B + 7) / 8), 256, 0, st>>>(bag_off, B, N, row_bag);
+    C2V_LAUNCH_OK("row_bag_kernel");
+    return C2V_OK;
+}
+
 int launch_encode_finalize(const EncodeArgs &a, int B, float *code_vector, cudaStream_t st)
 {
-    C2V_CUDA_OK(launch_pdl(encode_finalize_kernel, dim3((unsigned)B), dim3(128), 0, st, a, a.ws.tile_rows, code_vector));
+    C2V_CUDA_OK(launch_pdl(a.bag_off ? encode_finalize_kernel<true> : encode_finalize_kernel<false>, dim3((unsigned)B), dim3(128), 0,
+                           st, a, a.ws.tile_rows, code_vector));
     C2V_LAUNCH_OK("encode_finalize_kernel");
     return C2V_OK;
 }

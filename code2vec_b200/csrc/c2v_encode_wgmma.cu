@@ -133,7 +133,7 @@ int launch_split_w_tcgen05(const c2v_dims *d, const float *W, EncodeWorkspace &w
 // ------------------------------------------------------------------------------------
 // the kernel
 // ------------------------------------------------------------------------------------
-template <bool DROPOUT, int HV>
+template <bool DROPOUT, int HV, bool PACKED = false>
 __global__ void __launch_bounds__(WgCfg<(HV > 128)>::THREADS, 1)
 encode_wgmma_kernel(const EncodeArgs a)
 {
@@ -210,13 +210,14 @@ encode_wgmma_kernel(const EncodeArgs a)
 
             // ---- epilogue.  Fragment layout of the m64 accumulator: acc[4j + 2h + b] is row 16 w4 + lane/4 + 8h of
             //      this warpgroup's 64 rows, column 8j + 2 (lane & 3) + b.  A row's columns live in one lane quad.
-            long long row[2];
+            long long row[2], bag_r[2] = {0, 0};
             bool in_range[2];
             float nrm[2], shift[2];
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 row[h] = (long long)tile * C::ROWS + 64 * g + 16 * w4 + (lane >> 2) + 8 * h;
                 in_range[h] = row[h] < a.N;
+                if (PACKED) bag_r[h] = in_range[h] ? bag_of_row<true>(a, row[h]) : 0;     // rows past N: any valid bag, unused
                 // LayerNorm (model.py:55-56), one pass: sum and sum of squares together; padding columns are exactly 0.
                 // var = E[x^2] - mean^2 in fp32: relative error ~2^-24 (1 + mean^2 / var), far inside the 1e-4 budget.
                 float s = 0.f, q = 0.f;
@@ -259,7 +260,7 @@ encode_wgmma_kernel(const EncodeArgs a)
                     float y0 = tanh_from_scaled(fmaf(fmaf(acc[4 * j + 2 * h], nrm[h], shift[h]), gm.x, bt.x));
                     float y1 = tanh_from_scaled(fmaf(fmaf(acc[4 * j + 2 * h + 1], nrm[h], shift[h]), gm.y, bt.y));
                     if (DROPOUT) {
-                        const uint4 bits = dropout_bits(a.seed, row[h], c >> 2);
+                        const uint4 bits = dropout_bits(a.seed, PACKED ? dropout_row<true>(a, row[h], bag_r[h]) : row[h], c >> 2);
                         y0 *= dropout_mul((m4 & 1) ? bits.z : bits.x, a.drop_p, a.drop_scale);
                         y1 *= dropout_mul((m4 & 1) ? bits.w : bits.y, a.drop_p, a.drop_scale);
                     }
@@ -282,9 +283,11 @@ encode_wgmma_kernel(const EncodeArgs a)
             if (vrow0 < a.N) {
                 const long long vt = vrow0 / C::VROWS;
                 long long last = vrow0 + C::VROWS - 1; if (last > a.N - 1) last = a.N - 1;
-                const long long bag_lo = vrow0 / a.L, bag_hi = last / a.L;
+                // packed: up to 16 bags per slice (one per row); every bag in [bag_lo, bag_hi] has a row here (lengths >= 1)
+                const long long bag_lo = bag_of_row<PACKED>(a, vrow0), bag_hi = bag_of_row<PACKED>(a, last);
                 for (long long bag = bag_lo; bag <= bag_hi; ++bag) {
-                    const bool seg0 = in_range[0] && row[0] / a.L == bag, seg1 = in_range[1] && row[1] / a.L == bag;
+                    const bool seg0 = in_range[0] && (PACKED ? bag_r[0] : row[0] / a.L) == bag;
+                    const bool seg1 = in_range[1] && (PACKED ? bag_r[1] : row[1] / a.L) == bag;
                     const float m = warp_max(fmaxf(seg0 ? z[0] : -INFINITY, seg1 ? z[1] : -INFINITY));
                     const float e0 = seg0 ? __expf(z[0] - m) : 0.0f, e1 = seg1 ? __expf(z[1] - m) : 0.0f;
                     const size_t slot = (size_t)(vt + bag);
@@ -395,14 +398,23 @@ static int launch_wg(void (*kern)(const EncodeArgs), const EncodeArgs &a, cudaSt
     return C2V_OK;
 }
 
-int launch_encode_tcgen05(const EncodeArgs &a, cudaStream_t st)
+template <bool PACKED>
+static int launch_encode_wg(const EncodeArgs &a, cudaStream_t st)
 {
     const bool drop = a.drop_p > 0.0f;
-    if (a.H == 256) return launch_wg<true>(drop ? encode_wgmma_kernel<true, 256> : encode_wgmma_kernel<false, 256>, a, st);
-    if (a.H == 128) return launch_wg<false>(drop ? encode_wgmma_kernel<true, 128> : encode_wgmma_kernel<false, 128>, a, st);
-    if (a.H == 100) return launch_wg<false>(drop ? encode_wgmma_kernel<true, 100> : encode_wgmma_kernel<false, 100>, a, st);
+    if (a.H == 256)
+        return launch_wg<true>(drop ? encode_wgmma_kernel<true, 256, PACKED> : encode_wgmma_kernel<false, 256, PACKED>, a, st);
+    if (a.H == 128)
+        return launch_wg<false>(drop ? encode_wgmma_kernel<true, 128, PACKED> : encode_wgmma_kernel<false, 128, PACKED>, a, st);
+    if (a.H == 100)
+        return launch_wg<false>(drop ? encode_wgmma_kernel<true, 100, PACKED> : encode_wgmma_kernel<false, 100, PACKED>, a, st);
     set_error("encode_wgmma_kernel: encode_size %d not supported (100, 128 or 256)", a.H);
     return C2V_EUNSUPPORTED;
+}
+
+int launch_encode_tcgen05(const EncodeArgs &a, cudaStream_t st)
+{
+    return a.bag_off ? launch_encode_wg<true>(a, st) : launch_encode_wg<false>(a, st);
 }
 
 }  // namespace c2v

@@ -149,6 +149,120 @@ def encode_forward(dims, params, starts, paths, ends, drop_p=0.0, training=False
     return cv, att
 
 
+class PackedBags:
+    """A batch of variable-length bags in CSR form, without padding rows: bag b is contexts offsets[b] .. offsets[b+1]-1
+    of starts / paths / ends (int64 [N]).  Bag b is row b of the [B, L] batch without its zero-padded suffix, so every bag
+    holds 1 .. max_path_length contexts; a method with no contexts is a bag of one pad context (0, 0, 0).
+
+    The offsets (int64 [B + 1]) are validated on the host here -- offsets[0] = 0, non-decreasing, offsets[B] = N, every
+    bag length in [1, max_path_length] -- so that no malformed batch reaches a kernel.  Given as a host tensor / array /
+    list that costs nothing; given as a CUDA tensor it costs one device-to-host copy (and a synchronisation).
+    DeviceCorpus.build_packed computes them on the host and never pays it.
+
+    device_offsets: the same offsets already on the device of starts (no upload then); the caller guarantees that they hold
+    the values of `offsets`, which are the ones validated.
+
+    Attributes: starts / paths / ends [N] and offsets [B + 1] on the device of starts; offsets_host (numpy int64), B, N,
+    L (= max_path_length)."""
+
+    def __init__(self, starts, paths, ends, offsets, max_path_length, device_offsets=None):
+        import numpy as np
+        L = int(max_path_length)
+        if L < 1:
+            raise ValueError(f"PackedBags: max_path_length = {L} < 1")
+        if isinstance(offsets, torch.Tensor):
+            host = offsets.detach().to("cpu", torch.int64).numpy()
+        else:
+            host = np.asarray(offsets, dtype=np.int64)
+        host = np.ascontiguousarray(host, dtype=np.int64)
+        for name, t in (("starts", starts), ("paths", paths), ("ends", ends)):
+            if not isinstance(t, torch.Tensor) or t.dim() != 1:
+                raise ValueError(f"PackedBags: {name} must be a 1-D int64 tensor [N]")
+        N = int(starts.numel())
+        if paths.numel() != N or ends.numel() != N:
+            raise ValueError(f"PackedBags: starts / paths / ends hold {N} / {paths.numel()} / {ends.numel()} contexts")
+        if host.ndim != 1 or host.size < 2:
+            raise ValueError("PackedBags: offsets must be 1-D with B + 1 >= 2 entries")
+        if host[0] != 0 or host[-1] != N:
+            raise ValueError(f"PackedBags: offsets[0] = {host[0]} and offsets[B] = {host[-1]} must be 0 and N = {N}")
+        n = np.diff(host)
+        if (n < 1).any() or (n > L).any():
+            b = int(np.flatnonzero((n < 1) | (n > L))[0])
+            raise ValueError(f"PackedBags: bag {b} holds {int(n[b])} contexts; every bag needs 1 .. {L} "
+                             "(offsets must increase)")
+        self.starts = _idx(starts, "starts"); self.paths = _idx(paths, "paths"); self.ends = _idx(ends, "ends")
+        self.offsets_host = host
+        if device_offsets is not None:
+            if device_offsets.dtype != torch.int64 or device_offsets.device != starts.device or \
+                    tuple(device_offsets.shape) != host.shape:
+                raise ValueError("PackedBags: device_offsets must be int64 [B + 1] on the device of starts")
+            self.offsets = device_offsets.contiguous()
+        elif isinstance(offsets, torch.Tensor):
+            self.offsets = offsets.to(device=starts.device, dtype=torch.int64).contiguous()
+        else:
+            self.offsets = torch.from_numpy(host.copy()).to(starts.device)
+        self.B, self.N, self.L = int(host.size - 1), N, L
+
+    @property
+    def device(self):
+        return self.starts.device
+
+    def lengths(self):
+        """host numpy int64 [B]: contexts per bag"""
+        import numpy as np
+        return np.diff(self.offsets_host)
+
+    def padded(self):
+        """-> (starts, paths, ends) int64 [B, L] on the device: the same batch with a zero-padded suffix per bag"""
+        import numpy as np
+        n = self.lengths()
+        rows = np.repeat(np.arange(self.B), n)
+        cols = np.arange(self.N) - np.repeat(self.offsets_host[:-1], n)
+        flat = torch.from_numpy(rows * self.L + cols).to(self.device)
+        out = []
+        for t in (self.starts, self.paths, self.ends):
+            p = torch.zeros(self.B * self.L, dtype=torch.int64, device=self.device)
+            p[flat] = t
+            out.append(p.view(self.B, self.L))
+        return tuple(out)
+
+
+def encode_forward_packed(dims, params, bags, drop_p=0.0, training=False, seed=0, algo=_lib.ALGO_AUTO,
+                          check_indices=False, cache=None, weight=None, stash=False):
+    """encode_forward for a PackedBags batch -> (code_vector [B,H], attention [N]) (+ x_stash [N, H] with stash=True).
+    The code vector of a bag equals the [B, L] result of the same bag up to fp32 summation order; packed context j of bag
+    b draws the dropout mask of padded row b * L + j."""
+    lib = _lib.load()
+    _need_cuda(bags.starts, bags.paths, bags.ends, bags.offsets)
+    B, N, L = bags.B, bags.N, bags.L
+    dev = bags.device
+    with torch.cuda.device(dev):
+        cv = _empty((B, dims.encode), torch.float32, dev)
+        att = _empty((N,), torch.float32, dev)
+        nbytes = lib.c2v_encode_packed_workspace_bytes(ctypes.byref(dims), B, N)
+        if cache is not None and weight is not None:
+            ws, reuse = cache.get(nbytes, dev, weight)
+            if reuse:
+                algo = int(algo) | REUSE_PREP
+        else:
+            ws = _empty((nbytes,), torch.uint8, dev)
+        drop = Dropout(float(drop_p), 1 if training else 0, int(seed))
+        xs = _empty((N, dims.encode), torch.float32, dev) if stash else None
+        rc = lib.c2v_encode_forward_packed(ctypes.byref(dims), ctypes.byref(params), _ptr(bags.starts), _ptr(bags.paths),
+                                           _ptr(bags.ends), _ptr(bags.offsets), B, N, L, ctypes.byref(drop), _ptr(cv),
+                                           _ptr(att), _ptr(xs), _ptr(ws), ws.numel(), int(algo), _stream(dev))
+        _lib.check(rc, "c2v_encode_forward_packed")
+        if check_indices:
+            bad = lib.c2v_workspace_status(_ptr(ws), _stream(dev))
+            if bad > 0:
+                raise IndexError("index out of range in self")
+            if bad < 0:
+                _lib.check(int(bad), "c2v_workspace_status")
+    if stash:
+        return cv, att, xs
+    return cv, att
+
+
 def _label_ws(dims, B, dev, algo, cache, weight, nbytes=None, absmax_ready=False, fresh=True):
     """-> (workspace, algo with its flags) of a label-head call.  With a cache (and its weight, W_out) the cache's persistent
     workspace, plus REUSE_PREP while its W_out image is current and GRAD_ABSMAX_READY if absmax_ready.  Without one a fresh
@@ -466,6 +580,33 @@ def encode_backward(dims, params, starts, paths, ends, cv, att, d_cv, d_att, sha
                                                 _ptr(d_cv), _ptr(d_att), ctypes.byref(grads),
                                                 _ptr(ws), nbytes, phase, _stream(dev))
             _lib.check(rc, "c2v_encode_backward")
+            if phase == 1:
+                between_phases()
+    return g
+
+
+def encode_backward_packed(dims, params, bags, cv, att, d_cv, d_att, shapes, drop_p=0.0, training=False, seed=0,
+                           grads_out=None, x_stash=None, between_phases=None):
+    """encode_backward for a PackedBags batch: att / d_att [N], x_stash [N, H] from encode_forward_packed(stash=True)."""
+    lib = _lib.load()
+    B, N, L = bags.B, bags.N, bags.L
+    dev = bags.device
+    with torch.cuda.device(dev):
+        g = grads_out or {k: torch.zeros(s, dtype=torch.float32, device=dev) for k, s in shapes.items()}
+        grads = Grads(_ptr(g["terminal_embedding"]), _ptr(g["path_embedding"]), _ptr(g["input_linear"]),
+                      _ptr(g["ln_weight"]), _ptr(g["ln_bias"]), _ptr(g["attention"]))
+        nbytes = lib.c2v_encode_backward_packed_workspace_bytes(ctypes.byref(dims), B, N)
+        ws = _empty((nbytes,), torch.uint8, dev)
+        drop = Dropout(float(drop_p), 1 if training else 0, int(seed))
+        cv = _f32c(cv, "code_vector"); att = _f32c(att, "attention")
+        d_cv = _f32c(d_cv, "d_code_vector")
+        d_att = _f32c(d_att, "d_attention") if d_att is not None else None
+        for phase in ((1, 2) if between_phases is not None else (0,)):
+            rc = lib.c2v_encode_backward_packed(ctypes.byref(dims), ctypes.byref(params), _ptr(bags.starts), _ptr(bags.paths),
+                                                _ptr(bags.ends), _ptr(bags.offsets), B, N, L, ctypes.byref(drop), _ptr(cv),
+                                                _ptr(att), _ptr(x_stash), _ptr(d_cv), _ptr(d_att), ctypes.byref(grads),
+                                                _ptr(ws), nbytes, phase, _stream(dev))
+            _lib.check(rc, "c2v_encode_backward_packed")
             if phase == 1:
                 between_phases()
     return g

@@ -39,8 +39,15 @@ class _EncodeFn(torch.autograd.Function):
         # when a gradient will be asked for, keep x = c . W^T (105 MB per 1024 x 200 batch at encode_size 128) so that
         # the backward neither re-gathers the embedding rows nor redoes the input_linear GEMM
         stash = any(ctx.needs_input_grad[:6]) and os.environ.get("C2V_NO_STASH", "0") != "1"
-        res = CF.encode_forward(dims, params, starts, paths, ends, drop_p, training, seed, algo,
-                                cache=cache, weight=W, stash=stash)
+        # a PackedBags batch comes in the `starts` position (paths = ends = None); its attention is [N]
+        ctx.bags = starts if isinstance(starts, CF.PackedBags) else None
+        if ctx.bags is not None:
+            res = CF.encode_forward_packed(dims, params, ctx.bags, drop_p, training, seed, algo, cache=cache, weight=W,
+                                           stash=stash)
+            starts = None
+        else:
+            res = CF.encode_forward(dims, params, starts, paths, ends, drop_p, training, seed, algo,
+                                    cache=cache, weight=W, stash=stash)
         cv, att = res[0], res[1]
         ctx.x_stash = res[2] if stash else None
         ctx.save_for_backward(emb_t, emb_p, W, ln_g, ln_b, attn, starts, paths, ends, cv, att)
@@ -73,8 +80,12 @@ class _EncodeFn(torch.autograd.Function):
             for k in ("ln_weight", "ln_bias", "attention"):
                 grads_out[k] = torch.empty(shapes[k], dtype=torch.float32, device=cv.device)   # overwritten by the kernels
         hook = getattr(ctx.cache, "on_path_grads_ready", None) if fuse else None
-        g = CF.encode_backward(dims, params, starts, paths, ends, cv, att, d_cv, d_att, shapes, drop_p, training, seed,
-                               grads_out=grads_out, x_stash=ctx.x_stash, between_phases=hook)
+        if ctx.bags is not None:
+            g = CF.encode_backward_packed(dims, params, ctx.bags, cv, att, d_cv, d_att, shapes, drop_p, training, seed,
+                                          grads_out=grads_out, x_stash=ctx.x_stash, between_phases=hook)
+        else:
+            g = CF.encode_backward(dims, params, starts, paths, ends, cv, att, d_cv, d_att, shapes, drop_p, training, seed,
+                                   grads_out=grads_out, x_stash=ctx.x_stash, between_phases=hook)
         ctx.x_stash = None
         if fuse:
             return (None, None, None, g["ln_weight"], g["ln_bias"], g["attention"], None, None, None, None, None, None,
@@ -250,8 +261,12 @@ class Code2Vec(nn.Module):
         dims = self._dims()
         params = CF.make_params(self.terminal_embedding.weight, self.path_embedding.weight, self.input_linear.weight,
                                 self.input_layer_norm.weight, self.input_layer_norm.bias, self.attention_parameter)
-        code_vector, attention = CF.encode_forward(dims, params, starts, paths, ends, algo=self.algo,
-                                                   cache=self._enc_cache, weight=self.input_linear.weight)
+        if isinstance(starts, CF.PackedBags):
+            code_vector, attention = CF.encode_forward_packed(dims, params, starts, algo=self.algo, cache=self._enc_cache,
+                                                              weight=self.input_linear.weight)
+        else:
+            code_vector, attention = CF.encode_forward(dims, params, starts, paths, ends, algo=self.algo,
+                                                       cache=self._enc_cache, weight=self.input_linear.weight)
         return code_vector, attention, dims
 
     def _head_logits(self, code_vector, label, dims):
@@ -277,6 +292,9 @@ class Code2Vec(nn.Module):
         (`forward` itself raises it one call late, without synchronising: see functional.PrepCache.raise_deferred)."""
         self._enc_cache.raise_deferred(synchronize=True)
 
+    # Every entry point below also takes a functional.PackedBags batch in place of `starts`, with paths = ends = None: the
+    # encode then runs over its N contexts only (no padding rows), attention comes back as [N], aligned with the packed
+    # contexts, and the label heads run unchanged on the [b, H] code vectors.
     def forward(self, starts, paths, ends, label):
         code_vector, attention, dims = self._encode(starts, paths, ends)
         return self._head_logits(code_vector, label, dims), code_vector, attention
@@ -290,7 +308,7 @@ class Code2Vec(nn.Module):
         Shapes the fused kernel does not take, and algo="ffma", fall back to forward()'s head + eager log_softmax / NLL +
         torch.max."""
         code_vector, attention, dims = self._encode(starts, paths, ends)
-        if self.algo != _lib.ALGO_FFMA and CF.label_loss_supported(dims, starts.shape[0]):
+        if self.algo != _lib.ALGO_FFMA and CF.label_loss_supported(dims, code_vector.shape[0]):
             o = self.option
             angular = (o.angular_margin, o.inverse_temp) if o.angular_margin_loss else None
             loss, am, mx = _LabelLossFn.apply(code_vector, *self._head(), label, dims, self._label_algo, self._lab_cache,

@@ -153,6 +153,19 @@ int c2v_encode_forward_stash(const c2v_dims *d, const c2v_params *p, const int64
                              const c2v_dropout *drop, float *code_vector, float *attention, float *x_stash,
                              void *workspace, size_t workspace_bytes, int32_t algo, void *stream);
 
+/* Packed (CSR) batches: bag b is the N-row slice offsets[b] .. offsets[b+1]-1 of starts / paths / ends (int64 [N],
+ * device), offsets int64 [B + 1] (device) with offsets[0] = 0, offsets[B] = N and every bag 1 .. L contexts long: row b
+ * of a [B, L] batch without its zero-padded suffix.  No padding row is gathered, multiplied, stashed or back-propagated.
+ * code_vector [B, H]; attention [N], aligned with the packed contexts; x_stash [N, H] or NULL.  The mask rule is the
+ * same (starts > 0), and packed context j of bag b draws the dropout mask of row b * L + j -- the mask the same context
+ * has in the [B, L] layout at the same seed.  The offsets are not read on the host: the caller validates them.  Algo,
+ * flags, status word and status mirror as c2v_encode_forward_stash.  The workspace size depends on B and N only. */
+size_t c2v_encode_packed_workspace_bytes(const c2v_dims *d, int32_t B, int64_t N);
+int c2v_encode_forward_packed(const c2v_dims *d, const c2v_params *p, const int64_t *starts, const int64_t *paths,
+                              const int64_t *ends, const int64_t *offsets, int32_t B, int64_t N, int32_t L,
+                              const c2v_dropout *drop, float *code_vector, float *attention, float *x_stash,
+                              void *workspace, size_t workspace_bytes, int32_t algo, void *stream);
+
 /* Reads the status word of the last encode on this workspace (synchronises the
  * stream): returns the number of out-of-range indices seen, or a negative code. */
 int64_t c2v_workspace_status(void *workspace, void *stream);
@@ -311,6 +324,14 @@ int c2v_encode_backward_phased(const c2v_dims *d, const c2v_params *p, const int
                                const c2v_dropout *drop, const float *code_vector, const float *attention,
                                const float *x_stash, const float *d_code_vector, const float *d_attention,
                                const c2v_grads *grads, void *workspace, size_t workspace_bytes, int32_t phase, void *stream);
+/* c2v_encode_backward_phased for a packed batch (layout as c2v_encode_forward_packed): d_attention [N] or NULL,
+ * x_stash [N, H] or NULL. */
+size_t c2v_encode_backward_packed_workspace_bytes(const c2v_dims *d, int32_t B, int64_t N);
+int c2v_encode_backward_packed(const c2v_dims *d, const c2v_params *p, const int64_t *starts, const int64_t *paths,
+                               const int64_t *ends, const int64_t *offsets, int32_t B, int64_t N, int32_t L,
+                               const c2v_dropout *drop, const float *code_vector, const float *attention,
+                               const float *x_stash, const float *d_code_vector, const float *d_attention,
+                               const c2v_grads *grads, void *workspace, size_t workspace_bytes, int32_t phase, void *stream);
 
 /* ---- host-buffer call: what a reference-side caller with CPU tensors uses ----------
  * One whole Code2Vec.forward + torch.max for a batch held in HOST memory (pinned
@@ -349,6 +370,14 @@ int c2v_build_batch(const int64_t *offsets, const int32_t *contexts, int64_t n_i
                     const int64_t *item_ids, const int64_t *item_labels, int32_t B, int32_t L,
                     uint64_t seed, int64_t method_token, int64_t question_token, int64_t *starts,
                     int64_t *paths, int64_t *ends, int64_t *label, void *stream);
+/* The same bags as a packed batch: bag b goes to rows bag_offsets[b] .. bag_offsets[b+1]-1 of starts / paths / ends
+ * (int64 [N], device; bag_offsets int64 [B + 1], device).  The caller sizes bag b as min(n, L) contexts, n the item's
+ * context count, and as one context for an empty item or an id outside [0, n_items): that bag is one pad context
+ * (0, 0, 0).  Same selection as c2v_build_batch, so the result is its [B, L] batch without the zero suffix. */
+int c2v_build_batch_packed(const int64_t *offsets, const int32_t *contexts, int64_t n_items,
+                           const int64_t *item_ids, const int64_t *item_labels, int32_t B, int32_t L,
+                           uint64_t seed, int64_t method_token, int64_t question_token, const int64_t *bag_offsets,
+                           int64_t *starts, int64_t *paths, int64_t *ends, int64_t *label, void *stream);
 
 /* The variable-name task of the same builder (/root/reference/model/dataset_builder.py:152-204, `--infer_variable_name`):
  * a unit is an (item, @var_k alias) pair -- unit_item / unit_var (terminal index of @var_k) / unit_label [n_units], in the
