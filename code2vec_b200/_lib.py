@@ -98,6 +98,10 @@ SYMBOLS = {
                                        c_vp, c_vp, c_vp]),
     "c2v_build_batch_vars": (ctypes.c_int, [c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp, c_i32, c_i32, ctypes.c_uint64,
                                             c_i64, c_vp, c_i64, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "c2v_build_batch_vars_packed": (ctypes.c_int, [c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp, c_i32, c_i32,
+                                                   ctypes.c_uint64, c_i64, c_vp, c_i64, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp,
+                                                   c_vp, c_vp, c_vp]),
+    "c2v_count_unit_contexts": (ctypes.c_int, [c_vp, c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp]),
     "c2v_adam_step": (ctypes.c_int, [c_vp, c_vp, c_vp, c_vp, c_i64, c_f32, c_f32, c_f32, c_f32, c_f32, c_i64, c_f32, c_i32, c_vp]),
     "c2v_adam_step_sharded": (ctypes.c_int, [c_vp, c_vp, c_vp, _P(c_vp), _P(c_vp), c_i32, c_vp, c_vp, c_i64, c_i64, c_vp, c_i64,
                                              c_f32, c_f32, c_f32, c_f32, c_f32, c_i64, c_f32, c_vp]),
@@ -119,6 +123,10 @@ SYMBOLS = {
                                         c_vp, c_i32]),
     "c2v_forward_host_async": (ctypes.c_int, [c_vp, _P(Params), c_vp, c_vp, c_vp, c_vp, c_i32, c_vp, c_vp, c_vp,
                                               c_vp, c_vp, c_i32, _P(c_i64)]),
+    "c2v_forward_host_packed": (ctypes.c_int, [c_vp, _P(Params), c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_i64, c_vp, c_vp,
+                                               c_vp, c_vp, c_vp, c_i32]),
+    "c2v_forward_host_packed_async": (ctypes.c_int, [c_vp, _P(Params), c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_i64, c_vp,
+                                                     c_vp, c_vp, c_vp, c_vp, c_i32, _P(c_i64)]),
     "c2v_session_wait": (ctypes.c_int, [c_vp, c_i64]),
     "c2v_launch_count": (c_i64, []),
     "c2v_profile_enable": (ctypes.c_int, [c_i32]),

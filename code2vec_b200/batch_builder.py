@@ -1,6 +1,7 @@
 """Device-resident corpus + on-GPU batch construction: the drop-in for `DatasetBuilder.refresh_train_dataset` /
 `build_data` + the `DataLoader(shuffle=True)` of the reference's epoch loop (model/dataset_builder.py:55-63, :112-204,
-main.py:160-169) for the method-name task (`build`, `epoch`) and the variable-name task (`build_vars`, `epoch_vars`).  All arithmetic happens in libc2v_b200.so (`c2v_build_batch`); there is no
+main.py:160-169) for the method-name task (`build`, `epoch`) and the variable-name task (`build_vars`, `epoch_vars`), each
+also as packed batches (`build_packed`, `epoch_packed`, `build_vars_packed`, `epoch_vars_packed`).  All arithmetic happens in libc2v_b200.so (`c2v_build_batch`); there is no
 CPU fallback.
 
     corpus = DeviceCorpus.from_reader(reader, builder.train_items, device)          # once
@@ -103,6 +104,15 @@ class DeviceCorpus:
         self.var_pos = torch.from_numpy(pos).to(dev)
         self.variable_indexes = torch.from_numpy(var).to(dev)
         self.terminal_count, self.shuffle_variable_indexes = int(terminal_count), bool(shuffle_variable_indexes)
+        self.unit_counts = np.zeros(0, np.int64)      # matching contexts per unit, on the host: packed bag offsets
+        if self.n_units:
+            counts = torch.empty((self.n_units,), dtype=torch.int64, device=dev)
+            with torch.cuda.device(dev):
+                rc = _lib.load().c2v_count_unit_contexts(_ptr(self.offsets), _ptr(self.contexts), self.n_items,
+                                                         _ptr(self.unit_item), _ptr(self.unit_var), self.n_units, _ptr(counts),
+                                                         ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
+                _lib.check(rc, "c2v_count_unit_contexts")
+            self.unit_counts = counts.cpu().numpy()
 
     def build_vars(self, unit_ids, max_path_length, seed):
         """-> (starts, paths, ends, label) of the variable-name bags `unit_ids` (int64 [B] into the units)."""
@@ -161,26 +171,48 @@ class DeviceCorpus:
         the device in one pinned, asynchronous copy) or a CUDA tensor (one device-to-host copy of the ids, because the bag
         offsets are computed on the host)."""
         L = int(max_path_length)
-        if isinstance(item_ids, torch.Tensor) and item_ids.is_cuda:
-            ids = item_ids.to(dtype=torch.int64).reshape(-1).contiguous()
-            off = packed_offsets(self.counts, ids.cpu().numpy(), L)
-            off_dev = _upload(off, self.device)
-        else:
-            host_ids = (item_ids.numpy() if isinstance(item_ids, torch.Tensor) else np.asarray(item_ids)).astype(np.int64).reshape(-1)
-            off = packed_offsets(self.counts, host_ids, L)
-            staged = _upload(np.concatenate([host_ids, off]), self.device)
-            ids, off_dev = staged[:host_ids.size], staged[host_ids.size:]
-        return self._build_packed(ids, off, off_dev, L, seed)
+        return self._build_packed(*self._stage_packed(item_ids, self.counts, L), L, seed)
+
+    def _stage_packed(self, ids, counts, L):
+        """-> (device ids [B], host bag offsets, device bag offsets) of a packed batch over bags of counts[id] contexts"""
+        if isinstance(ids, torch.Tensor) and ids.is_cuda:
+            ids = ids.to(dtype=torch.int64).reshape(-1).contiguous()
+            off = packed_offsets(counts, ids.cpu().numpy(), L)
+            return ids, off, _upload(off, self.device)
+        host_ids = (ids.numpy() if isinstance(ids, torch.Tensor) else np.asarray(ids)).astype(np.int64).reshape(-1)
+        off = packed_offsets(counts, host_ids, L)
+        staged = _upload(np.concatenate([host_ids, off]), self.device)
+        return staged[:host_ids.size], off, staged[host_ids.size:]
+
+    def _epoch_staged(self, n, counts, batch_size, L, seed, shuffle, rank, world):
+        """the permutation of `epoch` over n ids, staged for packed batches -> (device ids, host offsets, device offsets)
+        per batch.  Per epoch, not per batch: one device-to-host copy of the permutation (the bag offsets are computed on
+        the host) and one pinned, asynchronous copy of every batch's offsets to the device; each batch takes its ids and
+        offsets as slices of device tensors."""
+        g = torch.Generator(device=self.device).manual_seed(int(seed))
+        order = torch.randperm(n, generator=g, device=self.device) if shuffle else torch.arange(n, device=self.device)
+        order = order[rank::world].contiguous()
+        host = order.cpu().numpy()
+        spans = [(lo, min(lo + batch_size, host.size)) for lo in range(0, host.size, batch_size)]
+        offs = [packed_offsets(counts, host[lo:hi], L) for lo, hi in spans]
+        if not offs:
+            return
+        all_dev = _upload(np.concatenate(offs), self.device)        # batch i's B + 1 offsets start at lo + i
+        for i, ((lo, hi), off) in enumerate(zip(spans, offs)):
+            yield order[lo:hi], off, all_dev[lo + i:hi + i + 1]
+
+    def _empty_packed(self, B, off, off_dev, L):
+        """-> (PackedBags, label [B]) to be filled by a packed builder: N = off[-1] rows"""
+        starts = torch.empty((int(off[-1]),), dtype=torch.int64, device=self.device)
+        bags = PackedBags(starts, torch.empty_like(starts), torch.empty_like(starts), off, L, device_offsets=off_dev)
+        return bags, torch.empty((B,), dtype=torch.int64, device=self.device)
 
     def _build_packed(self, ids, off, off_dev, L, seed):
         """c2v_build_batch_packed for device ids [B] and bag offsets given on the host (off) and on the device (off_dev)"""
         lib = _lib.load()
-        B, N = int(ids.numel()), int(off[-1])
+        B = int(ids.numel())
         with torch.cuda.device(self.device):
-            starts = torch.empty((N,), dtype=torch.int64, device=self.device)
-            bags = PackedBags(starts, torch.empty_like(starts), torch.empty_like(starts), off, L,
-                              device_offsets=off_dev)                                  # filled below
-            label = torch.empty((B,), dtype=torch.int64, device=self.device)
+            bags, label = self._empty_packed(B, off, off_dev, L)
             rc = lib.c2v_build_batch_packed(_ptr(self.offsets), _ptr(self.contexts), self.n_items, _ptr(ids), _ptr(self.labels),
                                             B, L, int(seed) & 0xFFFFFFFFFFFFFFFF, self.method_token, self.question_token,
                                             _ptr(bags.offsets), _ptr(bags.starts), _ptr(bags.paths), _ptr(bags.ends),
@@ -190,22 +222,48 @@ class DeviceCorpus:
 
     def epoch_packed(self, batch_size, max_path_length, seed, shuffle=True, rank=0, world=1):
         """`epoch` with packed batches: the same permutation, the same items in the same order -> (PackedBags, label) per
-        batch, as build_packed makes them.  Per epoch, not per batch: one device-to-host copy of the permutation (the bag
-        offsets are computed on the host) and one pinned, asynchronous copy of every batch's offsets to the device; each
-        batch takes its ids and offsets as slices of device tensors."""
+        batch, as build_packed makes them, with the transfers of `_epoch_staged`."""
         L = int(max_path_length)
-        g = torch.Generator(device=self.device).manual_seed(int(seed))
-        order = torch.randperm(self.n_items, generator=g, device=self.device) if shuffle else \
-            torch.arange(self.n_items, device=self.device)
-        order = order[rank::world].contiguous()
-        host = order.cpu().numpy()
-        spans = [(lo, min(lo + batch_size, host.size)) for lo in range(0, host.size, batch_size)]
-        offs = [packed_offsets(self.counts, host[lo:hi], L) for lo, hi in spans]
-        if not offs:
-            return
-        all_dev = _upload(np.concatenate(offs), self.device)        # batch i's B + 1 offsets start at lo + i
-        for i, ((lo, hi), off) in enumerate(zip(spans, offs)):
-            yield self._build_packed(order[lo:hi], off, all_dev[lo + i:hi + i + 1], L, seed)
+        for ids, off, off_dev in self._epoch_staged(self.n_items, self.counts, batch_size, L, seed, shuffle, rank, world):
+            yield self._build_packed(ids, off, off_dev, L, seed)
+
+    def build_vars_packed(self, unit_ids, max_path_length, seed):
+        """-> (PackedBags, label [B]): the bags `build_vars` returns for the same unit ids and seed, without the zero
+        suffix.  Bag b holds min(n, L) contexts (n = unit_counts[u], the unit's matching contexts); a unit without a match
+        or an id outside the units is a bag of one pad context (0, 0, 0).  unit_ids: host ints (one pinned, asynchronous
+        copy of ids and bag offsets) or a CUDA tensor (one device-to-host copy of the ids)."""
+        self._need_units()
+        L = int(max_path_length)
+        return self._build_vars_packed(*self._stage_packed(unit_ids, self.unit_counts, L), L, seed)
+
+    def _need_units(self):
+        if getattr(self, "unit_item", None) is None:
+            raise ValueError("no variable units: build the corpus from a reader with infer_variable=True")
+
+    def _build_vars_packed(self, ids, off, off_dev, L, seed):
+        """c2v_build_batch_vars_packed for device unit ids [B] and bag offsets on the host (off) and the device (off_dev)"""
+        lib = _lib.load()
+        B = int(ids.numel())
+        with torch.cuda.device(self.device):
+            bags, label = self._empty_packed(B, off, off_dev, L)
+            rc = lib.c2v_build_batch_vars_packed(_ptr(self.offsets), _ptr(self.contexts), self.n_items, _ptr(self.unit_item),
+                                                 _ptr(self.unit_var), _ptr(self.unit_label), self.n_units, _ptr(ids), B, L,
+                                                 int(seed) & 0xFFFFFFFFFFFFFFFF, self.question_token, _ptr(self.var_pos),
+                                                 self.terminal_count, _ptr(self.variable_indexes),
+                                                 int(self.variable_indexes.numel()), 1 if self.shuffle_variable_indexes else 0,
+                                                 _ptr(bags.offsets), _ptr(bags.starts), _ptr(bags.paths), _ptr(bags.ends),
+                                                 _ptr(label), ctypes.c_void_p(torch.cuda.current_stream(self.device).cuda_stream))
+            _lib.check(rc, "c2v_build_batch_vars_packed")
+        return bags, label
+
+    def epoch_vars_packed(self, batch_size, max_path_length, seed, shuffle=True, rank=0, world=1):
+        """`epoch_vars` with packed batches: the same units in the same order -> (PackedBags, label) per batch, as
+        build_vars_packed makes them, with the transfers of `_epoch_staged`."""
+        self._need_units()
+        L = int(max_path_length)
+        for ids, off, off_dev in self._epoch_staged(self.n_units, self.unit_counts, batch_size, L, seed, shuffle, rank,
+                                                    world):
+            yield self._build_vars_packed(ids, off, off_dev, L, seed)
 
     def epoch_vars(self, batch_size, max_path_length, seed, shuffle=True, rank=0, world=1):
         """the same pass over the variable-name units (dataset_builder.py:152-204)"""

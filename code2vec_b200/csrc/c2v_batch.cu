@@ -126,6 +126,32 @@ build_batch_kernel(const long long *__restrict__ offsets, const int *__restrict_
 // ---- variable-name task ---------------------------------------------------------------------------------------------
 constexpr int BB_MAX_VARS = 2048;      // |variable_indexes| (dataset/: 62, top11: 390)
 
+// context c (start, path, end) belongs to the bag of variable v when its start or end is v.
+// The count kernel and the builder both call this: a disagreement would silently give a bag of another length.
+__device__ __forceinline__ bool bb_var_match(const int *c, long long v) { return c[0] == v || c[2] == v; }
+
+// one warp per unit: counts[u] = the number of contexts of unit_item[u] that match unit_var[u] (0 for an unknown item)
+__global__ void __launch_bounds__(256)
+count_unit_contexts_kernel(const long long *__restrict__ offsets, const int *__restrict__ ctx, long long n_items,
+                           const long long *__restrict__ unit_item, const long long *__restrict__ unit_var,
+                           long long n_units, long long *__restrict__ counts)
+{
+    const long long u = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
+    const int lane = threadIdx.x & 31;
+    if (u >= n_units) return;
+    const long long item = unit_item[u];
+    long long cnt = 0;
+    if (item >= 0 && item < n_items) {
+        const long long lo = offsets[item], n = offsets[item + 1] - lo, v = unit_var[u];
+        for (long long j = lane; j < n; j += 32) cnt += bb_var_match(ctx + (lo + j) * 3, v) ? 1 : 0;
+    }
+    for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+    if (lane == 0) counts[u] = cnt;
+}
+
+// PACKED: bag b goes to rows bag_off[b] .. bag_off[b+1]-1 (its length: min(n_match, L), 1 for a unit without a match or
+// an unknown unit) instead of row b of the [B, L] tensors.  The selection still runs on L = max_path_length.
+template <bool PACKED = false>
 __global__ void __launch_bounds__(256)
 build_batch_vars_kernel(const long long *__restrict__ offsets, const int *__restrict__ ctx, long long n_items,
                         const long long *__restrict__ unit_item, const long long *__restrict__ unit_var,
@@ -134,7 +160,7 @@ build_batch_vars_kernel(const long long *__restrict__ offsets, const int *__rest
                         const int *__restrict__ var_pos, long long T, const long long *__restrict__ variable_indexes,
                         int n_vars, int shuffle,
                         long long *__restrict__ starts, long long *__restrict__ paths, long long *__restrict__ ends,
-                        long long *__restrict__ label)
+                        long long *__restrict__ label, const long long *__restrict__ bag_off)
 {
     __shared__ unsigned hist[256];
     __shared__ int s_warp[8];
@@ -144,10 +170,16 @@ build_batch_vars_kernel(const long long *__restrict__ offsets, const int *__rest
     __shared__ unsigned short s_sigma[BB_MAX_VARS];
     const int b = blockIdx.x, tid = threadIdx.x;
     const long long unit = unit_ids[b];
-    long long *rs = starts + (size_t)b * L, *rp = paths + (size_t)b * L, *re = ends + (size_t)b * L;
+    const long long row0 = PACKED ? bag_off[b] : (long long)b * L;
+    long long *rs = starts + row0, *rp = paths + row0, *re = ends + row0;
+    int cap = L;                                             // rows this bag may write
+    if (PACKED) {                                            // the host-computed length, clamped into [0, L]
+        const long long len = bag_off[b + 1] - row0;
+        cap = len < 0 ? 0 : (len > L ? L : (int)len);
+    }
     const long long item = (unit >= 0 && unit < n_units) ? unit_item[unit] : -1;
     if (item < 0 || item >= n_items) {                      // not a unit of this corpus: an all-pad bag
-        for (int j = tid; j < L; j += 256) { rs[j] = 0; rp[j] = 0; re[j] = 0; }
+        for (int j = tid; j < cap; j += 256) { rs[j] = 0; rp[j] = 0; re[j] = 0; }
         if (label && tid == 0) label[b] = 0;
         return;
     }
@@ -178,7 +210,7 @@ build_batch_vars_kernel(const long long *__restrict__ offsets, const int *__rest
         }
         return t;
     };
-    auto match = [&](long long j) { const int *c = ctx + (lo + j) * 3; return c[0] == v || c[2] == v; };
+    auto match = [&](long long j) { return bb_var_match(ctx + (lo + j) * 3, v); };
     auto emit = [&](int pos, long long j) {
         const int *c = ctx + (lo + j) * 3;
         rs[pos] = remap(c[0]); rp[pos] = c[1]; re[pos] = remap(c[2]);
@@ -235,11 +267,11 @@ build_batch_vars_kernel(const long long *__restrict__ offsets, const int *__rest
         const int eq_rank = base_eq + bb_block_scan(is_eq, s_warp, &tot_eq);
         const int take = (m && (n_match <= L || key < Tkey || (is_eq && eq_rank < need_eq))) ? 1 : 0;
         const int pos = base_pos + bb_block_scan(take, s_warp, &tot_take);
-        if (take) emit(pos, j);
+        if (take && (!PACKED || pos < cap)) emit(pos, j);
         base_eq += tot_eq; base_pos += tot_take;
     }
     const int filled = n_match < L ? n_match : L;
-    for (int j = filled + tid; j < L; j += 256) { rs[j] = 0; rp[j] = 0; re[j] = 0; }     // pad_inputs (:212-219)
+    for (int j = filled + tid; j < cap; j += 256) { rs[j] = 0; rp[j] = 0; re[j] = 0; }   // pad_inputs (:212-219)
 }
 
 }  // namespace c2v
@@ -282,6 +314,28 @@ extern "C" int c2v_build_batch_packed(const int64_t *offsets, const int32_t *con
     return C2V_OK;
 }
 
+// argument checks of both variable-name builders, before any CUDA call
+static int vars_args_ok(const char *fn, const int64_t *offsets, const int32_t *contexts, int64_t n_items,
+                        const int64_t *unit_item, const int64_t *unit_var, int64_t n_units, const int64_t *unit_ids,
+                        int32_t B, int32_t L, const int32_t *var_pos, const int64_t *variable_indexes, int32_t n_vars,
+                        int32_t shuffle_variable_indexes, const int64_t *starts, const int64_t *paths, const int64_t *ends)
+{
+    if (!offsets || !contexts || !unit_item || !unit_var || !unit_ids || !starts || !paths || !ends || n_items < 1 ||
+        n_units < 1 || B < 1 || L < 1) {
+        set_error("%s: bad argument", fn);
+        return C2V_EINVAL;
+    }
+    if (shuffle_variable_indexes && (!var_pos || !variable_indexes || n_vars < 0)) {
+        set_error("%s: shuffle_variable_indexes needs var_pos and variable_indexes", fn);
+        return C2V_EINVAL;
+    }
+    if (n_vars > BB_MAX_VARS) {
+        set_error("%s: %d variable indexes (max %d)", fn, n_vars, BB_MAX_VARS);
+        return C2V_EUNSUPPORTED;
+    }
+    return C2V_OK;
+}
+
 extern "C" int c2v_build_batch_vars(const int64_t *offsets, const int32_t *contexts, int64_t n_items,
                                     const int64_t *unit_item, const int64_t *unit_var, const int64_t *unit_label,
                                     int64_t n_units, const int64_t *unit_ids, int32_t B, int32_t L, uint64_t seed,
@@ -289,26 +343,55 @@ extern "C" int c2v_build_batch_vars(const int64_t *offsets, const int32_t *conte
                                     const int64_t *variable_indexes, int32_t n_vars, int32_t shuffle_variable_indexes,
                                     int64_t *starts, int64_t *paths, int64_t *ends, int64_t *label, void *stream)
 {
-    if (!offsets || !contexts || !unit_item || !unit_var || !unit_ids || !starts || !paths || !ends || n_items < 1 ||
-        n_units < 1 || B < 1 || L < 1) {
-        set_error("c2v_build_batch_vars: bad argument");
-        return C2V_EINVAL;
-    }
-    if (shuffle_variable_indexes && (!var_pos || !variable_indexes || n_vars < 0)) {
-        set_error("c2v_build_batch_vars: shuffle_variable_indexes needs var_pos and variable_indexes");
-        return C2V_EINVAL;
-    }
-    if (n_vars > BB_MAX_VARS) {
-        set_error("c2v_build_batch_vars: %d variable indexes (max %d)", n_vars, BB_MAX_VARS);
-        return C2V_EUNSUPPORTED;
-    }
+    const int rc = vars_args_ok("c2v_build_batch_vars", offsets, contexts, n_items, unit_item, unit_var, n_units, unit_ids,
+                                B, L, var_pos, variable_indexes, n_vars, shuffle_variable_indexes, starts, paths, ends);
+    if (rc != C2V_OK) return rc;
     build_batch_vars_kernel<<<(unsigned)B, 256, 0, static_cast<cudaStream_t>(stream)>>>(
         reinterpret_cast<const long long *>(offsets), contexts, n_items, reinterpret_cast<const long long *>(unit_item),
         reinterpret_cast<const long long *>(unit_var), reinterpret_cast<const long long *>(unit_label), n_units,
         reinterpret_cast<const long long *>(unit_ids), L, seed, question_token, var_pos, terminal_count,
         reinterpret_cast<const long long *>(variable_indexes), n_vars, shuffle_variable_indexes,
         reinterpret_cast<long long *>(starts), reinterpret_cast<long long *>(paths), reinterpret_cast<long long *>(ends),
-        reinterpret_cast<long long *>(label));
+        reinterpret_cast<long long *>(label), nullptr);
     C2V_LAUNCH_OK("build_batch_vars_kernel");
+    return C2V_OK;
+}
+
+extern "C" int c2v_build_batch_vars_packed(const int64_t *offsets, const int32_t *contexts, int64_t n_items,
+                                           const int64_t *unit_item, const int64_t *unit_var, const int64_t *unit_label,
+                                           int64_t n_units, const int64_t *unit_ids, int32_t B, int32_t L, uint64_t seed,
+                                           int64_t question_token, const int32_t *var_pos, int64_t terminal_count,
+                                           const int64_t *variable_indexes, int32_t n_vars,
+                                           int32_t shuffle_variable_indexes, const int64_t *bag_offsets, int64_t *starts,
+                                           int64_t *paths, int64_t *ends, int64_t *label, void *stream)
+{
+    if (!bag_offsets) { set_error("c2v_build_batch_vars_packed: bad argument (bag_offsets is NULL)"); return C2V_EINVAL; }
+    const int rc = vars_args_ok("c2v_build_batch_vars_packed", offsets, contexts, n_items, unit_item, unit_var, n_units,
+                                unit_ids, B, L, var_pos, variable_indexes, n_vars, shuffle_variable_indexes, starts, paths,
+                                ends);
+    if (rc != C2V_OK) return rc;
+    build_batch_vars_kernel<true><<<(unsigned)B, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        reinterpret_cast<const long long *>(offsets), contexts, n_items, reinterpret_cast<const long long *>(unit_item),
+        reinterpret_cast<const long long *>(unit_var), reinterpret_cast<const long long *>(unit_label), n_units,
+        reinterpret_cast<const long long *>(unit_ids), L, seed, question_token, var_pos, terminal_count,
+        reinterpret_cast<const long long *>(variable_indexes), n_vars, shuffle_variable_indexes,
+        reinterpret_cast<long long *>(starts), reinterpret_cast<long long *>(paths), reinterpret_cast<long long *>(ends),
+        reinterpret_cast<long long *>(label), reinterpret_cast<const long long *>(bag_offsets));
+    C2V_LAUNCH_OK("build_batch_vars_kernel<packed>");
+    return C2V_OK;
+}
+
+extern "C" int c2v_count_unit_contexts(const int64_t *offsets, const int32_t *contexts, int64_t n_items,
+                                       const int64_t *unit_item, const int64_t *unit_var, int64_t n_units, int64_t *counts,
+                                       void *stream)
+{
+    if (!offsets || !contexts || !unit_item || !unit_var || !counts || n_items < 1 || n_units < 1) {
+        set_error("c2v_count_unit_contexts: bad argument (NULL pointer, n_items < 1 or n_units < 1)");
+        return C2V_EINVAL;
+    }
+    count_unit_contexts_kernel<<<(unsigned)((n_units + 7) / 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        reinterpret_cast<const long long *>(offsets), contexts, n_items, reinterpret_cast<const long long *>(unit_item),
+        reinterpret_cast<const long long *>(unit_var), n_units, reinterpret_cast<long long *>(counts));
+    C2V_LAUNCH_OK("count_unit_contexts_kernel");
     return C2V_OK;
 }

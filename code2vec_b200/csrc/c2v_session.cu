@@ -21,7 +21,7 @@ struct c2v_session {
     int max_B, L;
     cudaStream_t s_up, s_run, s_down;
     struct Slot {
-        long long *d_idx;      // starts | paths | ends | label
+        long long *d_idx;      // starts | paths | ends | label | bag offsets (packed calls)
         float *d_cv, *d_att, *d_out, *d_score;
         long long *d_pred;
         void *ws_enc, *ws_lab;
@@ -61,9 +61,13 @@ int c2v_session_create(int device, const c2v_dims *d, int32_t max_B, int32_t L, 
     const size_t n = (size_t)max_B * L;
     for (int i = 0; i < kSlots; ++i) {
         c2v_session::Slot &q = s->slot[i];
-        q.ws_enc_bytes = c2v_encode_workspace_bytes(d, max_B, L);
+        // one slot serves padded and packed calls in any order: the packed workspace keeps the status word and the weight
+        // images where the padded one has them and appends its row -> bag map, so REUSE_PREP stays valid across layouts
+        const size_t ws_pad = c2v_encode_workspace_bytes(d, max_B, L);
+        const size_t ws_packed = c2v_encode_packed_workspace_bytes(d, max_B, (int64_t)n);
+        q.ws_enc_bytes = ws_pad > ws_packed ? ws_pad : ws_packed;
         q.ws_lab_bytes = c2v_label_workspace_bytes(d, max_B);
-        C2V_CUDA_OK(cudaMalloc(&q.d_idx, (3 * n + max_B) * sizeof(long long)));
+        C2V_CUDA_OK(cudaMalloc(&q.d_idx, (3 * n + max_B + max_B + 1) * sizeof(long long)));
         C2V_CUDA_OK(cudaMalloc(&q.d_cv, (size_t)max_B * d->encode * sizeof(float)));
         C2V_CUDA_OK(cudaMalloc(&q.d_att, n * sizeof(float)));
         C2V_CUDA_OK(cudaMalloc(&q.d_out, (size_t)max_B * d->label_count * sizeof(float)));
@@ -91,16 +95,13 @@ void c2v_session_destroy(c2v_session *s)
     delete s;
 }
 
-int c2v_forward_host_async(c2v_session *s, const c2v_params *p, const int64_t *starts,
-                           const int64_t *paths, const int64_t *ends, const int64_t *label,
-                           int32_t B, float *outputs, float *code_vector, float *attention,
-                           int64_t *pred_label, float *pred_score, int32_t algo, int64_t *ticket)
+// Both layouts once the arguments are checked: [B, L] (offsets == NULL, n = B * L) or packed (n = N contexts, host
+// offsets [B + 1] already validated).
+static int forward_host_impl(c2v_session *s, const c2v_params *p, const int64_t *starts, const int64_t *paths,
+                             const int64_t *ends, const int64_t *offsets, const int64_t *label, int32_t B, size_t n,
+                             float *outputs, float *code_vector, float *attention, int64_t *pred_label, float *pred_score,
+                             int32_t algo, int64_t *ticket)
 {
-    if (!s || !p || !starts || !paths || !ends || !code_vector || !attention || !ticket) {
-        set_error("c2v_forward_host: NULL argument");
-        return C2V_EINVAL;
-    }
-    if (B < 1 || B > s->max_B) { set_error("c2v_forward_host: B=%d not in [1,%d]", B, s->max_B); return C2V_EINVAL; }
     C2V_CUDA_OK(cudaSetDevice(s->device));
     const int64_t t = s->next_ticket;
     c2v_session::Slot &q = s->slot[t % kSlots];
@@ -108,21 +109,24 @@ int c2v_forward_host_async(c2v_session *s, const c2v_params *p, const int64_t *s
         C2V_CUDA_OK(cudaEventSynchronize(q.down_done));
         q.busy = false;
     }
-    const size_t n = (size_t)B * s->L;
-    long long *d_s = q.d_idx, *d_p = q.d_idx + n, *d_e = q.d_idx + 2 * n, *d_l = q.d_idx + 3 * n;
+    long long *d_s = q.d_idx, *d_p = q.d_idx + n, *d_e = q.d_idx + 2 * n, *d_l = q.d_idx + 3 * n, *d_off = d_l + B;
     C2V_CUDA_OK(cudaMemcpyAsync(d_s, starts, n * 8, cudaMemcpyHostToDevice, s->s_up));
     C2V_CUDA_OK(cudaMemcpyAsync(d_p, paths, n * 8, cudaMemcpyHostToDevice, s->s_up));
     C2V_CUDA_OK(cudaMemcpyAsync(d_e, ends, n * 8, cudaMemcpyHostToDevice, s->s_up));
     if (label) C2V_CUDA_OK(cudaMemcpyAsync(d_l, label, (size_t)B * 8, cudaMemcpyHostToDevice, s->s_up));
+    if (offsets) C2V_CUDA_OK(cudaMemcpyAsync(d_off, offsets, ((size_t)B + 1) * 8, cudaMemcpyHostToDevice, s->s_up));
     C2V_CUDA_OK(cudaEventRecord(q.up_done, s->s_up));
     C2V_CUDA_OK(cudaStreamWaitEvent(s->s_run, q.up_done, 0));
 
     // weight images are per slot: honour the caller's reuse promise only once this slot has them
     const int base_algo = algo & 0xff;
     const int reuse = ((algo & C2V_FLAG_REUSE_PREP) && q.prepped) ? C2V_FLAG_REUSE_PREP : 0;
-    int rc = c2v_encode_forward(&s->dims, p, (const int64_t *)d_s, (const int64_t *)d_p,
-                                (const int64_t *)d_e, B, s->L, nullptr, q.d_cv, q.d_att, q.ws_enc,
-                                q.ws_enc_bytes, base_algo | reuse, s->s_run);
+    int rc = offsets
+        ? c2v_encode_forward_packed(&s->dims, p, (const int64_t *)d_s, (const int64_t *)d_p, (const int64_t *)d_e,
+                                    (const int64_t *)d_off, B, (int64_t)n, s->L, nullptr, q.d_cv, q.d_att, nullptr, q.ws_enc,
+                                    q.ws_enc_bytes, base_algo | reuse, s->s_run)
+        : c2v_encode_forward(&s->dims, p, (const int64_t *)d_s, (const int64_t *)d_p, (const int64_t *)d_e, B, s->L, nullptr,
+                             q.d_cv, q.d_att, q.ws_enc, q.ws_enc_bytes, base_algo | reuse, s->s_run);
     if (rc != C2V_OK) return rc;
     const bool want_head = outputs || pred_label || pred_score;
     // the [B, C] logits are only materialised when the caller asked for them (or the fused arg-max cannot serve this shape):
@@ -155,6 +159,50 @@ int c2v_forward_host_async(c2v_session *s, const c2v_params *p, const int64_t *s
     return C2V_OK;
 }
 
+int c2v_forward_host_async(c2v_session *s, const c2v_params *p, const int64_t *starts,
+                           const int64_t *paths, const int64_t *ends, const int64_t *label,
+                           int32_t B, float *outputs, float *code_vector, float *attention,
+                           int64_t *pred_label, float *pred_score, int32_t algo, int64_t *ticket)
+{
+    if (!s || !p || !starts || !paths || !ends || !code_vector || !attention || !ticket) {
+        set_error("c2v_forward_host: NULL argument");
+        return C2V_EINVAL;
+    }
+    if (B < 1 || B > s->max_B) { set_error("c2v_forward_host: B=%d not in [1,%d]", B, s->max_B); return C2V_EINVAL; }
+    return forward_host_impl(s, p, starts, paths, ends, nullptr, label, B, (size_t)B * s->L, outputs, code_vector, attention,
+                             pred_label, pred_score, algo, ticket);
+}
+
+int c2v_forward_host_packed_async(c2v_session *s, const c2v_params *p, const int64_t *starts, const int64_t *paths,
+                                  const int64_t *ends, const int64_t *offsets, const int64_t *label, int32_t B, int64_t N,
+                                  float *outputs, float *code_vector, float *attention, int64_t *pred_label,
+                                  float *pred_score, int32_t algo, int64_t *ticket)
+{
+    if (!s || !p || !starts || !paths || !ends || !offsets || !code_vector || !attention || !ticket) {
+        set_error("c2v_forward_host_packed: NULL argument");
+        return C2V_EINVAL;
+    }
+    if (B < 1 || B > s->max_B) { set_error("c2v_forward_host_packed: B=%d not in [1,%d]", B, s->max_B); return C2V_EINVAL; }
+    // the offsets are host memory: check them here, before anything is copied or launched
+    if (offsets[0] != 0) {
+        set_error("c2v_forward_host_packed: offsets[0] = %lld, must be 0", (long long)offsets[0]);
+        return C2V_EINVAL;
+    }
+    for (int32_t b = 0; b < B; ++b) {
+        const int64_t len = offsets[b + 1] - offsets[b];
+        if (len < 1 || len > s->L) {
+            set_error("c2v_forward_host_packed: bag %d holds %lld contexts, must hold 1 .. %d", b, (long long)len, s->L);
+            return C2V_EINVAL;
+        }
+    }
+    if (offsets[B] != N) {
+        set_error("c2v_forward_host_packed: offsets[B] = %lld != N = %lld", (long long)offsets[B], (long long)N);
+        return C2V_EINVAL;
+    }
+    return forward_host_impl(s, p, starts, paths, ends, offsets, label, B, (size_t)N, outputs, code_vector, attention,
+                             pred_label, pred_score, algo, ticket);
+}
+
 int c2v_session_wait(c2v_session *s, int64_t ticket)
 {
     if (!s) { set_error("session is NULL"); return C2V_EINVAL; }
@@ -177,6 +225,18 @@ int c2v_forward_host(c2v_session *s, const c2v_params *p, const int64_t *starts,
     int64_t t = 0;
     int rc = c2v_forward_host_async(s, p, starts, paths, ends, label, B, outputs, code_vector,
                                     attention, pred_label, pred_score, algo, &t);
+    if (rc != C2V_OK) return rc;
+    return c2v_session_wait(s, t);
+}
+
+int c2v_forward_host_packed(c2v_session *s, const c2v_params *p, const int64_t *starts, const int64_t *paths,
+                            const int64_t *ends, const int64_t *offsets, const int64_t *label, int32_t B, int64_t N,
+                            float *outputs, float *code_vector, float *attention, int64_t *pred_label, float *pred_score,
+                            int32_t algo)
+{
+    int64_t t = 0;
+    int rc = c2v_forward_host_packed_async(s, p, starts, paths, ends, offsets, label, B, N, outputs, code_vector, attention,
+                                           pred_label, pred_score, algo, &t);
     if (rc != C2V_OK) return rc;
     return c2v_session_wait(s, t);
 }

@@ -358,6 +358,23 @@ int c2v_forward_host_async(c2v_session *s, const c2v_params *p,
                            float *outputs, float *code_vector, float *attention,
                            int64_t *pred_label, float *pred_score, int32_t algo, int64_t *ticket);
 int c2v_session_wait(c2v_session *s, int64_t ticket);
+/* The same calls for a packed (CSR) batch in host memory (layout as c2v_encode_forward_packed): starts / paths / ends
+ * int64 [N], offsets int64 [B + 1] (host), attention [N], aligned with the packed contexts; everything else as above.
+ * Both the index upload and the attention download scale with N instead of B * L.  The offsets are validated on the
+ * host before anything is copied or launched: C2V_EINVAL (c2v_last_error names the bag) unless offsets[0] == 0, every
+ * bag holds 1 .. L contexts (L: the session's), offsets[B] == N and 1 <= B <= max_B.  A session serves padded and
+ * packed calls in any order, C2V_FLAG_REUSE_PREP included. */
+int c2v_forward_host_packed(c2v_session *s, const c2v_params *p,
+                            const int64_t *starts, const int64_t *paths, const int64_t *ends,
+                            const int64_t *offsets, const int64_t *label, int32_t B, int64_t N,
+                            float *outputs /* [B,C] or NULL */, float *code_vector /* [B,H] */,
+                            float *attention /* [N] */, int64_t *pred_label /* [B] or NULL */,
+                            float *pred_score /* [B] or NULL */, int32_t algo);
+int c2v_forward_host_packed_async(c2v_session *s, const c2v_params *p,
+                                  const int64_t *starts, const int64_t *paths, const int64_t *ends,
+                                  const int64_t *offsets, const int64_t *label, int32_t B, int64_t N,
+                                  float *outputs, float *code_vector, float *attention,
+                                  int64_t *pred_label, float *pred_score, int32_t algo, int64_t *ticket);
 
 /* On-GPU batch construction for the method-name task: replaces DatasetBuilder.build_data
  * (model/dataset_builder.py:112-150, infer_method branch).  The corpus stays on the device as CSR:
@@ -392,6 +409,25 @@ int c2v_build_batch_vars(const int64_t *offsets, const int32_t *contexts, int64_
                          int64_t question_token, const int32_t *var_pos, int64_t terminal_count,
                          const int64_t *variable_indexes, int32_t n_vars, int32_t shuffle_variable_indexes,
                          int64_t *starts, int64_t *paths, int64_t *ends, int64_t *label, void *stream);
+/* The number of contexts each unit's bag draws from: counts[u] (int64 [n_units], device) = the contexts of item
+ * unit_item[u] whose start or end is unit_var[u] -- the match rule of c2v_build_batch_vars --, 0 when the item is
+ * outside [0, n_items).  Depends on the corpus only, not on the seed: a caller counts once and sizes packed bags from it
+ * on the host. */
+int c2v_count_unit_contexts(const int64_t *offsets, const int32_t *contexts, int64_t n_items,
+                            const int64_t *unit_item, const int64_t *unit_var, int64_t n_units, int64_t *counts,
+                            void *stream);
+/* The same bags as a packed batch: bag b goes to rows bag_offsets[b] .. bag_offsets[b+1]-1 of starts / paths / ends
+ * (int64 [N], device; bag_offsets int64 [B + 1], device, not NULL).  The caller sizes bag b as min(counts[u], L)
+ * contexts (c2v_count_unit_contexts) and as one context for a unit without a match or an id outside [0, n_units): that
+ * bag is one pad context (0, 0, 0).  Same selection and labels as c2v_build_batch_vars, so the result is its [B, L]
+ * batch without the zero suffix; nothing is written outside a bag's rows, whatever the offsets say. */
+int c2v_build_batch_vars_packed(const int64_t *offsets, const int32_t *contexts, int64_t n_items,
+                                const int64_t *unit_item, const int64_t *unit_var, const int64_t *unit_label,
+                                int64_t n_units, const int64_t *unit_ids, int32_t B, int32_t L, uint64_t seed,
+                                int64_t question_token, const int32_t *var_pos, int64_t terminal_count,
+                                const int64_t *variable_indexes, int32_t n_vars, int32_t shuffle_variable_indexes,
+                                const int64_t *bag_offsets, int64_t *starts, int64_t *paths, int64_t *ends,
+                                int64_t *label, void *stream);
 
 /* Fused flat-buffer Adam: torch.optim.Adam(..., lr, betas, weight_decay) of main.py:138 +
  * optimizer.step() (:175) + optimizer.zero_grad() (:171) for all parameters in one launch.  param / grad / exp_avg /
