@@ -13,6 +13,8 @@ C2V_OK, C2V_EINVAL, C2V_ECUDA, C2V_EWORKSPACE, C2V_EINDEX, C2V_EUNSUPPORTED = 0,
 ALGO_AUTO, ALGO_FFMA, ALGO_TCGEN05 = 0, 1, 2
 ABI_VERSION = 1
 TOPK_MAX = 16                # C2V_TOPK_MAX: the largest k of the fused top-k (c2v_label_topk / c2v_angular_topk)
+KNN_EXCLUDE_MAX = 4          # C2V_KNN_EXCLUDE_MAX: excluded bank rows per query of c2v_knn_topk / c2v_knn_pairs
+KNN_MAX_Q = 2048             # queries per c2v_knn_* call
 
 c_i32, c_i64, c_f32, c_vp, c_sz = ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_void_p, ctypes.c_size_t
 
@@ -45,6 +47,10 @@ class DeviceInfo(ctypes.Structure):
 class CorpusInfo(ctypes.Structure):
     _fields_ = [("n_items", c_i64), ("n_contexts", c_i64), ("n_aliases", c_i64), ("label_bytes", c_i64),
                 ("alias_bytes", c_i64), ("alias_name_bytes", c_i64)]
+
+
+class VectorsInfo(ctypes.Structure):
+    _fields_ = [("n", c_i64), ("header_items", c_i64), ("H", c_i32), ("reserved", c_i32), ("name_bytes", c_i64)]
 
 
 # every symbol include/c2v_b200.h declares: (restype, argtypes)
@@ -141,6 +147,18 @@ SYMBOLS = {
     "c2v_format_float": (ctypes.c_int, [c_f32, ctypes.c_char_p, c_sz]),
     "c2v_write_code_vectors": (ctypes.c_int, [ctypes.c_char_p, ctypes.c_char_p, c_i64, c_i64, c_i32, c_vp, c_vp, c_vp, c_vp,
                                               c_i64, ctypes.c_char_p, ctypes.c_char_p, c_vp, c_vp, c_vp]),
+    "c2v_read_code_vectors": (ctypes.c_int, [ctypes.c_char_p, c_i32, _P(c_vp)]),
+    "c2v_vectors_get_info": (ctypes.c_int, [c_vp, _P(VectorsInfo)]),
+    "c2v_vectors_export": (ctypes.c_int, [c_vp, c_vp, c_vp, c_vp]),
+    "c2v_vectors_free": (None, [c_vp]),
+    "c2v_knn_prep_workspace_bytes": (c_sz, [c_i64, c_i32]),
+    "c2v_knn_prepare": (ctypes.c_int, [c_vp, c_i64, c_i32, c_vp, c_sz, c_vp]),
+    "c2v_knn_topk_workspace_bytes": (c_sz, [c_i64, c_i32, c_i32, c_i32]),
+    "c2v_knn_topk": (ctypes.c_int, [c_vp, c_i64, c_i32, c_vp, c_i32, c_i32, c_vp, c_i32, c_vp, c_vp, c_vp, c_sz, c_vp, c_sz,
+                                    c_i32, c_vp]),
+    "c2v_knn_pairs_workspace_bytes": (c_sz, [c_i64, c_i32, c_i32]),
+    "c2v_knn_pairs": (ctypes.c_int, [c_vp, c_i64, c_i32, c_vp, c_i32, c_f32, c_vp, c_i32, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp,
+                                     c_vp, c_sz, c_vp, c_sz, c_i32, c_vp]),
 }
 
 _lib = None

@@ -259,6 +259,28 @@ class CorpusReader(object):
         return np.asarray(ui, np.int64), np.asarray(uv, np.int64), np.asarray(ul, np.int64)
 
 
+def read_code_vectors(vector_file, header="auto"):
+    """The file write_code_vectors writes, read back -> (vectors float32 [n, H], names [n], header_items or None).
+    header: "auto" (the first line is a header when it is two tab-separated integers), True or False.  A write followed
+    by a read is bit-exact (every NaN reads back as a NaN)."""
+    lib = _lib.load()
+    mode = {"auto": -1, True: 1, False: 0}[header]
+    h = ctypes.c_void_p()
+    _lib.check(lib.c2v_read_code_vectors(str(vector_file).encode(), mode, ctypes.byref(h)), "c2v_read_code_vectors")
+    try:
+        info = _lib.VectorsInfo()
+        _lib.check(lib.c2v_vectors_get_info(h, ctypes.byref(info)), "c2v_vectors_get_info")
+        vec = np.empty((info.n, info.H), np.float32)
+        offs = np.empty(info.n + 1, np.int64)
+        blob = ctypes.create_string_buffer(max(1, info.name_bytes))
+        _lib.check(lib.c2v_vectors_export(h, vec.ctypes.data_as(ctypes.c_void_p), offs.ctypes.data_as(ctypes.c_void_p),
+                                          ctypes.cast(blob, ctypes.c_void_p)), "c2v_vectors_export")
+        names = _strings(blob.raw[:info.name_bytes], offs)
+        return vec, names, (None if info.header_items < 0 else int(info.header_items))
+    finally:
+        lib.c2v_vectors_free(h)
+
+
 def write_code_vectors(vector_file, mode, code_vectors, labels, label_vocab, header_items=None, encode_size=None,
                        test_result_file=None, ids=None, pred_labels=None, pred_scores=None, result_mode="w"):
     """main.py:393-423 for a whole pass at once.  code_vectors: float32 [n, H] (torch CPU/CUDA tensor or ndarray),

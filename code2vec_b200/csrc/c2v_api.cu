@@ -641,6 +641,138 @@ int c2v_angular_topk(const c2v_dims *d, const c2v_params *p, const float *code_v
     return label_gemm(d, p, code_vector, B, nullptr, nullptr, nullptr, workspace, workspace_bytes, algo, stream, &la);
 }
 
+// ---- similarity search (c2v_knn_*) ------------------------------------------------------------------------------------
+static const long long kKnnMaxN = 0xFFFFFFFEll;      // the top-k keys hold ~column in 32 bits: N < 2^32 - 1
+static const int kKnnMaxQ = 2048;
+
+static bool aligned16(const void *p) { return ((uintptr_t)p & 15) == 0; }
+
+// the bank's shape: C2V_EINVAL / C2V_EUNSUPPORTED with the message, or C2V_OK
+static int knn_shape_ok(const char *fn, long long N, int H)
+{
+    if (N < 1 || N > kKnnMaxN || H < 1) {
+        set_error("%s: N=%lld, H=%d: needs 1 <= N < 2^32 - 1 and H >= 1", fn, N, H);
+        return C2V_EINVAL;
+    }
+    if (H % 4 != 0 || H > 256) {
+        set_error("%s: the tensor-core similarity needs encode_size %% 4 == 0 and <= 256 (got %d)", fn, H);
+        return C2V_EUNSUPPORTED;
+    }
+    return C2V_OK;
+}
+
+size_t c2v_knn_prep_workspace_bytes(int64_t N, int32_t H)
+{
+    if (N < 1 || N > kKnnMaxN || H < 4 || H > 256 || H % 4) return 0;
+    return align_up(knn_prep_bytes(N, H), 1024);
+}
+
+size_t c2v_knn_topk_workspace_bytes(int64_t N, int32_t H, int32_t Q, int32_t k)
+{
+    if (!c2v_knn_prep_workspace_bytes(N, H) || Q < 1 || Q > kKnnMaxQ || k < 1 || k > C2V_TOPK_MAX) return 0;
+    return align_up(knn_query_bytes(N, H, Q, k), 1024);
+}
+
+size_t c2v_knn_pairs_workspace_bytes(int64_t N, int32_t H, int32_t Q)
+{
+    if (!c2v_knn_prep_workspace_bytes(N, H) || Q < 1 || Q > kKnnMaxQ) return 0;
+    return align_up(knn_query_bytes(N, H, Q, 0), 1024);
+}
+
+int c2v_knn_prepare(const float *bank, int64_t N, int32_t H, void *prep, size_t prep_bytes, void *stream)
+{
+    if (!bank || !aligned16(bank)) { set_error("c2v_knn_prepare: bank is NULL or not 16-byte aligned"); return C2V_EINVAL; }
+    const int rc = knn_shape_ok("c2v_knn_prepare", N, H);
+    if (rc != C2V_OK) return rc;
+    const size_t need = knn_prep_bytes(N, H);
+    if (!prep || prep_bytes < need || !aligned16(prep)) {
+        set_error("c2v_knn_prepare: prep workspace missing, misaligned or too small: %zu < %zu", prep ? prep_bytes : (size_t)0,
+                  need);
+        return C2V_EWORKSPACE;
+    }
+    return launch_knn_prepare(bank, N, H, prep, static_cast<cudaStream_t>(stream));
+}
+
+// argument checks shared by c2v_knn_topk / c2v_knn_pairs (k == 0: pairs), all before any CUDA call
+static int knn_args_ok(const char *fn, const float *bank, long long N, int H, const float *queries, int Q, int k,
+                       const int64_t *exclude, int X, void *prep, size_t prep_bytes, const void *ws, size_t ws_bytes,
+                       int flags)
+{
+    if (!bank || !queries) { set_error("%s: NULL bank / queries", fn); return C2V_EINVAL; }
+    if (!aligned16(bank) || !aligned16(queries)) { set_error("%s: bank / queries must be 16-byte aligned", fn); return C2V_EINVAL; }
+    int rc = knn_shape_ok(fn, N, H);
+    if (rc != C2V_OK) return rc;
+    if (Q < 1 || Q > kKnnMaxQ) { set_error("%s: Q=%d: needs 1 <= Q <= %d (cut larger query sets into chunks)", fn, Q, kKnnMaxQ); return C2V_EINVAL; }
+    if (X < 0 || X > C2V_KNN_EXCLUDE_MAX || (X > 0 && !exclude)) {
+        set_error("%s: X=%d exclusions per query: needs 0 <= X <= %d and exclude != NULL when X > 0", fn, X, C2V_KNN_EXCLUDE_MAX);
+        return C2V_EINVAL;
+    }
+    if (flags & ~(C2V_FLAG_REUSE_PREP | C2V_FLAG_NO_PDL)) { set_error("%s: unknown flags 0x%x", fn, flags); return C2V_EINVAL; }
+    if (k > 0 && (k > C2V_TOPK_MAX || (long long)k > N - X)) {
+        set_error("%s: k=%d: needs 1 <= k <= %d and k <= N - X (N=%lld, X=%d)", fn, k, C2V_TOPK_MAX, N, X);
+        return C2V_EINVAL;
+    }
+    const size_t need_prep = knn_prep_bytes(N, H), need = knn_query_bytes(N, H, Q, k);
+    if (!prep || prep_bytes < need_prep || !aligned16(prep)) {
+        set_error("%s: prep workspace missing, misaligned or too small: %zu < %zu", fn, prep ? prep_bytes : (size_t)0, need_prep);
+        return C2V_EWORKSPACE;
+    }
+    if (!ws || ws_bytes < need || !aligned16(ws)) {
+        set_error("%s: workspace missing, misaligned or too small: %zu < %zu", fn, ws ? ws_bytes : (size_t)0, need);
+        return C2V_EWORKSPACE;
+    }
+    return C2V_OK;
+}
+
+static int knn_run(KnnArgs &a, int flags, void *stream)
+{
+    g_pdl_this_call = (flags & C2V_FLAG_NO_PDL) == 0;
+    a.reuse_prep = (flags & C2V_FLAG_REUSE_PREP) != 0;
+    return launch_knn(a, static_cast<cudaStream_t>(stream));
+}
+
+int c2v_knn_topk(const float *bank, int64_t N, int32_t H, const float *queries, int32_t Q, int32_t k,
+                 const int64_t *exclude, int32_t X, int64_t *indices, float *sims, void *prep, size_t prep_bytes,
+                 void *workspace, size_t workspace_bytes, int32_t flags, void *stream)
+{
+    if (!indices || !sims) { set_error("c2v_knn_topk: NULL indices / sims"); return C2V_EINVAL; }
+    if (k < 1) { set_error("c2v_knn_topk: k=%d < 1", k); return C2V_EINVAL; }
+    const int rc = knn_args_ok("c2v_knn_topk", bank, N, H, queries, Q, k, exclude, X, prep, prep_bytes, workspace,
+                               workspace_bytes, flags);
+    if (rc != C2V_OK) return rc;
+    KnnArgs a = {};
+    a.bank = bank; a.N = N; a.H = H; a.queries = queries; a.Q = Q;
+    a.exclude = X > 0 ? reinterpret_cast<const long long *>(exclude) : nullptr; a.X = X;
+    a.prep = prep; a.ws = workspace;
+    a.k = k; a.indices = reinterpret_cast<long long *>(indices); a.sims = sims;
+    return knn_run(a, flags, stream);
+}
+
+int c2v_knn_pairs(const float *bank, int64_t N, int32_t H, const float *queries, int32_t Q, float threshold,
+                  const int64_t *exclude, int32_t X, int64_t self_offset, int64_t query_base, int64_t capacity, int64_t *pair_query,
+                  int64_t *pair_index, float *pair_sim, int64_t *count, void *prep, size_t prep_bytes, void *workspace,
+                  size_t workspace_bytes, int32_t flags, void *stream)
+{
+    if (!count) { set_error("c2v_knn_pairs: NULL count"); return C2V_EINVAL; }
+    if (capacity < 0 || (capacity > 0 && (!pair_query || !pair_index || !pair_sim))) {
+        set_error("c2v_knn_pairs: capacity=%lld: needs capacity >= 0 and the three outputs when it is > 0", (long long)capacity);
+        return C2V_EINVAL;
+    }
+    if (threshold != threshold) { set_error("c2v_knn_pairs: threshold is NaN"); return C2V_EINVAL; }
+    const int rc = knn_args_ok("c2v_knn_pairs", bank, N, H, queries, Q, 0, exclude, X, prep, prep_bytes, workspace,
+                               workspace_bytes, flags);
+    if (rc != C2V_OK) return rc;
+    KnnArgs a = {};
+    a.bank = bank; a.N = N; a.H = H; a.queries = queries; a.Q = Q;
+    a.exclude = X > 0 ? reinterpret_cast<const long long *>(exclude) : nullptr; a.X = X;
+    a.prep = prep; a.ws = workspace;
+    a.threshold = threshold; a.self_offset = self_offset < 0 ? -1 : self_offset; a.query_base = query_base;
+    a.capacity = capacity;
+    a.pair_query = reinterpret_cast<long long *>(pair_query); a.pair_index = reinterpret_cast<long long *>(pair_index);
+    a.pair_sim = pair_sim; a.count = reinterpret_cast<long long *>(count);
+    return knn_run(a, flags, stream);
+}
+
 int c2v_angular_forward_train(const c2v_dims *d, const c2v_params *p, const float *code_vector, const int64_t *label,
                               int32_t B, float margin, float inverse_temp, float *outputs, float *cosine,
                               float *inv_norms, void *stream)

@@ -174,6 +174,20 @@ float *label_topk_inv_norms(const c2v_dims *d, int B, int k, void *ws);     // w
 int launch_label_tcgen05_ex(const c2v_dims *d, const float *cv, int B, const float *Wout, const float *bias,
                             float *out, long long *argmax, float *maxval, void *ws, size_t ws_bytes, bool reuse_prep,
                             cudaStream_t st, const LabelLossArgs *la);
+// similarity search over a code-vector bank on the label GEMM (c2v_knn_*): top-k mode when k > 0, pairs mode otherwise
+struct KnnArgs {
+    const float *bank; long long N; int H;
+    const float *queries; int Q;
+    const long long *exclude; int X;                          // [Q, X] or NULL
+    void *prep, *ws; bool reuse_prep;                         // knn_prep_bytes / knn_query_bytes
+    int k; long long *indices; float *sims;                   // top-k
+    float threshold; long long self_offset, query_base, capacity;    // pairs
+    long long *pair_query, *pair_index; float *pair_sim; long long *count;
+};
+size_t knn_prep_bytes(long long N, int H);
+size_t knn_query_bytes(long long N, int H, int Q, int k);
+int launch_knn_prepare(const float *bank, long long N, int H, void *prep, cudaStream_t st);
+int launch_knn(const KnnArgs &a, cudaStream_t st);
 
 // ---------------------------------------------------------------------------------
 // device helpers

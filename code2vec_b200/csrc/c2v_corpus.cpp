@@ -469,3 +469,133 @@ int c2v_write_code_vectors(const char *vector_path, const char *mode, int64_t he
 }
 
 }  // extern "C"
+
+// ---- reading the vector file back (c2v_read_code_vectors) ------------------------------------------------------------
+struct c2v_vectors {
+    std::vector<float> vec;              // [n, H]
+    std::vector<int64_t> name_off;       // [n + 1]
+    std::string names;
+    int64_t header_items = -1;
+    int32_t H = 0;
+};
+
+namespace {
+
+// `a\tb` with two integers (the header c2v_write_code_vectors writes)
+bool is_header(const char *b, const char *e, long long *items, long long *H)
+{
+    const char *t = (const char *)memchr(b, '\t', (size_t)(e - b));
+    return t && !memchr(t + 1, '\t', (size_t)(e - t - 1)) && parse_int(b, t, items) && parse_int(t + 1, e, H);
+}
+
+// one `name\tv0 v1 ...` line (without its '\n'); H < 0: the first data line, which sets H
+bool read_vector_line(c2v_vectors *v, const char *b, const char *e, long long line_no, std::string *err)
+{
+    char msg[160];
+    while (e > b && (e[-1] == '\r' || e[-1] == ' ')) --e;
+    const char *t = (const char *)memchr(b, '\t', (size_t)(e - b));
+    if (!t) {
+        snprintf(msg, sizeof(msg), "line %lld: no tab between the name and the values", line_no);
+        *err = msg;
+        return false;
+    }
+    const size_t n0 = v->vec.size();
+    const char *p = t + 1;
+    while (true) {
+        while (p < e && *p == ' ') ++p;
+        if (p == e) break;
+        double x = 0.0;
+        // from_chars: correctly rounded like strtod, but independent of the process locale; it takes no leading '+'
+        const auto r = std::from_chars(p + (*p == '+'), e, x);
+        if (r.ec == std::errc::invalid_argument || (r.ptr < e && *r.ptr != ' ')) {
+            snprintf(msg, sizeof(msg), "line %lld: value %zu is not a number", line_no, v->vec.size() - n0);
+            *err = msg;
+            return false;
+        }
+        if (r.ec == std::errc::result_out_of_range)      // what strtod returns there: +-HUGE_VAL or a denormal / zero
+            x = strtod(std::string(p, r.ptr).c_str(), nullptr);
+        v->vec.push_back((float)x);
+        p = r.ptr;
+    }
+    const long long got = (long long)(v->vec.size() - n0);
+    if (v->H == 0) v->H = (int32_t)got;
+    if (got != v->H || got == 0) {
+        snprintf(msg, sizeof(msg), "line %lld: %lld values, expected %d", line_no, got, v->H);
+        *err = msg;
+        return false;
+    }
+    v->names.append(b, (size_t)(t - b));
+    v->name_off.push_back((int64_t)v->names.size());
+    return true;
+}
+
+}  // namespace
+
+extern "C" {
+
+int c2v_read_code_vectors(const char *path, int32_t header, c2v_vectors **out)
+{
+    if (!path || !out || header < -1 || header > 1) { set_error("c2v_read_code_vectors: bad argument"); return C2V_EINVAL; }
+    const int fd = open(path, O_RDONLY);
+    if (fd < 0) { set_error("cannot open %s: %s", path, strerror(errno)); return C2V_EINVAL; }
+    struct stat st;
+    if (fstat(fd, &st) != 0) { set_error("fstat %s: %s", path, strerror(errno)); close(fd); return C2V_EINVAL; }
+    const size_t size = (size_t)st.st_size;
+    const char *m = nullptr;
+    if (size > 0) {
+        void *mp = mmap(nullptr, size, PROT_READ, MAP_PRIVATE, fd, 0);
+        if (mp == MAP_FAILED) { set_error("mmap %s: %s", path, strerror(errno)); close(fd); return C2V_EINVAL; }
+        madvise(mp, size, MADV_SEQUENTIAL);
+        m = (const char *)mp;
+    }
+    close(fd);
+    c2v_vectors *v = new c2v_vectors();
+    v->name_off.push_back(0);
+    std::string err;
+    bool ok = true;
+    long long line_no = 0;
+    for (size_t pos = 0; pos < size && ok;) {
+        const char *b = m + pos;
+        const char *nl = (const char *)memchr(b, '\n', size - pos);
+        const char *e = nl ? nl : m + size;
+        pos = (size_t)(e - m) + 1;
+        ++line_no;
+        if (line_no == 1 && header != 0) {
+            long long items = 0, H = 0;
+            if (is_header(b, e, &items, &H)) {
+                if (H < 1 || H > (1 << 20)) { err = "line 1: header encode_size out of range"; ok = false; break; }
+                v->header_items = items; v->H = (int32_t)H;
+                continue;
+            }
+            if (header == 1) { err = "line 1: expected the `n_items\\tencode_size` header"; ok = false; break; }
+        }
+        ok = read_vector_line(v, b, e, line_no, &err);
+    }
+    if (m) munmap((void *)m, size);
+    if (!ok) { set_error("%s: %s", path, err.c_str()); delete v; return C2V_EINVAL; }
+    *out = v;
+    return C2V_OK;
+}
+
+int c2v_vectors_get_info(const c2v_vectors *v, c2v_vectors_info *info)
+{
+    if (!v || !info) { set_error("c2v_vectors_get_info: NULL argument"); return C2V_EINVAL; }
+    info->n = (int64_t)(v->name_off.size() - 1);
+    info->header_items = v->header_items;
+    info->H = v->H; info->reserved = 0;
+    info->name_bytes = (int64_t)v->names.size();
+    return C2V_OK;
+}
+
+int c2v_vectors_export(const c2v_vectors *v, float *vectors, int64_t *name_offsets, char *name_blob)
+{
+    if (!v) { set_error("c2v_vectors_export: NULL handle"); return C2V_EINVAL; }
+    if (vectors && !v->vec.empty()) memcpy(vectors, v->vec.data(), v->vec.size() * sizeof(float));
+    if (name_offsets) memcpy(name_offsets, v->name_off.data(), v->name_off.size() * sizeof(int64_t));
+    if (name_blob && !v->names.empty()) memcpy(name_blob, v->names.data(), v->names.size());
+    return C2V_OK;
+}
+
+void c2v_vectors_free(c2v_vectors *v) { delete v; }
+
+}  // extern "C"

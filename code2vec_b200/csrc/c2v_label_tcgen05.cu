@@ -163,6 +163,16 @@ struct LtLoss {
     unsigned long long *topk; // top-k mode: per CTA 512 lists (column quarter x 128 rows) of topk_k keys, see lt_topk_insert
     int topk_k;
 };
+// Similarity modes (SIM != 0; the label modes pass it zeroed).  Its own parameter, behind all the others, so that the label
+// instantiations keep their parameter layout.  LtLoss's icv / iw are then the row factors of sim_prep_kernel, so that the
+// epilogue's value is the cosine itself.
+struct LtSim {
+    const long long *excl; int excl_n;        // [M, excl_n] columns that never enter row m's results (< 0: none) or NULL
+    float thr; long long self_off;            // pairs: cos >= thr; self_off >= 0: row m is column self_off + m, keep col > it
+    long long *pq, *pi; float *ps;            // pairs out: (qbase + row, column, cos) while the slot is < cap
+    long long qbase;
+    long long cap; unsigned long long *pcount; // pairs: every match adds 1 to *pcount (whatever cap is)
+};
 
 // Top-k mode (the label_gemm_v2_kernel<*, true> instantiations): a thread of the epilogue (one row, one column quarter of
 // its CTA's m-tile) keeps the topk_k largest keys  lt_orderable(v) << 32 | ~col  it has seen, sorted descending, in its
@@ -221,13 +231,18 @@ constexpr int SMEM_BYTES = SMEM_BAR_OFF + 128 + 1024;
 // ANG: the angular-margin epilogue (see LtLoss); a template parameter so that the plain head compiles without it.
 // TOPK: the running top-k epilogue (lt_topk_insert) instead of logits / arg-max / dlogits; needs lane order (per_m > 0,
 // a CTA sees every column of its slice for its rows).  With ANG the logits are s cos without the margin: no label is read.
-template <bool ANG, bool TOPK>
+// SIM (with ANG, lane order, hdr unused): similarity search over a code-vector bank (c2v_knn_*), the value being the cosine
+// itself (see LtSim).  SIM_KNN is the top-k mode with the columns of sm.excl left out; SIM_PAIRS writes every
+// (row, column, cos) with cos >= sm.thr instead.
+constexpr int SIM_NONE = 0, SIM_KNN = 1, SIM_PAIRS = 2;
+template <bool ANG, bool TOPK, int SIM = SIM_NONE>
 __global__ void __launch_bounds__(lt2::THREADS, 1)
 label_gemm_v2_kernel(const uint8_t *__restrict__ imgA, const uint8_t *__restrict__ imgB,
                      const float *__restrict__ bias, const float *__restrict__ hdr, float *__restrict__ out,
                      int M, long long N, int nkb, int n_mt, long long n_nt, long long n_tiles,
                      unsigned long long *__restrict__ keys, unsigned *__restrict__ ticket,
-                     long long *__restrict__ argmax, float *__restrict__ maxval, int dbg, const LtLoss ls, const int per_m)
+                     long long *__restrict__ argmax, float *__restrict__ maxval, int dbg, const LtLoss ls, const int per_m,
+                     const LtSim sm)
 {
     extern __shared__ unsigned char smem_raw[];
     const uint32_t raw = lt_smem_u32(smem_raw);
@@ -284,7 +299,7 @@ label_gemm_v2_kernel(const uint8_t *__restrict__ imgA, const uint8_t *__restrict
         // ---- epilogue: thread = output row x 32 columns.  Bounds and addresses are hoisted out of the
         //      per-element code (the epilogue is issue-bound otherwise).
         const int q = warp & 3, cq = warp >> 2;
-        const float inv_scale = hdr[0];
+        const float inv_scale = SIM != SIM_NONE ? 1.0f : hdr[0];
         const bool vec_ok = (N % 4 == 0);
         float *stg = stage_all + warp * 32 * lt2::STG_LD;
         float *sbias = reinterpret_cast<float *>(smem + lt2::SMEM_BIAS_OFF) + warp * 32;
@@ -310,6 +325,36 @@ label_gemm_v2_kernel(const uint8_t *__restrict__ imgA, const uint8_t *__restrict
             tk_list = ls.topk + ((size_t)blockIdx.x * 512 + cq * 128 + q * 32 + lane) * ls.topk_k;
             for (int j = 0; j < ls.topk_k; ++j) tk_list[j] = 0ull;
         }
+        // similarity: this thread's excluded columns (0xFFFFFFFF: none), loaded once -- in lane order the row is fixed -- into
+        // its slot of the arg-max table, which these modes do not use (in registers they would spill).  A column >= N lands
+        // in the last tile's invalid columns (j >= n_cols), which never count anyway.
+        static_assert(C2V_KNN_EXCLUDE_MAX == 4 && lt2::N_EPI_WARPS * 32 * 16 <= lt2::TAB_BYTES, "one uint4 per thread");
+        if constexpr (SIM != SIM_NONE) {
+            uint32_t ex[4] = {0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu};
+            const long long grow = (long long)rg.mt * lt::TM + q * 32 + lane;
+            if (sm.excl && grow < M) {
+#pragma unroll
+                for (int u = 0; u < 4; ++u)
+                    if (u < sm.excl_n) {
+                        const long long x = sm.excl[grow * sm.excl_n + u];
+                        ex[u] = (x >= 0 && x < N) ? (uint32_t)x : 0xFFFFFFFFu;
+                    }
+            }
+            asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(base + lt2::SMEM_TAB_OFF + 16u * threadIdx.x),
+                         "r"(ex[0]), "r"(ex[1]), "r"(ex[2]), "r"(ex[3]) : "memory");
+        }
+        auto excl_mask = [&](long long c0) {                 // bit j: column c0 + j is excluded for this thread's row
+            uint32_t ex[4];
+            asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(ex[0]), "=r"(ex[1]), "=r"(ex[2]), "=r"(ex[3])
+                         : "r"(base + lt2::SMEM_TAB_OFF + 16u * threadIdx.x) : "memory");
+            uint32_t m = 0;
+#pragma unroll
+            for (int u = 0; u < 4; ++u) {
+                const uint32_t dl = ex[u] - (uint32_t)c0;
+                m |= dl < 32u ? 1u << dl : 0u;
+            }
+            return m;
+        };
         for (int i = 0; i < my_tiles; ++i) {
             const LtTile tt = tile_of(i);
             const long long nt = tt.nt; const int mt = tt.mt;
@@ -381,7 +426,8 @@ label_gemm_v2_kernel(const uint8_t *__restrict__ imgA, const uint8_t *__restrict
                     v[j] = r[j] * inv_scale * icv_r * w4.x; v[j + 1] = r[j + 1] * inv_scale * icv_r * w4.y;
                     v[j + 2] = r[j + 2] * inv_scale * icv_r * w4.z; v[j + 3] = r[j + 3] * inv_scale * icv_r * w4.w;
                 }
-                if constexpr (TOPK) {                                               // label-free: s cos, no margin
+                if constexpr (SIM != SIM_NONE) {                                    // the cosine itself
+                } else if constexpr (TOPK) {                                        // label-free: s cos, no margin
 #pragma unroll
                     for (int j = 0; j < 32; ++j) v[j] *= ls.s;
                 } else {
@@ -402,7 +448,7 @@ label_gemm_v2_kernel(const uint8_t *__restrict__ imgA, const uint8_t *__restrict
                     for (int j = 0; j < 32; ++j) v[j] = (j == tji ? phi : v[j]) * ls.s;
                 }
             }
-            if (ls.part || ls.lse) {
+            if (SIM != SIM_PAIRS && (ls.part || ls.lse)) {
                 const long long grow = row0 + lane;                                     // this thread's output row
                 const long long lab = (grow < M && ls.label) ? ls.label[grow] : -1;
                 const long long tj = lab - col0;                                        // label's column inside this block
@@ -479,10 +525,50 @@ label_gemm_v2_kernel(const uint8_t *__restrict__ imgA, const uint8_t *__restrict
                         const int j = __ffs(cand) - 1;
                         cand &= cand - 1;
                         const uint32_t h = ks[j];
-                        if (h > tk_thr)
+                        // an excluded column never enters the list (checked here, on the rare candidates, not per element)
+                        if (h > tk_thr && (SIM != SIM_KNN || !((excl_mask(col0) >> j) & 1u)))
                             tk_thr = lt_topk_insert(tk_list, ls.topk_k, ((unsigned long long)h << 32) |
                                                                             (unsigned long long)(0xFFFFFFFFu - (uint32_t)(col0 + j)));
                     } while (cand);
+                }
+                __syncwarp();
+                continue;
+            }
+            if constexpr (SIM == SIM_PAIRS) {
+                // the row's matches in this block; one atomic per warp reserves the slots of all 32 rows (exclusive scan of
+                // the per-thread counts), and the count grows by every match even where the slots run out
+                const long long grow = row0 + lane;
+                uint32_t hit = 0;
+                if (lane < n_rows) {
+                    const long long lim = sm.self_off >= 0 ? sm.self_off + grow : -1;
+#pragma unroll
+                    for (int j = 0; j < 32; ++j) hit |= (j < n_cols && v[j] >= sm.thr && col0 + j > lim) ? (1u << j) : 0u;
+                    hit &= ~excl_mask(col0);
+                }
+                const int nh = __popc(hit);
+                int incl = nh;
+#pragma unroll
+                for (int o = 1; o < 32; o <<= 1) {
+                    const int t = __shfl_up_sync(0xffffffffu, incl, o);
+                    if (lane >= o) incl += t;
+                }
+                const int tot = __shfl_sync(0xffffffffu, incl, 31);
+                if (tot) {
+                    unsigned long long base = 0;
+                    if (lane == 31) base = atomicAdd(sm.pcount, (unsigned long long)tot);
+                    long long slot = (long long)__shfl_sync(0xffffffffu, base, 31) + (incl - nh);
+                    if (hit) {
+                        // the row's values go back to its own staging slot (read above), so that the loop can index them
+                        float *vs = stage_all + (q * 32 + lane) * xld + xcol;
+#pragma unroll
+                        for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4 *>(vs + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
+                        do {
+                            const int j = __ffs(hit) - 1;
+                            hit &= hit - 1;
+                            if (slot < sm.cap) { sm.pq[slot] = sm.qbase + grow; sm.pi[slot] = col0 + j; sm.ps[slot] = vs[j]; }
+                            ++slot;
+                        } while (hit);
+                    }
                 }
                 __syncwarp();
                 continue;
@@ -904,7 +990,7 @@ int launch_label_tcgen05_ex(const c2v_dims *d, const float *cv, int B, const flo
                            (const uint8_t *)imgA, (const uint8_t *)imgB, bias, (const float *)hdr, out, B, C, nkb, (int)mt,
                            (long long)nt, n_tiles, fused_arg ? keys : (unsigned long long *)nullptr, ticket,
                            fused_arg ? argmax : (long long *)nullptr, fused_arg ? maxval : (float *)nullptr,
-                           getenv("C2V_K2_FLAGS") ? atoi(getenv("C2V_K2_FLAGS")) : 0, ls, per_m));
+                           getenv("C2V_K2_FLAGS") ? atoi(getenv("C2V_K2_FLAGS")) : 0, ls, per_m, LtSim{}));
     C2V_LAUNCH_OK("label_gemm_v2_kernel");
     if (want_loss) {
         loss_partials_reduce_kernel<<<dim3((unsigned)(Mpad / 32), LT_PSPLIT), 256, 0, st>>>(part, (int)(nt * 4), Mpad, part2);
@@ -925,6 +1011,151 @@ int launch_label_tcgen05_ex(const c2v_dims *d, const float *cv, int B, const flo
     if (want_arg && !fused_arg) {
         if (!out) { set_error("label loss without logits: arg-max needs B <= %d", lt2::MAX_MT * 128); return C2V_EUNSUPPORTED; }
         return launch_loss_argmax(out, nullptr, B, C, nullptr, argmax, maxval, nullptr, st);
+    }
+    return C2V_OK;
+}
+
+// ---- similarity search over a code-vector bank (c2v_knn_*) -----------------------------------------------------------
+// Rows -> the GEMM operand image (split_rows_kernel's layout), each row scaled by its own power of two 2^k so that its
+// largest element lands in [2^13, 2^14) (fp16's range is used in full whatever the row's magnitude), and
+// fac[r] = 1 / max(|x_r 2^k|, 1e-12 2^k) = 2^-k / max(|x_r|, 1e-12).  Then cos(q, b) = (q 2^kq . b 2^kb) fac_q fac_b, with
+// F.normalize's clamp; a zero row has fac = 1e12 and a zero dot product, so similarity 0.  One warp per row of the
+// 128-row padded range (rows >= R are zero).  H % 4 == 0 and H <= 256: two float4 groups per lane.
+__global__ void __launch_bounds__(256)
+sim_prep_kernel(const float *__restrict__ X, long long R, int H, int nkb, uint8_t *__restrict__ img, float *__restrict__ fac)
+{
+    const int lane = threadIdx.x & 31;
+    const long long rows = (R + 127) / 128 * 128;
+    const long long wstride = ((long long)gridDim.x * blockDim.x) >> 5;
+    for (long long row = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; row < rows; row += wstride) {
+        float4 v[2];
+        float m = 0.0f;
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+            const int k = (lane + 32 * u) * 4;
+            v[u] = (row < R && k < H) ? *reinterpret_cast<const float4 *>(X + row * H + k) : make_float4(0.f, 0.f, 0.f, 0.f);
+            m = fmaxf(m, fmaxf(fmaxf(fabsf(v[u].x), fabsf(v[u].y)), fmaxf(fabsf(v[u].z), fabsf(v[u].w))));
+        }
+        m = warp_max(m);
+        int e = 14;                                            // zero or non-finite rows: scale 1
+        if (m > 0.0f && m <= 3.4e38f) frexpf(m, &e);
+        const int ks = 14 - e > 126 ? 126 : (14 - e < -126 ? -126 : 14 - e);
+        const float sc = ldexpf(1.0f, ks);
+        float ss = 0.0f;
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+            v[u].x *= sc; v[u].y *= sc; v[u].z *= sc; v[u].w *= sc;
+            ss += v[u].x * v[u].x + v[u].y * v[u].y + v[u].z * v[u].z + v[u].w * v[u].w;
+        }
+        ss = warp_sum(ss);
+        if (lane == 0 && row < R) fac[row] = 1.0f / fmaxf(sqrtf(ss), 1e-12f * sc);
+        const long long tile = row >> 7;
+        const int r = (int)(row & 127);
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+            const int k = (lane + 32 * u) * 4;
+            if (k >= nkb * lt::KB) continue;
+            const __half2 h01 = __floats2half2_rn(v[u].x, v[u].y), h23 = __floats2half2_rn(v[u].z, v[u].w);
+            const float2 f01 = __half22float2(h01), f23 = __half22float2(h23);
+            const __half2 l01 = __floats2half2_rn(v[u].x - f01.x, v[u].y - f01.y);
+            const __half2 l23 = __floats2half2_rn(v[u].z - f23.x, v[u].w - f23.y);
+            uint8_t *base = img + (tile * nkb + k / lt::KB) * (size_t)(2 * lt::TILE_BYTES);
+            const uint32_t off = lt_sw128(r, k % lt::KB);
+            *reinterpret_cast<uint2 *>(base + off) = make_uint2(*reinterpret_cast<const unsigned *>(&h01), *reinterpret_cast<const unsigned *>(&h23));
+            *reinterpret_cast<uint2 *>(base + lt::TILE_BYTES + off) = make_uint2(*reinterpret_cast<const unsigned *>(&l01), *reinterpret_cast<const unsigned *>(&l23));
+        }
+    }
+}
+
+// prep workspace (the bank's image, then fac [N]): depends on N and H only, so one prep serves every query chunk
+size_t knn_prep_bytes(long long N, int H)
+{
+    const size_t nkb = (size_t)(H + 63) / 64, nt = (size_t)((N + 127) / 128);
+    return nt * nkb * 2 * lt::TILE_BYTES + align_up((size_t)N * sizeof(float), 1024);
+}
+// call workspace: the query image, fac [Q], then (top-k) 512 lists of k keys per CTA of the GEMM
+size_t knn_query_bytes(long long N, int H, int Q, int k)
+{
+    const size_t nkb = (size_t)(H + 63) / 64, mt = (size_t)(Q + 127) / 128;
+    const long long n_tiles = (long long)mt * ((N + 127) / 128);
+    const size_t ctas = (size_t)(n_tiles < LT_TOPK_MAX_CTAS ? n_tiles : LT_TOPK_MAX_CTAS);
+    return mt * nkb * 2 * lt::TILE_BYTES + align_up((size_t)Q * sizeof(float), 1024) + align_up(ctas * 512 * (size_t)k * 8, 1024);
+}
+
+static int launch_sim_prep(const float *X, long long R, int H, uint8_t *img, float *fac, int sms, cudaStream_t st)
+{
+    const long long blocks = ((R + 127) / 128 * 128 + 7) / 8;             // 8 warps (rows) per block
+    sim_prep_kernel<<<(unsigned)(blocks < sms * 32ll ? blocks : sms * 32ll), 256, 0, st>>>(X, R, H, (H + 63) / 64, img, fac);
+    C2V_LAUNCH_OK("sim_prep_kernel");
+    return C2V_OK;
+}
+
+static int knn_sms(int *sms)
+{
+    int dev = 0;
+    C2V_CUDA_OK(cudaGetDevice(&dev));
+    C2V_CUDA_OK(cudaDeviceGetAttribute(sms, cudaDevAttrMultiProcessorCount, dev));
+    return C2V_OK;
+}
+
+int launch_knn_prepare(const float *bank, long long N, int H, void *prep, cudaStream_t st)
+{
+    int sms = 0;
+    const int rc = knn_sms(&sms);
+    if (rc != C2V_OK) return rc;
+    uint8_t *img = static_cast<uint8_t *>(prep);
+    const size_t nt = (size_t)((N + 127) / 128), nkb = (size_t)(H + 63) / 64;
+    return launch_sim_prep(bank, N, H, img, reinterpret_cast<float *>(img + nt * nkb * 2 * lt::TILE_BYTES), sms, st);
+}
+
+// The arguments were checked by the caller (c2v_knn_topk / c2v_knn_pairs): Q <= 2048, H % 4 == 0, H <= 256, N < 2^32 - 1,
+// workspaces of knn_prep_bytes / knn_query_bytes.
+int launch_knn(const KnnArgs &a, cudaStream_t st)
+{
+    int sms = 0;
+    int rc = knn_sms(&sms);
+    if (rc != C2V_OK) return rc;
+    const int H = a.H, nkb = (H + 63) / 64;
+    const long long N = a.N;
+    const size_t mt = (size_t)(a.Q + 127) / 128, nt = (size_t)((N + 127) / 128);
+    uint8_t *imgB = static_cast<uint8_t *>(a.prep);
+    const float *fb = reinterpret_cast<const float *>(imgB + nt * nkb * 2 * lt::TILE_BYTES);
+    uint8_t *imgA = static_cast<uint8_t *>(a.ws);
+    float *fq = reinterpret_cast<float *>(imgA + mt * nkb * 2 * lt::TILE_BYTES);
+    unsigned long long *lists = reinterpret_cast<unsigned long long *>(reinterpret_cast<uint8_t *>(fq) +
+                                                                       align_up((size_t)a.Q * sizeof(float), 1024));
+    if (!a.reuse_prep && (rc = launch_knn_prepare(a.bank, N, H, a.prep, st)) != C2V_OK) return rc;
+    if ((rc = launch_sim_prep(a.queries, a.Q, H, imgA, fq, sms, st)) != C2V_OK) return rc;
+
+    LtLoss ls;
+    memset(&ls, 0, sizeof(ls));
+    ls.icv = fq; ls.iw = fb;
+    LtSim sm = {};
+    sm.excl = a.exclude; sm.excl_n = a.exclude ? a.X : 0;
+    const bool topk = a.k > 0;
+    if (topk) {
+        ls.topk = lists; ls.topk_k = a.k;
+    } else {
+        sm.thr = a.threshold; sm.self_off = a.self_offset; sm.cap = a.capacity; sm.qbase = a.query_base;
+        sm.pq = a.pair_query; sm.pi = a.pair_index; sm.ps = a.pair_sim;
+        sm.pcount = reinterpret_cast<unsigned long long *>(a.count);
+    }
+    auto *kern = topk ? label_gemm_v2_kernel<true, true, SIM_KNN> : label_gemm_v2_kernel<true, false, SIM_PAIRS>;
+    C2V_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, lt2::SMEM_BYTES));
+    const long long n_tiles = (long long)mt * (long long)nt;
+    int grid = (int)(n_tiles < sms ? n_tiles : sms);
+    if (grid > LT_TOPK_MAX_CTAS) grid = LT_TOPK_MAX_CTAS;
+    const int per_m = grid / (int)mt;                       // lane order: a CTA keeps one m-tile, so its rows are fixed
+    if (per_m < 1) { set_error("similarity search: %d SMs for %zu m-tiles", sms, mt); return C2V_EUNSUPPORTED; }
+    C2V_CUDA_OK(launch_pdl(kern, dim3((unsigned)grid), dim3(lt2::THREADS), (size_t)lt2::SMEM_BYTES, st, (const uint8_t *)imgA,
+                           (const uint8_t *)imgB, (const float *)nullptr, (const float *)nullptr, (float *)nullptr, a.Q, N, nkb,
+                           (int)mt, (long long)nt, n_tiles, (unsigned long long *)nullptr, (unsigned *)nullptr,
+                           (long long *)nullptr, (float *)nullptr, 0, ls, per_m, sm));
+    C2V_LAUNCH_OK("label_gemm_v2_kernel");
+    if (topk) {
+        topk_merge_kernel<<<(unsigned)((a.Q + 7) / 8), 256, 0, st>>>(lists, a.k, a.Q, (int)mt, per_m, nullptr, 0,
+                                                                     a.indices, a.sims, nullptr);
+        C2V_LAUNCH_OK("topk_merge_kernel");
     }
     return C2V_OK;
 }

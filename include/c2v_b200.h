@@ -271,6 +271,43 @@ int c2v_angular_topk(const c2v_dims *d, const c2v_params *p, const float *code_v
                      float inverse_temp, int64_t *indices, float *values, float *probs, void *workspace,
                      size_t workspace_bytes, int32_t algo, void *stream);
 
+/* ---- similarity search over code vectors (not in the reference) ----------------------------------------------------
+ * A bank of N code vectors bank [N, H] and queries [Q, H] (fp32, device, 16-byte aligned).  The similarity is
+ *   cos(q, b) = (q . b) / (max(|q|, 1e-12) max(|b|, 1e-12))       (F.normalize's clamp: a zero vector scores 0)
+ * computed on the tensor cores with the label GEMM's fp32-accurate 3-pass fp16 hi / lo split (each row scaled by its own
+ * power of two first); no [Q, N] block is ever written.  Results rank by similarity descending, then bank index ascending
+ * (torch.sort(descending=True, stable=True)).  Supported: 4 <= H <= 256, H % 4 == 0 (else C2V_EUNSUPPORTED),
+ * 1 <= N < 2^32 - 1, 1 <= Q <= 2048.
+ * prep: caller-owned, c2v_knn_prep_workspace_bytes(N, H): the bank's fp16 hi / lo image and its row factors (the inverse
+ * norms).  c2v_knn_prepare builds it; a query call builds it too unless `flags` holds C2V_FLAG_REUSE_PREP, which promises
+ * that prep holds the prepared image of this same bank, unchanged since.  workspace: per call, c2v_knn_*_workspace_bytes.
+ * flags: C2V_FLAG_REUSE_PREP, C2V_FLAG_NO_PDL.
+ * exclude: int64 [Q, X] (X <= C2V_KNN_EXCLUDE_MAX) bank rows that never appear in query q's results, e.g. the query's own
+ * row, or the inputs of an analogy; entries < 0 (or >= N) are ignored.  NULL when X == 0.
+ * All argument checks run before any CUDA call. */
+#define C2V_KNN_EXCLUDE_MAX 4
+size_t c2v_knn_prep_workspace_bytes(int64_t N, int32_t H);
+int c2v_knn_prepare(const float *bank, int64_t N, int32_t H, void *prep, size_t prep_bytes, void *stream);
+/* The k most similar non-excluded bank rows of every query: indices int64 [Q, k], sims fp32 [Q, k].
+ * 1 <= k <= C2V_TOPK_MAX and k <= N - X (C2V_EINVAL otherwise). */
+size_t c2v_knn_topk_workspace_bytes(int64_t N, int32_t H, int32_t Q, int32_t k);
+int c2v_knn_topk(const float *bank, int64_t N, int32_t H, const float *queries, int32_t Q, int32_t k,
+                 const int64_t *exclude, int32_t X, int64_t *indices, float *sims, void *prep, size_t prep_bytes,
+                 void *workspace, size_t workspace_bytes, int32_t flags, void *stream);
+/* Every (query, bank row) pair with cos >= threshold that is not excluded.  self_offset >= 0 marks a self-join: query i
+ * is bank row self_offset + i, and only rows index > self_offset + i are reported (each unordered pair once, never the
+ * query itself); self_offset < 0: every bank row is a candidate.  A match of query i and bank row j is written as
+ * pair_query[slot] = query_base + i, pair_index[slot] = j (int64) and pair_sim[slot] (fp32), slot being the value *count
+ * had plus the matches before it, while slot < capacity; *count (int64,
+ * device) grows by the exact number of matches in any case, so that the caller sees an overflow and can re-run with
+ * capacity >= *count.  The caller zeroes *count; consecutive calls without a reset append to the same buffers.  The order
+ * of the pairs is unspecified.  capacity >= 0 (the outputs may be NULL when it is 0: a counting pass). */
+size_t c2v_knn_pairs_workspace_bytes(int64_t N, int32_t H, int32_t Q);
+int c2v_knn_pairs(const float *bank, int64_t N, int32_t H, const float *queries, int32_t Q, float threshold,
+                  const int64_t *exclude, int32_t X, int64_t self_offset, int64_t query_base, int64_t capacity, int64_t *pair_query,
+                  int64_t *pair_index, float *pair_sim, int64_t *count, void *prep, size_t prep_bytes, void *workspace,
+                  size_t workspace_bytes, int32_t flags, void *stream);
+
 /* ---- loss / predict next to the path ----------------------------------------------
  * main.py:251-264: mean over the batch of -log_softmax(outputs)[label] (NLLLoss
  * weights are identically 1); main.py:285: torch.max(dim=1).
@@ -497,6 +534,24 @@ int c2v_write_code_vectors(const char *vector_path, const char *mode, int64_t he
                            const float *code_vectors, const int64_t *label, const char *names_blob,
                            const int64_t *name_offsets, int64_t n_names, const char *result_path, const char *result_mode,
                            const int64_t *ids, const int64_t *pred_label, const float *pred_score);
+
+/* Reader of the vector file c2v_write_code_vectors writes (word2vec text format): an optional `n_items\tencode_size`
+ * header, then `name\tv0 v1 ...` lines.  header: 1 = the first line is the header, 0 = there is none, -1 = auto (the
+ * first line is a header when it is two tab-separated integers).  H comes from the header, else from the first line;
+ * every line must hold H values (C2V_EINVAL naming the line otherwise).  The header's item count is reported, not
+ * enforced.  Values are parsed as doubles, correctly rounded, then cast to fp32, so a write followed by a read is
+ * bit-exact (-0.0, subnormals, inf; every NaN reads back as a NaN).  Host-only. */
+typedef struct c2v_vectors c2v_vectors;
+typedef struct c2v_vectors_info {
+    int64_t n, header_items;   /* rows read; the header's item count or -1 */
+    int32_t H, reserved;
+    int64_t name_bytes;
+} c2v_vectors_info;
+int c2v_read_code_vectors(const char *path, int32_t header, c2v_vectors **out);
+int c2v_vectors_get_info(const c2v_vectors *v, c2v_vectors_info *info);
+/* vectors fp32 [n, H], name_offsets [n + 1] into name_blob (UTF-8, not terminated); any pointer may be NULL = skip */
+int c2v_vectors_export(const c2v_vectors *v, float *vectors, int64_t *name_offsets, char *name_blob);
+void c2v_vectors_free(c2v_vectors *v);
 
 /* Counts kernels launched by this library since load (bench.py's gpu_launches). */
 int64_t c2v_launch_count(void);
