@@ -39,6 +39,10 @@ class Dropout(ctypes.Structure):
     _fields_ = [("p", c_f32), ("training", c_i32), ("seed", ctypes.c_uint64)]
 
 
+class RowSlots(ctypes.Structure):
+    _fields_ = [("terminal", c_vp), ("path", c_vp)]
+
+
 class DeviceInfo(ctypes.Structure):
     _fields_ = [("cc_major", c_i32), ("cc_minor", c_i32), ("sm_count", c_i32), ("reserved", c_i32),
                 ("global_mem_bytes", c_i64), ("smem_per_block_optin", c_i64)]
@@ -123,6 +127,16 @@ SYMBOLS = {
                                                    c_vp, c_vp, c_vp, c_vp, c_vp, _P(Grads), c_vp, c_sz, c_vp]),
     "c2v_encode_backward_phased": (ctypes.c_int, [_P(Dims), _P(Params), c_vp, c_vp, c_vp, c_i32, c_i32, _P(Dropout),
                                                   c_vp, c_vp, c_vp, c_vp, c_vp, _P(Grads), c_vp, c_sz, c_i32, c_vp]),
+    "c2v_sparse_rows_workspace_bytes": (c_sz, [c_i64]),
+    "c2v_sparse_rows": (ctypes.c_int, [c_vp, c_i64, c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_sz, c_vp]),
+    "c2v_encode_backward_sparse": (ctypes.c_int, [_P(Dims), _P(Params), c_vp, c_vp, c_vp, c_i32, c_i32, _P(Dropout),
+                                                  c_vp, c_vp, c_vp, c_vp, c_vp, _P(Grads), _P(RowSlots), c_vp, c_sz, c_i32,
+                                                  c_vp]),
+    "c2v_encode_backward_packed_sparse": (ctypes.c_int, [_P(Dims), _P(Params), c_vp, c_vp, c_vp, c_vp, c_i32, c_i64, c_i32,
+                                                         _P(Dropout), c_vp, c_vp, c_vp, c_vp, c_vp, _P(Grads), _P(RowSlots),
+                                                         c_vp, c_sz, c_i32, c_vp]),
+    "c2v_sparse_adam_step": (ctypes.c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_i32, ctypes.c_double,
+                                            ctypes.c_double, ctypes.c_double, ctypes.c_double, c_i64, c_vp]),
     "c2v_session_create": (ctypes.c_int, [ctypes.c_int, _P(Dims), c_i32, c_i32, _P(c_vp)]),
     "c2v_session_destroy": (None, [c_vp]),
     "c2v_forward_host": (ctypes.c_int, [c_vp, _P(Params), c_vp, c_vp, c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp,

@@ -3,7 +3,8 @@
 // optimizer.zero_grad() (:171) for ALL parameters in one launch over flat fp32 buffers: reads p, g, m, v once, writes
 // p, m, v and the zeroed gradient (ready for the next backward), and folds the 1/world of the data-parallel mean into
 // the gradient read (the all_reduce then is a plain sum).  Dense on purpose: momentum keeps moving embedding rows that
-// received no gradient, so a row-sparse Adam would not be the reference's optimizer.
+// received no gradient, so a row-sparse Adam would not be the reference's optimizer.  That row-sparse Adam
+// (torch.optim.SparseAdam, for tables with sparse gradients) is sparse_adam_step_kernel at the end of this file, opt-in.
 // Same operation order as torch's single-tensor Adam (amsgrad=False, maximize=False):
 //   g += wd * p;  m += (g - m) * (1 - b1);  v = v * b2 + (1 - b2) * g * g;
 //   p -= (lr / (1 - b1^t)) * m / (sqrt(v) / sqrt(1 - b2^t) + eps)
@@ -245,9 +246,40 @@ adam_step_bulk_kernel(const float *__restrict__ p_local, const AdamPeers peers, 
     __threadfence_system();
 }
 
+// ------------------------------------------------------------------------------------------------------------------
+// torch.optim._functional.sparse_adam on the rows of a coalesced gradient, every operation rounded as torch rounds it
+// (the _rn intrinsics keep nvcc from contracting a multiply and an add into one fma).  One warp per gradient row.
+// ------------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+sparse_adam_step_kernel(float *__restrict__ p, float *__restrict__ m, float *__restrict__ v, const float *__restrict__ g,
+                        const long long *__restrict__ rows, long long U, long long n_rows, int E, float neg_step_size,
+                        float one_minus_b1, float one_minus_b2, float eps)
+{
+    const int lane = threadIdx.x & 31;
+    const long long n_warps = (long long)gridDim.x * (blockDim.x >> 5);
+    for (long long i = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); i < U; i += n_warps) {
+        const long long r = rows[i];
+        if (r < 0 || r >= n_rows) continue;
+        const float *gi = g + (size_t)i * E;
+        float *pr = p + (size_t)r * E, *mr = m + (size_t)r * E, *vr = v + (size_t)r * E;
+        for (int c = lane; c < E; c += 32) {
+            const float gg = gi[c], m0 = mr[c], v0 = vr[c];
+            const float u1 = __fmul_rn(__fsub_rn(gg, m0), one_minus_b1);              // (g - m) * (1 - b1)
+            const float u2 = __fmul_rn(__fsub_rn(__fmul_rn(gg, gg), v0), one_minus_b2); // (g^2 - v) * (1 - b2)
+            mr[c] = __fadd_rn(m0, u1);
+            vr[c] = __fadd_rn(v0, u2);
+            const float numer = __fadd_rn(u1, m0);
+            const float denom = __fadd_rn(__fsqrt_rn(__fadd_rn(u2, v0)), eps);
+            pr[c] = __fadd_rn(pr[c], __fmul_rn(neg_step_size, __fdiv_rn(numer, denom)));
+        }
+    }
+}
+
 }  // namespace c2v
 
 using namespace c2v;
+
+static bool misaligned(const void *ptr, uintptr_t a) { return (reinterpret_cast<uintptr_t>(ptr) & (a - 1)) != 0; }
 
 extern "C" int c2v_adam_step(float *param, float *grad, float *exp_avg, float *exp_avg_sq, int64_t n, float lr,
                              float beta1, float beta2, float eps, float weight_decay, int64_t step, float grad_scale,
@@ -376,5 +408,39 @@ extern "C" int c2v_adam_step_sharded_bulk(const float *param_local, float *const
         param_local, peers, world, exp_avg_slice, exp_avg_sq_slice, slice_begin, slice_n, chunk, step_size, 1.0f - beta1, beta2,
         1.0f - beta2, inv_sqrt_bc2, eps, weight_decay, grad_scale);
     C2V_LAUNCH_OK("adam_step_bulk_kernel");
+    return C2V_OK;
+}
+
+extern "C" int c2v_sparse_adam_step(float *param, float *exp_avg, float *exp_avg_sq, const float *values,
+                                    const int64_t *rows, int64_t U, int64_t n_rows, int32_t E, double lr, double beta1,
+                                    double beta2, double eps, int64_t step, void *stream)
+{
+    if (U < 0 || n_rows < 1 || E < 1 || E > 65536 || step < 1) {
+        set_error("c2v_sparse_adam_step: bad argument (U = %lld, n_rows = %lld, E = %d, step = %lld)", (long long)U,
+                  (long long)n_rows, E, (long long)step);
+        return C2V_EINVAL;
+    }
+    if (!param || !exp_avg || !exp_avg_sq || (U > 0 && (!values || !rows))) {
+        set_error("c2v_sparse_adam_step: NULL pointer argument");
+        return C2V_EINVAL;
+    }
+    if (misaligned(param, 4) || misaligned(exp_avg, 4) || misaligned(exp_avg_sq, 4) || misaligned(values, 4) ||
+        misaligned(rows, 8)) {
+        set_error("c2v_sparse_adam_step: misaligned pointer (float buffers: 4 bytes, rows: 8)");
+        return C2V_EINVAL;
+    }
+    if (U == 0) return C2V_OK;
+    // torch: step_size = lr * sqrt(1 - b2^t) / (1 - b1^t) and the 1 - b factors in double, applied to float tensors
+    const double bc1 = 1.0 - pow(beta1, (double)step), bc2 = 1.0 - pow(beta2, (double)step);
+    const double step_size = lr * sqrt(bc2) / bc1;
+    int dev = 0, sms = 0;
+    C2V_CUDA_OK(cudaGetDevice(&dev));
+    C2V_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    long long blocks = (U + 7) / 8;
+    if (blocks > (long long)sms * 8) blocks = (long long)sms * 8;
+    sparse_adam_step_kernel<<<(unsigned)blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        param, exp_avg, exp_avg_sq, values, reinterpret_cast<const long long *>(rows), U, n_rows, E, (float)(-step_size),
+        (float)(1.0 - beta1), (float)(1.0 - beta2), (float)eps);
+    C2V_LAUNCH_OK("sparse_adam_step_kernel");
     return C2V_OK;
 }

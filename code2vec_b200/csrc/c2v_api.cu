@@ -43,7 +43,7 @@ int launch_colsum(const float *X, int B, long long C, float *out, cudaStream_t s
 int launch_encode_backward(const c2v_dims *d, const c2v_params *p, const EncodeArgs &a, int B,
                            const float *cv, const float *attention, const float *d_cv,
                            const float *d_att, const c2v_grads *g, void *ws, size_t ws_bytes,
-                           cudaStream_t st, const float *x_stash, int phase);
+                           cudaStream_t st, const float *x_stash, int phase, const c2v_row_slots *slots);
 size_t encode_backward_workspace_bytes(const c2v_dims *d, int B, int L);
 size_t encode_backward_workspace_bytes_n(const c2v_dims *d, int B, long long N, bool packed);
 bool label_tcgen05_shape_ok(const c2v_dims *d);
@@ -900,7 +900,8 @@ static int encode_backward_impl(const c2v_dims *d, const c2v_params *p, const in
                                 const int64_t *ends, const int64_t *offsets, int32_t B, long long N, int32_t L,
                                 const c2v_dropout *drop, const float *code_vector, const float *attention,
                                 const float *x_stash, const float *d_code_vector, const float *d_attention,
-                                const c2v_grads *grads, void *workspace, size_t workspace_bytes, int32_t phase, void *stream)
+                                const c2v_grads *grads, void *workspace, size_t workspace_bytes, int32_t phase, void *stream,
+                                const c2v_row_slots *slots = nullptr)
 {
     if (!grads->terminal_embedding || !grads->path_embedding || !grads->input_linear ||
         !grads->ln_weight || !grads->ln_bias || !grads->attention) {
@@ -926,7 +927,7 @@ static int encode_backward_impl(const c2v_dims *d, const c2v_params *p, const in
     a.n_bags = B;
     return launch_encode_backward(d, p, a, B, code_vector, attention, d_code_vector, d_attention,
                                   grads, workspace, workspace_bytes,
-                                  static_cast<cudaStream_t>(stream), x_stash, phase);
+                                  static_cast<cudaStream_t>(stream), x_stash, phase, slots);
 }
 
 int c2v_encode_backward_phased(const c2v_dims *d, const c2v_params *p, const int64_t *starts,
@@ -968,6 +969,63 @@ int c2v_encode_backward_packed(const c2v_dims *d, const c2v_params *p, const int
     if (!packed_shape_ok("c2v_encode_backward_packed", B, N, L)) return C2V_EINVAL;
     return encode_backward_impl(d, p, starts, paths, ends, offsets, B, N, L, drop, code_vector, attention, x_stash,
                                 d_code_vector, d_attention, grads, workspace, workspace_bytes, phase, stream);
+}
+
+// the checks the sparse backwards add to those of their dense counterparts
+static bool row_slots_ok(const char *fn, const c2v_row_slots *slots, const c2v_grads *grads)
+{
+    if (!slots || !grads) {
+        set_error("%s: NULL pointer argument", fn);
+        return false;
+    }
+    const uintptr_t sa = reinterpret_cast<uintptr_t>(slots->terminal) | reinterpret_cast<uintptr_t>(slots->path);
+    uintptr_t va = 0;
+    if (slots->terminal) va |= reinterpret_cast<uintptr_t>(grads->terminal_embedding);
+    if (slots->path) va |= reinterpret_cast<uintptr_t>(grads->path_embedding);
+    if ((sa & 3) || (va & 15)) {
+        set_error("%s: misaligned pointer (slot maps: 4 bytes, compact gradient buffers: 16)", fn);
+        return false;
+    }
+    return true;
+}
+
+int c2v_encode_backward_sparse(const c2v_dims *d, const c2v_params *p, const int64_t *starts, const int64_t *paths,
+                               const int64_t *ends, int32_t B, int32_t L, const c2v_dropout *drop,
+                               const float *code_vector, const float *attention, const float *x_stash,
+                               const float *d_code_vector, const float *d_attention, const c2v_grads *grads,
+                               const c2v_row_slots *slots, void *workspace, size_t workspace_bytes, int32_t phase,
+                               void *stream)
+{
+    if (phase < 0 || phase > 2) { set_error("c2v_encode_backward_sparse: phase %d", phase); return C2V_EINVAL; }
+    if (!dims_ok(d)) return C2V_EINVAL;
+    if (!p || !starts || !paths || !ends || !code_vector || !attention || !d_code_vector || !grads ||
+        !workspace || B < 1 || L < 1) {
+        set_error("c2v_encode_backward_sparse: bad argument");
+        return C2V_EINVAL;
+    }
+    if (!row_slots_ok("c2v_encode_backward_sparse", slots, grads)) return C2V_EINVAL;
+    return encode_backward_impl(d, p, starts, paths, ends, nullptr, B, (long long)B * L, L, drop, code_vector, attention,
+                                x_stash, d_code_vector, d_attention, grads, workspace, workspace_bytes, phase, stream, slots);
+}
+
+int c2v_encode_backward_packed_sparse(const c2v_dims *d, const c2v_params *p, const int64_t *starts,
+                                      const int64_t *paths, const int64_t *ends, const int64_t *offsets, int32_t B,
+                                      int64_t N, int32_t L, const c2v_dropout *drop, const float *code_vector,
+                                      const float *attention, const float *x_stash, const float *d_code_vector,
+                                      const float *d_attention, const c2v_grads *grads, const c2v_row_slots *slots,
+                                      void *workspace, size_t workspace_bytes, int32_t phase, void *stream)
+{
+    if (phase < 0 || phase > 2) { set_error("c2v_encode_backward_packed_sparse: phase %d", phase); return C2V_EINVAL; }
+    if (!dims_ok(d)) return C2V_EINVAL;
+    if (!p || !starts || !paths || !ends || !offsets || !code_vector || !attention || !d_code_vector || !grads ||
+        !workspace) {
+        set_error("c2v_encode_backward_packed_sparse: NULL pointer argument");
+        return C2V_EINVAL;
+    }
+    if (!packed_shape_ok("c2v_encode_backward_packed_sparse", B, N, L)) return C2V_EINVAL;
+    if (!row_slots_ok("c2v_encode_backward_packed_sparse", slots, grads)) return C2V_EINVAL;
+    return encode_backward_impl(d, p, starts, paths, ends, offsets, B, N, L, drop, code_vector, attention, x_stash,
+                                d_code_vector, d_attention, grads, workspace, workspace_bytes, phase, stream, slots);
 }
 
 }  // extern "C"

@@ -30,7 +30,8 @@ bool backward_dw_tc_ok(const EncodeArgs &a);
 bool backward_dc_tc_ok(const EncodeArgs &a);
 size_t backward_dc_tc_workspace_bytes();
 int launch_backward_dc_tc(const EncodeArgs &a, const float *W, const float *dx, const unsigned *dx_absmax, void *ws,
-                          float *g_emb_t, float *g_emb_p, cudaStream_t st, int sv_mask, bool build_image);
+                          float *g_emb_t, float *g_emb_p, cudaStream_t st, int sv_mask, bool build_image,
+                          const c2v_row_slots *slots);
 int launch_backward_dw_tc(const EncodeArgs &a, const float *dx, const unsigned *dx_absmax, float *dW, cudaStream_t st);
 
 struct BackwardArgs {
@@ -94,9 +95,10 @@ __device__ __forceinline__ void load_wrow_chunk(const float *__restrict__ W, int
     }
 }
 
-template <bool VEC, bool PACKED = false>
+// SPARSE: compact embedding gradients as in backward_dc_tc_kernel (slot maps in sl, a parameter behind the others)
+template <bool VEC, bool PACKED = false, bool SPARSE = false>
 __global__ void __launch_bounds__(THREADS)
-backward_rows_kernel(const EncodeArgs a, const BackwardArgs b, const int Hs)
+backward_rows_kernel(const EncodeArgs a, const BackwardArgs b, const int Hs, const c2v_row_slots sl)
 {
     extern __shared__ __align__(16) unsigned char smem[];
     const FfmaSmem lay = ffma_smem_layout(Hs);
@@ -207,6 +209,14 @@ backward_rows_kernel(const EncodeArgs a, const BackwardArgs b, const int Hs)
             for (int c = H + lane; c < Hs; c += 32) xr[c] = 0.0f;
         }
         __syncthreads();
+
+        if constexpr (SPARSE) {              // compact gradients: scatter into the rows' slots (tables with a slot map)
+            for (int i = tid; i < 3 * TM; i += THREADS) {
+                const int *slot = i / TM == 1 ? sl.path : sl.terminal;
+                if (slot) sidx[i] = slot[sidx[i]];
+            }
+            __syncthreads();
+        }
 
         // ---- dC = dX . W  (K = H), 128 columns of D at a time, scattered into the embedding grads
         const int n_cb = b.skip_dc ? 0 : (D + NB - 1) / NB, n_hc = (H + KC - 1) / KC;
@@ -545,7 +555,8 @@ size_t encode_backward_workspace_bytes(const c2v_dims *d, int B, int L)
 
 int launch_encode_backward(const c2v_dims *d, const c2v_params *p, const EncodeArgs &a_in, int B,
                            const float *cv, const float *attention, const float *d_cv, const float *d_att,
-                           const c2v_grads *g, void *ws, size_t ws_bytes, cudaStream_t st, const float *x_stash, int phase)
+                           const c2v_grads *g, void *ws, size_t ws_bytes, cudaStream_t st, const float *x_stash, int phase,
+                           const c2v_row_slots *slots)
 {
     // phase 0: the whole backward.  Phases 1 / 2 split it where the path table's gradient is complete (all state between
     // the two calls lives in the workspace): 1 = per-row work + dC of the path sub-vector + dW, 2 = dC of start / end.
@@ -580,7 +591,7 @@ int launch_encode_backward(const c2v_dims *d, const c2v_params *p, const EncodeA
             if (!split_ok) return C2V_OK;                       // phase 1 already did everything
             a.n_tiles = (int)((a.N + TM - 1) / TM);
             return launch_backward_dc_tc(a, p->input_linear, dx, dx_absmax, dc_ws, g->terminal_embedding, g->path_embedding, st,
-                                         5, false);
+                                         5, false, slots);
         }
         if (phase == 1 && !split_ok) phase = 0;
     }
@@ -635,11 +646,11 @@ int launch_encode_backward(const c2v_dims *d, const c2v_params *p, const EncodeA
         else (packed ? backward_rows_lite_kernel<2, true> : backward_rows_lite_kernel<2>)<<<sms * 8, 256, 0, st>>>(a, b);
         C2V_LAUNCH_OK("backward_rows_lite_kernel");
         if (phase == 1) {                                       // path sub-vector + dW; start / end follow in phase 2
-            rc = launch_backward_dc_tc(a, p->input_linear, dx, dx_absmax, dc_ws, g->terminal_embedding, g->path_embedding, st, 2, true);
+            rc = launch_backward_dc_tc(a, p->input_linear, dx, dx_absmax, dc_ws, g->terminal_embedding, g->path_embedding, st, 2, true, slots);
             if (rc != C2V_OK) return rc;
             return launch_backward_dw_tc(a, dx, dx_absmax, g->input_linear, st);
         }
-        rc = launch_backward_dc_tc(a, p->input_linear, dx, dx_absmax, dc_ws, g->terminal_embedding, g->path_embedding, st, 7, true);
+        rc = launch_backward_dc_tc(a, p->input_linear, dx, dx_absmax, dc_ws, g->terminal_embedding, g->path_embedding, st, 7, true, slots);
         if (rc != C2V_OK) return rc;
         const char *dw_env2 = getenv("C2V_BACKWARD_DW");
         if (backward_dw_tc_ok(a) && !(dw_env2 && !strcmp(dw_env2, "ffma")))
@@ -648,17 +659,22 @@ int launch_encode_backward(const c2v_dims *d, const c2v_params *p, const EncodeA
         goto dw_ffma;
     }
     {
-    auto kern = packed ? (vec ? backward_rows_kernel<true, true> : backward_rows_kernel<false, true>)
-                       : (vec ? backward_rows_kernel<true> : backward_rows_kernel<false>);
+    const bool sparse = !dc_tc && slots && (slots->terminal || slots->path);     // (with dc_tc K3c scatters)
+    auto kern = sparse ? (packed ? (vec ? backward_rows_kernel<true, true, true> : backward_rows_kernel<false, true, true>)
+                                 : (vec ? backward_rows_kernel<true, false, true> : backward_rows_kernel<false, false, true>))
+                       : (packed ? (vec ? backward_rows_kernel<true, true> : backward_rows_kernel<false, true>)
+                                 : (vec ? backward_rows_kernel<true> : backward_rows_kernel<false>));
+    c2v_row_slots sl = {nullptr, nullptr};
+    if (sparse) sl = *slots;
     C2V_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     int occ = 1;
     C2V_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, THREADS, smem));
     if (occ < 1) occ = 1;
     int grid = a.n_tiles < sms * occ ? a.n_tiles : sms * occ;
-    kern<<<grid, THREADS, smem, st>>>(a, b, Hs);
+    kern<<<grid, THREADS, smem, st>>>(a, b, Hs, sl);
     C2V_LAUNCH_OK("backward_rows_kernel");
     if (dc_tc) {
-        rc = launch_backward_dc_tc(a, p->input_linear, dx, dx_absmax, dc_ws, g->terminal_embedding, g->path_embedding, st, 7, true);
+        rc = launch_backward_dc_tc(a, p->input_linear, dx, dx_absmax, dc_ws, g->terminal_embedding, g->path_embedding, st, 7, true, slots);
         if (rc != C2V_OK) return rc;
     }
 

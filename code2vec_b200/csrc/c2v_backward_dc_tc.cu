@@ -87,10 +87,15 @@ split_wt_kernel(const float *__restrict__ W, int H, int E, int n_hb, int n_db, c
     }
 }
 
+// SPARSE: a table whose slot map in sl is not NULL gets its gradient in compact form, row r of the table adding into row
+// sl.<table>[r] of the [U, E] buffer passed as its gradient (sparse embedding gradients, c2v_sparse_rows).  The slot maps
+// are a parameter of their own behind all the others, so that the dense instantiation keeps its parameter layout.
+template <bool SPARSE = false>
 __global__ void __launch_bounds__(dct::THREADS, 1)
 backward_dc_tc_kernel(const EncodeArgs a, const float *__restrict__ dx, const unsigned *__restrict__ dx_absmax,
                       const uint8_t *__restrict__ wt_img, const float *__restrict__ wt_hdr,
-                      float *__restrict__ g_emb_t, float *__restrict__ g_emb_p, const int sv_mask, const int n_hb)
+                      float *__restrict__ g_emb_t, float *__restrict__ g_emb_p, const int sv_mask, const int n_hb,
+                      const c2v_row_slots sl)
 {
     const int db = (int)blockIdx.y;                     // this CTA's 128-wide window of d inside every sub-vector
     // sv_mask: which sub-vectors (bit 0 start, 1 path, 2 end) this launch handles.  The training step runs the path
@@ -255,6 +260,10 @@ backward_dc_tc_kernel(const EncodeArgs a, const float *__restrict__ dx, const un
                 for (int h = 0; h < 2; ++h) {
                     if (!in_range[h]) continue;
                     float *dst = tab + (size_t)idx[h][sv] * a.Et + db * dct::E;
+                    if constexpr (SPARSE) {           // compact gradient: the row's slot (tables without a slot map: the row)
+                        const int *slot = sv == 1 ? sl.path : sl.terminal;
+                        if (slot) dst = tab + (size_t)slot[idx[h][sv]] * a.Et + db * dct::E;
+                    }
 #pragma unroll
                     for (int j = 0; j < 16; ++j) {
                         const int c = 8 * j + 2 * m4;
@@ -276,7 +285,8 @@ size_t backward_dc_tc_workspace_bytes() { return 1024 + 4 * dct::IMG_BYTES; }   
 
 // ws: [0, 1024) header {1/scale, scale} | W^T images [db][hb]
 int launch_backward_dc_tc(const EncodeArgs &a_in, const float *W, const float *dx, const unsigned *dx_absmax, void *ws,
-                          float *g_emb_t, float *g_emb_p, cudaStream_t st, int sv_mask, bool build_image)
+                          float *g_emb_t, float *g_emb_p, cudaStream_t st, int sv_mask, bool build_image,
+                          const c2v_row_slots *slots)
 {
     EncodeArgs a = a_in;
     a.n_tiles = (int)((a.N + dct::ROWS - 1) / dct::ROWS);
@@ -295,12 +305,16 @@ int launch_backward_dc_tc(const EncodeArgs &a_in, const float *W, const float *d
     int dev = 0, sms = 0;
     C2V_CUDA_OK(cudaGetDevice(&dev));
     C2V_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    C2V_CUDA_OK(cudaFuncSetAttribute(backward_dc_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dct::SMEM_BYTES));
+    const bool sparse = slots && (slots->terminal || slots->path);
+    auto kern = sparse ? backward_dc_tc_kernel<true> : backward_dc_tc_kernel<false>;
+    C2V_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, dct::SMEM_BYTES));
     int grid = sms / n_db;                                 // one CTA per SM over the d windows
     if (grid > a.n_tiles) grid = a.n_tiles;
     if (grid < 1) grid = 1;
-    backward_dc_tc_kernel<<<dim3(grid, n_db), dct::THREADS, dct::SMEM_BYTES, st>>>(a, dx, dx_absmax, img, hdr, g_emb_t, g_emb_p,
-                                                                                sv_mask & 7, n_hb);
+    c2v_row_slots sl = {nullptr, nullptr};
+    if (sparse) sl = *slots;
+    kern<<<dim3(grid, n_db), dct::THREADS, dct::SMEM_BYTES, st>>>(a, dx, dx_absmax, img, hdr, g_emb_t, g_emb_p, sv_mask & 7,
+                                                                  n_hb, sl);
     C2V_LAUNCH_OK("backward_dc_tc_kernel");
     return C2V_OK;
 }

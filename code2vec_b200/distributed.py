@@ -424,3 +424,56 @@ def broadcast_parameters(model, src=0):
             # a write through .data does not bump Tensor._version, which the model's cached weight images
             # (functional.PrepCache) are keyed on: bump it so the next forward rebuilds them
             torch.autograd.graph.increment_version(t)
+
+
+class FusedSparseAdam(torch.optim.SparseAdam):
+    """torch.optim.SparseAdam whose step is one kernel per parameter (`c2v_sparse_adam_step`): for the rows of the
+    coalesced sparse gradient it reads g, p, exp_avg and exp_avg_sq once and writes p, exp_avg and exp_avg_sq, with torch's
+    operation order and rounding, so parameters and state stay bit-identical to torch.optim.SparseAdam's.  Only step() is
+    overridden: parameter groups, hyper-parameter checks and state_dict are torch's and interchange with
+    torch.optim.SparseAdam in both directions.  For the embedding tables of a Code2Vec whose `.sparse` is set (see
+    INTEGRATION.md, "Sparse embedding gradients").  Lazy Adam: rows a batch does not touch keep their moments and do not
+    move, unlike the dense torch.optim.Adam of the reference.  Single process only: a data-parallel reduction of sparse
+    gradients is not implemented, and without one the replicas would drift apart."""
+
+    @torch.no_grad()
+    def step(self, closure=None):
+        from . import functional as CF
+        loss = None
+        if closure is not None:
+            with torch.enable_grad():
+                loss = closure()
+        if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+            raise NotImplementedError("FusedSparseAdam: sparse gradients are not reduced across processes "
+                                      f"(world size {dist.get_world_size()}); use one process or dense gradients")
+        for group in self.param_groups:
+            beta1, beta2 = group["betas"]
+            maximize = group.get("maximize", False)
+            lr = group["lr"]
+            lr = float(lr.item()) if isinstance(lr, torch.Tensor) else float(lr)
+            for p in group["params"]:
+                if p.grad is None:
+                    continue
+                grad = p.grad
+                if not grad.is_sparse:
+                    raise RuntimeError("SparseAdam does not support dense gradients, please consider Adam instead")
+                state = self.state[p]
+                if len(state) == 0:
+                    state["step"] = 0
+                    state["exp_avg"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+                    state["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+                state["step"] += 1
+                if maximize:
+                    grad = -grad
+                if not grad.is_coalesced():
+                    grad = grad.coalesce()
+                if grad.sparse_dim() != 1:
+                    raise NotImplementedError("FusedSparseAdam: gradients must be sparse in the first dimension only "
+                                              "(row-sparse, as nn.Embedding(sparse=True) produces)")
+                values = grad._values()
+                if values.numel() == 0:                          # torch skips an empty gradient (the step still counts)
+                    continue
+                CF.sparse_adam_step(p, state["exp_avg"], state["exp_avg_sq"], values, grad._indices()[0], lr, beta1,
+                                    beta2, group["eps"], state["step"])
+                torch.autograd.graph.increment_version(p)        # raw-pointer writes: bump the version counter
+        return loss

@@ -6,7 +6,7 @@ import os
 import torch
 
 from . import _lib
-from ._lib import Dims, Dropout, Grads, Params
+from ._lib import Dims, Dropout, Grads, Params, RowSlots
 
 
 # C2V_POISON=1: every buffer handed to the library uninitialised (workspaces, outputs, stashes) is filled with 0xFF bytes
@@ -554,10 +554,17 @@ def label_backward(dims, params, cv, d_out, need_cv=True, need_w=True, need_b=Tr
     return d_cv, (d_w if need_w else None), d_b
 
 
+def _row_slots(slots):
+    """(terminal slot map or None, path slot map or None) -> c2v_row_slots (the tensors stay with the caller)"""
+    return RowSlots(_ptr(slots[0]), _ptr(slots[1]))
+
+
 def encode_backward(dims, params, starts, paths, ends, cv, att, d_cv, d_att, shapes, drop_p=0.0, training=False,
-                    seed=0, grads_out=None, x_stash=None, between_phases=None):
+                    seed=0, grads_out=None, x_stash=None, between_phases=None, slots=None):
     """Gradients of the six encode parameters; returns dict name -> tensor.  x_stash: what encode_forward(stash=True)
-    returned for this batch (skips the re-gather + recompute GEMM)."""
+    returned for this batch (skips the re-gather + recompute GEMM).  slots: (terminal, path) slot maps of sparse_rows()
+    for this batch, None for a dense table; grads_out then holds the zero-filled compact [U, E] buffer of every table
+    with a slot map (c2v_encode_backward_sparse)."""
     lib = _lib.load()
     B, L = starts.shape
     dev = starts.device
@@ -575,10 +582,13 @@ def encode_backward(dims, params, starts, paths, ends, cv, att, d_cv, d_att, sha
         # between_phases: called after the path sub-vector's gradients are complete (c2v_encode_backward_phased), e.g. to
         # start their data-parallel reduction on another stream while start / end / dW are still being computed
         for phase in ((1, 2) if between_phases is not None else (0,)):
-            rc = lib.c2v_encode_backward_phased(ctypes.byref(dims), ctypes.byref(params), _ptr(starts), _ptr(paths), _ptr(ends),
-                                                B, L, ctypes.byref(drop), _ptr(cv), _ptr(att), _ptr(x_stash),
-                                                _ptr(d_cv), _ptr(d_att), ctypes.byref(grads),
-                                                _ptr(ws), nbytes, phase, _stream(dev))
+            args = (ctypes.byref(dims), ctypes.byref(params), _ptr(starts), _ptr(paths), _ptr(ends), B, L, ctypes.byref(drop),
+                    _ptr(cv), _ptr(att), _ptr(x_stash), _ptr(d_cv), _ptr(d_att), ctypes.byref(grads))
+            if slots is None:
+                rc = lib.c2v_encode_backward_phased(*args, _ptr(ws), nbytes, phase, _stream(dev))
+            else:
+                rc = lib.c2v_encode_backward_sparse(*args, ctypes.byref(_row_slots(slots)), _ptr(ws), nbytes, phase,
+                                                    _stream(dev))
             _lib.check(rc, "c2v_encode_backward")
             if phase == 1:
                 between_phases()
@@ -586,7 +596,7 @@ def encode_backward(dims, params, starts, paths, ends, cv, att, d_cv, d_att, sha
 
 
 def encode_backward_packed(dims, params, bags, cv, att, d_cv, d_att, shapes, drop_p=0.0, training=False, seed=0,
-                           grads_out=None, x_stash=None, between_phases=None):
+                           grads_out=None, x_stash=None, between_phases=None, slots=None):
     """encode_backward for a PackedBags batch: att / d_att [N], x_stash [N, H] from encode_forward_packed(stash=True)."""
     lib = _lib.load()
     B, N, L = bags.B, bags.N, bags.L
@@ -602,11 +612,65 @@ def encode_backward_packed(dims, params, bags, cv, att, d_cv, d_att, shapes, dro
         d_cv = _f32c(d_cv, "d_code_vector")
         d_att = _f32c(d_att, "d_attention") if d_att is not None else None
         for phase in ((1, 2) if between_phases is not None else (0,)):
-            rc = lib.c2v_encode_backward_packed(ctypes.byref(dims), ctypes.byref(params), _ptr(bags.starts), _ptr(bags.paths),
-                                                _ptr(bags.ends), _ptr(bags.offsets), B, N, L, ctypes.byref(drop), _ptr(cv),
-                                                _ptr(att), _ptr(x_stash), _ptr(d_cv), _ptr(d_att), ctypes.byref(grads),
-                                                _ptr(ws), nbytes, phase, _stream(dev))
+            args = (ctypes.byref(dims), ctypes.byref(params), _ptr(bags.starts), _ptr(bags.paths), _ptr(bags.ends),
+                    _ptr(bags.offsets), B, N, L, ctypes.byref(drop), _ptr(cv), _ptr(att), _ptr(x_stash), _ptr(d_cv),
+                    _ptr(d_att), ctypes.byref(grads))
+            if slots is None:
+                rc = lib.c2v_encode_backward_packed(*args, _ptr(ws), nbytes, phase, _stream(dev))
+            else:
+                rc = lib.c2v_encode_backward_packed_sparse(*args, ctypes.byref(_row_slots(slots)), _ptr(ws), nbytes, phase,
+                                                           _stream(dev))
             _lib.check(rc, "c2v_encode_backward_packed")
             if phase == 1:
                 between_phases()
     return g
+
+
+def sparse_rows(indices, vocab):
+    """Row map of one embedding table for one batch (c2v_sparse_rows): indices is a list of one or two int64 CUDA tensors
+    (any shape; e.g. [starts, ends] for the terminal table) -> (slot int32 [vocab], rows int64 [min(vocab, n)] whose
+    first U entries are the distinct rows the batch indexes, ascending, count int64 [1] = U), all on the device and
+    enqueued on the current stream.  Out-of-range indices count as row 0, as the encode reads them."""
+    lib = _lib.load()
+    idx = [_idx(t, "indices").reshape(-1) for t in indices]
+    if not 1 <= len(idx) <= 2:
+        raise ValueError("sparse_rows takes one or two index tensors")
+    _need_cuda(*idx)
+    a = idx[0]
+    b = idx[1] if len(idx) == 2 else None
+    n_a, n_b = a.numel(), (b.numel() if b is not None else 0)
+    vocab = int(vocab)
+    dev = a.device
+    nbytes = lib.c2v_sparse_rows_workspace_bytes(vocab)
+    if nbytes == 0:
+        raise ValueError(f"sparse_rows: vocab = {vocab} outside [1, 2^31)")
+    with torch.cuda.device(dev):
+        slot = _empty((vocab,), torch.int32, dev)
+        rows = _empty((min(vocab, n_a + n_b),), torch.int64, dev)
+        count = _empty((1,), torch.int64, dev)
+        ws = _empty((nbytes,), torch.uint8, dev)
+        rc = lib.c2v_sparse_rows(_ptr(a) if n_a else None, n_a, _ptr(b) if n_b else None, n_b, vocab, _ptr(slot),
+                                 _ptr(rows) if rows.numel() else None, _ptr(count), _ptr(ws), nbytes, _stream(dev))
+        _lib.check(rc, "c2v_sparse_rows")
+    return slot, rows, count
+
+
+def sparse_adam_step(param, exp_avg, exp_avg_sq, values, rows, lr, beta1, beta2, eps, step):
+    """torch.optim.SparseAdam's update of param / exp_avg / exp_avg_sq [n, E] (contiguous fp32 CUDA) at the distinct rows
+    `rows` (int64 [U]) from the gradient values [U, E] of a coalesced sparse gradient (c2v_sparse_adam_step); step is
+    the step count after this step."""
+    lib = _lib.load()
+    _need_cuda(param, exp_avg, exp_avg_sq, values, rows)
+    for t, name in ((param, "param"), (exp_avg, "exp_avg"), (exp_avg_sq, "exp_avg_sq")):
+        if t.dtype != torch.float32 or not t.is_contiguous() or t.shape != param.shape:
+            raise TypeError(f"{name} must be contiguous fp32 of the parameter's shape")
+    n, E = param.shape[0], param[0].numel()
+    values = _f32c(values, "values").reshape(-1, E)
+    rows = _idx(rows, "rows").reshape(-1)
+    if values.shape[0] != rows.numel():
+        raise ValueError(f"sparse_adam_step: {values.shape[0]} value rows for {rows.numel()} indices")
+    dev = param.device
+    with torch.cuda.device(dev):
+        rc = lib.c2v_sparse_adam_step(_ptr(param), _ptr(exp_avg), _ptr(exp_avg_sq), _ptr(values), _ptr(rows), rows.numel(),
+                                      n, E, float(lr), float(beta1), float(beta2), float(eps), int(step), _stream(dev))
+        _lib.check(rc, "c2v_sparse_adam_step")

@@ -34,7 +34,8 @@ class _EncodeFn(torch.autograd.Function):
     """gathers -> concat -> input_linear -> LayerNorm -> tanh -> dropout -> attention -> code vector."""
 
     @staticmethod
-    def forward(ctx, emb_t, emb_p, W, ln_g, ln_b, attn, starts, paths, ends, dims, drop_p, training, seed, algo, cache):
+    def forward(ctx, emb_t, emb_p, W, ln_g, ln_b, attn, starts, paths, ends, dims, drop_p, training, seed, algo, cache,
+                sparse=(False, False)):
         params = CF.make_params(emb_t, emb_p, W, ln_g, ln_b, attn)
         # when a gradient will be asked for, keep x = c . W^T (105 MB per 1024 x 200 batch at encode_size 128) so that
         # the backward neither re-gathers the embedding rows nor redoes the input_linear GEMM
@@ -50,6 +51,24 @@ class _EncodeFn(torch.autograd.Function):
                                     cache=cache, weight=W, stash=stash)
         cv, att = res[0], res[1]
         ctx.x_stash = res[2] if stash else None
+        # sparse embedding gradients (nn.Embedding.sparse): the row map of each such table is built here, where the indices
+        # are at hand; the backward needs U on the host only to shape the final sparse tensor, so U travels to pinned
+        # memory behind an event and the backward's one host wait is on that event
+        ctx.row_maps = None
+        want = (sparse[0] and ctx.needs_input_grad[0], sparse[1] and ctx.needs_input_grad[1])
+        if any(want):
+            s_, p_, e_ = (ctx.bags.starts, ctx.bags.paths, ctx.bags.ends) if ctx.bags is not None else (starts, paths, ends)
+            with torch.cuda.device(s_.device):       # row maps, copies and event all on the stream of the batch's device
+                maps = (CF.sparse_rows([s_, e_], dims.terminal_count) if want[0] else None,
+                        CF.sparse_rows([p_], dims.path_count) if want[1] else None)
+                counts = torch.zeros(2, dtype=torch.int64, pin_memory=True)
+                for i, m in enumerate(maps):
+                    if m is not None:
+                        counts[i:i + 1].copy_(m[2], non_blocking=True)
+                ready = torch.cuda.Event()
+                ready.record(torch.cuda.current_stream(s_.device))
+            # kept with the graph (freed with it), so that a backward with retain_graph=True can run again
+            ctx.row_maps = (maps, counts, ready)
         ctx.save_for_backward(emb_t, emb_p, W, ln_g, ln_b, attn, starts, paths, ends, cv, att)
         ctx.cfg = (dims, drop_p, training, seed)
         ctx.cache = cache
@@ -70,7 +89,13 @@ class _EncodeFn(torch.autograd.Function):
         # optimizers): the embedding-table and input_linear gradients -- 99.9 % of the bytes -- are scatter-added straight into
         # the existing dense .grad buffers instead of into fresh zero-filled tensors that autograd would then add to .grad
         # (at cfg2: a 360 MB fill plus a 1.1 GB read-modify-write per step).  Autograd gets None for those three inputs.
-        big = (("terminal_embedding", emb_t), ("path_embedding", emb_p), ("input_linear", W))
+        # sparse tables: the backward accumulates their rows into compact [U_max, E] buffers (row r -> row slot[r])
+        maps = ctx.row_maps[0] if ctx.row_maps is not None else (None, None)
+        compact = {k: torch.zeros((m[1].numel(), t.shape[1]), dtype=torch.float32, device=cv.device)
+                   for k, m, t in (("terminal_embedding", maps[0], emb_t), ("path_embedding", maps[1], emb_p))
+                   if m is not None}
+        big = tuple((k, t) for k, t in (("terminal_embedding", emb_t), ("path_embedding", emb_p), ("input_linear", W))
+                    if k not in compact)
         fuse = bool(getattr(ctx.cache, "fuse_grad_accumulation", False)) and all(
             t.grad is not None and t.grad.dtype == torch.float32 and t.grad.is_contiguous() and t.grad.shape == t.shape
             and t.grad.device == t.device for _, t in big)
@@ -79,19 +104,33 @@ class _EncodeFn(torch.autograd.Function):
             grads_out = {k: t.grad for k, t in big}
             for k in ("ln_weight", "ln_bias", "attention"):
                 grads_out[k] = torch.empty(shapes[k], dtype=torch.float32, device=cv.device)   # overwritten by the kernels
-        hook = getattr(ctx.cache, "on_path_grads_ready", None) if fuse else None
+        elif compact:                                # (no dense buffer for a sparse table: its rows go to `compact`)
+            grads_out = {k: torch.zeros(s, dtype=torch.float32, device=cv.device) for k, s in shapes.items()
+                         if k not in compact}
+        if compact:
+            grads_out.update(compact)
+        hook = getattr(ctx.cache, "on_path_grads_ready", None) if fuse and maps[1] is None else None
+        slots = tuple(m[0] if m is not None else None for m in maps) if compact else None
         if ctx.bags is not None:
             g = CF.encode_backward_packed(dims, params, ctx.bags, cv, att, d_cv, d_att, shapes, drop_p, training, seed,
-                                          grads_out=grads_out, x_stash=ctx.x_stash, between_phases=hook)
+                                          grads_out=grads_out, x_stash=ctx.x_stash, between_phases=hook, slots=slots)
         else:
             g = CF.encode_backward(dims, params, starts, paths, ends, cv, att, d_cv, d_att, shapes, drop_p, training, seed,
-                                   grads_out=grads_out, x_stash=ctx.x_stash, between_phases=hook)
+                                   grads_out=grads_out, x_stash=ctx.x_stash, between_phases=hook, slots=slots)
         ctx.x_stash = None
-        if fuse:
-            return (None, None, None, g["ln_weight"], g["ln_bias"], g["attention"], None, None, None, None, None, None,
-                    None, None, None)
-        return (g["terminal_embedding"], g["path_embedding"], g["input_linear"], g["ln_weight"], g["ln_bias"],
-                g["attention"], None, None, None, None, None, None, None, None, None)
+        out = {k: (None if fuse else g[k]) for k in ("terminal_embedding", "path_embedding", "input_linear")}
+        if compact:
+            _, counts, ready = ctx.row_maps
+            ready.synchronize()                      # U of each sparse table (the row maps were built in the forward)
+            for i, (k, t) in enumerate((("terminal_embedding", emb_t), ("path_embedding", emb_p))):
+                if k in compact:
+                    U = int(counts[i])
+                    rows = maps[i][1][:U].view(1, U)
+                    out[k] = torch.sparse_coo_tensor(rows, compact[k][:U], t.shape, is_coalesced=True, check_invariants=False)
+                    if ctx.cache is not None:            # what Code2Vec's post-accumulate hook recognises (is_coalesced)
+                        ctx.cache.sparse_indices[k] = (rows.data_ptr(), U)
+        return (out["terminal_embedding"], out["path_embedding"], out["input_linear"], g["ln_weight"], g["ln_bias"],
+                g["attention"], None, None, None, None, None, None, None, None, None, None)
 
 
 class _LabelFn(torch.autograd.Function):
@@ -221,6 +260,9 @@ class Code2Vec(nn.Module):
         # optimizer starts that table's data-parallel reduction there (ShardedFlatAdam.early_step)
         self.on_path_grads_ready = None
         self._lab_cache = CF.PrepCache()
+        # sparse embedding gradients (opt-in: terminal_embedding.sparse / path_embedding.sparse, as on nn.Embedding)
+        self._enc_cache.sparse_indices = {}
+        self._sparse_hooks = None
 
     # -- helpers ---------------------------------------------------------------------------
     def _dims(self):
@@ -249,11 +291,34 @@ class Code2Vec(nn.Module):
         training = self.training and self.input_dropout is not None
         drop_p = float(self.option.dropout_prob) if training else 0.0
         seed = self._next_seed() if training else 0
+        sparse = (bool(self.terminal_embedding.sparse), bool(self.path_embedding.sparse))
+        if any(sparse):
+            self._watch_sparse_grads()
         code_vector, attention = _EncodeFn.apply(
             self.terminal_embedding.weight, self.path_embedding.weight, self.input_linear.weight,
             self.input_layer_norm.weight, self.input_layer_norm.bias, self.attention_parameter,
-            starts, paths, ends, dims, drop_p, training, seed, self.algo, self._enc_cache)
+            starts, paths, ends, dims, drop_p, training, seed, self.algo, self._enc_cache, sparse)
         return code_vector, attention, dims
+
+    def _watch_sparse_grads(self):
+        """Sparse embedding gradients leave the backward coalesced, but torch's AccumulateGrad drops that flag when it
+        makes the tensor the parameter's .grad.  A post-accumulate hook on each table sets it back when .grad's indices are
+        the very tensor the backward produced (a first backward into an empty .grad); after accumulation over several
+        backwards the flag stays whatever torch made it.  Registered once, on the first forward with a sparse table."""
+        if self._sparse_hooks:
+            return
+        cache = self._enc_cache
+
+        def mark(key):
+            def hook(p):
+                g, made = p.grad, cache.sparse_indices.pop(key, None)
+                if g is not None and g.is_sparse and made is not None and not g.is_coalesced():
+                    ind = g._indices()
+                    if (ind.data_ptr(), ind.shape[1]) == made:
+                        g._coalesced_(True)
+            return hook
+        self._sparse_hooks = [self.terminal_embedding.weight.register_post_accumulate_grad_hook(mark("terminal_embedding")),
+                              self.path_embedding.weight.register_post_accumulate_grad_hook(mark("path_embedding"))]
 
     def _encode_eval(self, starts, paths, ends):
         """the encode of predict() / predict_topk(), without autograd or dropout -> (code_vector, attention, dims)"""

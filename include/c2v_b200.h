@@ -370,6 +370,49 @@ int c2v_encode_backward_packed(const c2v_dims *d, const c2v_params *p, const int
                                const float *x_stash, const float *d_code_vector, const float *d_attention,
                                const c2v_grads *grads, void *workspace, size_t workspace_bytes, int32_t phase, void *stream);
 
+/* ---- sparse embedding gradients (nn.Embedding(sparse=True) + torch.optim.SparseAdam) ----------------------------
+ * Row map of one embedding table for one batch: the sorted set of rows the batch indexes, and where each sits in it.
+ * idx_a [n_a] and idx_b [n_b] (int64, device; either may be NULL when its length is 0) are the batch's indices into a
+ * table of `vocab` rows; out-of-range indices count as row 0, as the encode reads them.  Writes
+ *   rows  int64 [U], ascending: the distinct rows (room for min(vocab, n_a + n_b) entries; NULL if n_a + n_b == 0)
+ *   slot  int32 [vocab]: slot[rows[i]] = i, -1 for rows the batch does not touch
+ *   count int64 [1] (device): U
+ * Mark, scan and compact over the vocabulary: O(vocab + n_a + n_b), no sort.  vocab < 2^31 (slot is int32). */
+size_t c2v_sparse_rows_workspace_bytes(int64_t vocab);
+int c2v_sparse_rows(const int64_t *idx_a, int64_t n_a, const int64_t *idx_b, int64_t n_b, int64_t vocab, int32_t *slot,
+                    int64_t *rows, int64_t *count, void *workspace, size_t workspace_bytes, void *stream);
+
+/* Slot maps (c2v_sparse_rows) of the tables whose gradient the encode backward writes in compact form; NULL = dense. */
+typedef struct c2v_row_slots {
+    const int32_t *terminal;
+    const int32_t *path;
+} c2v_row_slots;
+/* c2v_encode_backward_phased / c2v_encode_backward_packed with compact embedding gradients: for a table whose slot map
+ * in `slots` is not NULL, grads->terminal_embedding / path_embedding is a [U, E] values buffer (zero-filled by the
+ * caller, 16-byte aligned) and row r's gradient is accumulated into its row slot[r] instead of row r of the table.  The
+ * map must be the one c2v_sparse_rows built from this batch's indices. */
+int c2v_encode_backward_sparse(const c2v_dims *d, const c2v_params *p, const int64_t *starts, const int64_t *paths,
+                               const int64_t *ends, int32_t B, int32_t L, const c2v_dropout *drop,
+                               const float *code_vector, const float *attention, const float *x_stash,
+                               const float *d_code_vector, const float *d_attention, const c2v_grads *grads,
+                               const c2v_row_slots *slots, void *workspace, size_t workspace_bytes, int32_t phase,
+                               void *stream);
+int c2v_encode_backward_packed_sparse(const c2v_dims *d, const c2v_params *p, const int64_t *starts,
+                                      const int64_t *paths, const int64_t *ends, const int64_t *offsets, int32_t B,
+                                      int64_t N, int32_t L, const c2v_dropout *drop, const float *code_vector,
+                                      const float *attention, const float *x_stash, const float *d_code_vector,
+                                      const float *d_attention, const c2v_grads *grads, const c2v_row_slots *slots,
+                                      void *workspace, size_t workspace_bytes, int32_t phase, void *stream);
+
+/* torch.optim.SparseAdam's update (torch.optim._functional.sparse_adam, same operation order, no fused multiply-add)
+ * of the U rows `rows` (int64, distinct) of param / exp_avg / exp_avg_sq [n_rows, E] from the coalesced gradient
+ * values [U, E]: lazy Adam, rows outside `rows` keep their parameters and moments.  lr, betas and eps are the
+ * optimizer's double-precision hyper-parameters; step >= 1 is the step count after this step.  Rows outside
+ * [0, n_rows) are skipped. */
+int c2v_sparse_adam_step(float *param, float *exp_avg, float *exp_avg_sq, const float *values, const int64_t *rows,
+                         int64_t U, int64_t n_rows, int32_t E, double lr, double beta1, double beta2, double eps,
+                         int64_t step, void *stream);
+
 /* ---- host-buffer call: what a reference-side caller with CPU tensors uses ----------
  * One whole Code2Vec.forward + torch.max for a batch held in HOST memory (pinned
  * for full speed): copies the int64 indices in, runs encode + label head +
