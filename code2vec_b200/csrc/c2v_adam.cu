@@ -14,6 +14,16 @@
 
 namespace c2v {
 
+// The gradient Adam sees: g * gscale (the 1/world of the data-parallel mean) + wd * p (weight decay), rounded once
+// relative to the result.  fmaf(wd, p, g * gscale) alone would round g * gscale first, and where the two terms nearly
+// cancel that rounding is large next to the result (then m is off by tens of ulp); the second fmaf recovers the product's
+// rounding error exactly.  With wd == 0, or an exact gscale (world 1), both forms give the same value.
+__device__ __forceinline__ float adam_grad(float g, float gscale, float wd, float p) {
+    const float gs = g * gscale;
+    if (wd == 0.0f) return gs;
+    return fmaf(wd, p, gs) + fmaf(g, gscale, -gs);
+}
+
 __global__ void __launch_bounds__(256)
 adam_step_kernel(float4 *__restrict__ p, float4 *__restrict__ g, float4 *__restrict__ m, float4 *__restrict__ v,
                  long long n4, float *__restrict__ pt, float *__restrict__ gt, float *__restrict__ mt, float *__restrict__ vt,
@@ -21,8 +31,7 @@ adam_step_kernel(float4 *__restrict__ p, float4 *__restrict__ g, float4 *__restr
                  float wd, float gscale, int zero_grad)
 {
     auto upd = [&](float &pp, float &gg, float &mm, float &vv) {
-        float gr = gg * gscale;
-        if (wd != 0.0f) gr = fmaf(wd, pp, gr);
+        const float gr = adam_grad(gg, gscale, wd, pp);
         mm = mm + (gr - mm) * one_minus_b1;                 // exp_avg.lerp_(grad, 1 - beta1)
         vv = vv * b2 + one_minus_b2 * gr * gr;              // exp_avg_sq.mul_(beta2).addcmul_(grad, grad, value=1 - beta2)
         const float denom = sqrtf(vv) * inv_sqrt_bc2 + eps;
@@ -79,8 +88,7 @@ adam_step_sharded_kernel(const float *__restrict__ p_local, float *__restrict__ 
                          float wd, float gscale)
 {
     auto upd = [&](float &pp, float gg, float &mm, float &vv) {
-        float gr = gg * gscale;
-        if (wd != 0.0f) gr = fmaf(wd, pp, gr);
+        const float gr = adam_grad(gg, gscale, wd, pp);
         mm = mm + (gr - mm) * one_minus_b1;
         vv = vv * b2 + one_minus_b2 * gr * gr;
         const float denom = sqrtf(vv) * inv_sqrt_bc2 + eps;
@@ -180,8 +188,7 @@ adam_step_bulk_kernel(const float *__restrict__ p_local, const AdamPeers peers, 
         }
     };
     auto upd = [&](float &pp, float gg, float &mm, float &vv) {
-        float gr = gg * gscale;
-        if (wd != 0.0f) gr = fmaf(wd, pp, gr);
+        const float gr = adam_grad(gg, gscale, wd, pp);
         mm = mm + (gr - mm) * one_minus_b1;
         vv = vv * b2 + one_minus_b2 * gr * gr;
         const float denom = sqrtf(vv) * inv_sqrt_bc2 + eps;

@@ -115,6 +115,24 @@ class FlatAdam:
         self.bucket.zero()
 
 
+def sharded_layout(n_early, numel, world, rank):
+    """The flat-buffer layout of ShardedFlatAdam for `numel` parameters of which the first `n_early` form the early
+    region (0: no early region).  -> (regions, slices, state_numel):
+      regions      [(begin, length)] in the flat buffers, each length padded to a multiple of 4 * world
+      slices       [(begin, length, state_offset)] of this rank per region: the owned part of the flat buffers and where
+                   its exp_avg / exp_avg_sq sit in the rank's state buffers
+      state_numel  elements of the rank's exp_avg (and of its exp_avg_sq)"""
+    q = 4 * world
+    pad = lambda n: (n + q - 1) // q * q
+    regions = ([(0, pad(n_early))] if n_early else []) + [(pad(n_early) if n_early else 0, pad(numel - n_early))]
+    slices, o = [], 0
+    for begin, n in regions:
+        sl = n // world
+        slices.append((begin + rank * sl, sl, o))
+        o += sl
+    return regions, slices, o
+
+
 class ShardedFlatAdam:
     """Data-parallel Adam with the optimizer state sharded over the ranks and the gradient reduction fused into the
     optimizer kernel.  Same update rule, dense, as
@@ -155,20 +173,11 @@ class ShardedFlatAdam:
         if dt != torch.float32:
             raise TypeError("parameters must be fp32")
         self.numel = sum(p.numel() for p in self.params)
-        q = 4 * self.world
-        pad = lambda n: (n + q - 1) // q * q
         n_early = sum(p.numel() for p in first)
-        # regions: (begin, length) in the flat buffers; region 0 = the early parameters (absent when there are none)
-        self.regions = ([(0, pad(n_early))] if n_early else []) + \
-            [(pad(n_early) if n_early else 0, pad(self.numel - n_early))]
-        self.padded = sum(n for _, n in self.regions)
+        # regions: (begin, length) in the flat buffers; region 0 = the early parameters (absent when there are none);
         # this rank's slice of every region, and where its optimizer state sits in exp_avg / exp_avg_sq
-        self.slices, o = [], 0
-        for begin, n in self.regions:
-            sl = n // self.world
-            self.slices.append((begin + self.rank * sl, sl, o))
-            o += sl
-        self.state_numel = o
+        self.regions, self.slices, self.state_numel = sharded_layout(n_early, self.numel, self.world, self.rank)
+        self.padded = sum(n for _, n in self.regions)
         self._auto = transport == "auto"
         self.transport, self._hdl = self._allocate(transport, dev)
         self._grad_views = ([], [])

@@ -10,7 +10,8 @@ import torch.multiprocessing as mp
 import torch.nn as nn
 import torch.nn.functional as F
 
-from code2vec_b200.distributed import FlatGradBucket, broadcast_parameters, ddp_step, shard_items, shard_range
+from code2vec_b200.distributed import (FlatGradBucket, broadcast_parameters, ddp_step, shard_items, shard_range,
+                                       sharded_layout)
 
 
 def test_shard_range_partitions_everything():
@@ -97,8 +98,8 @@ def test_bucket_is_one_buffer_and_detects_broken_views():
 # ---- sharded optimizer (reduce-scatter -> Adam on the owned slice -> all-gather) --------------------------------
 def _torch_adam_slice(self, p_slice, g_slice, zero_grad=False, state=None):
     m_, v_ = state if state is not None else (self.exp_avg, self.exp_avg_sq)
-    """CPU stand-in for `c2v_adam_step` (same operation order; the CUDA kernel is checked against torch.optim.Adam on
-    the GPU by tests/test_backward_parity_gpu.py / test_adam_gpu): TEST INFRASTRUCTURE, patched in below."""
+    """CPU stand-in for `c2v_adam_step` (same operation order; the CUDA kernels are checked against an fp64 Adam on the
+    GPU by tests/test_adam_gpu.py): TEST INFRASTRUCTURE, patched in below."""
     b1, b2 = self.betas
     g = g_slice * (1.0 / self.world)
     if self.weight_decay:
@@ -124,6 +125,9 @@ def _sharded_worker(rank, world, port, ret):
         opt = ShardedFlatAdam(model.parameters(), lr=0.01, weight_decay=0.01, early=[model.lin.weight])   # two regions
         assert opt.transport == "nccl" and opt.padded % (4 * world) == 0 and opt.exp_avg.numel() * world == opt.padded
         assert len(opt.regions) == 2 and opt.params[0] is model.lin.weight
+        # lin.weight (40) is region 0, emb.weight + lin.bias (405) region 1, both padded to multiples of 4 * world = 8
+        assert opt.regions == [(0, 40), (40, 408)] and opt.padded == 448
+        assert opt.slices == [(20 * rank, 20, 0), (40 + 204 * rank, 204, 20)] and opt.state_numel == 224
         g = torch.Generator().manual_seed(7)
         loss_fn = lambda out, lab: F.nll_loss(F.log_softmax(out, dim=1), lab)
         for step in range(3):
@@ -138,6 +142,24 @@ def _sharded_worker(rank, world, port, ret):
         ret["layout"] = (opt.regions, [s_[1:] for s_ in opt.slices])
     finally:
         dist.destroy_process_group()
+
+
+def test_sharded_layout_tiles_every_region():
+    for n_early, numel in ((0, 1), (0, 445), (40, 445), (3, 4), (5003, 75004)):
+        for world in (1, 2, 3, 4, 7, 16):
+            per_rank = [sharded_layout(n_early, numel, world, r) for r in range(world)]
+            regions = per_rank[0][0]
+            assert len(regions) == (2 if n_early else 1)
+            assert regions[0][0] == 0 and all(n % (4 * world) == 0 for _, n in regions)
+            assert regions[-1][0] + regions[-1][1] - numel < 4 * world * len(regions)
+            if n_early:
+                assert n_early <= regions[0][1] < n_early + 4 * world and regions[1][0] == regions[0][1]
+            for r, (reg, slices, state_numel) in enumerate(per_rank):
+                assert reg == regions and state_numel == sum(n for _, n in regions) // world
+                o = 0
+                for (begin, n), (lo, sl, so) in zip(regions, slices):
+                    assert sl == n // world and lo == begin + r * sl and so == o      # slice r of the region, state packed
+                    o += sl
 
 
 def test_sharded_adam_two_ranks_equal_single_process_adam_on_the_global_batch():
