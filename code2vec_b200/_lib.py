@@ -15,6 +15,7 @@ ABI_VERSION = 1
 TOPK_MAX = 16                # C2V_TOPK_MAX: the largest k of the fused top-k (c2v_label_topk / c2v_angular_topk)
 KNN_EXCLUDE_MAX = 4          # C2V_KNN_EXCLUDE_MAX: excluded bank rows per query of c2v_knn_topk / c2v_knn_pairs
 KNN_MAX_Q = 2048             # queries per c2v_knn_* call
+DROPOUT_SEED_ON_DEVICE = 2   # C2V_DROPOUT_SEED_ON_DEVICE: c2v_dropout.seed is the device address of the key
 
 c_i32, c_i64, c_f32, c_vp, c_sz = ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_void_p, ctypes.c_size_t
 
@@ -113,6 +114,9 @@ SYMBOLS = {
                                                    c_vp, c_vp, c_vp]),
     "c2v_count_unit_contexts": (ctypes.c_int, [c_vp, c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp]),
     "c2v_adam_step": (ctypes.c_int, [c_vp, c_vp, c_vp, c_vp, c_i64, c_f32, c_f32, c_f32, c_f32, c_f32, c_i64, c_f32, c_i32, c_vp]),
+    "c2v_adam_step_capturable": (ctypes.c_int, [c_vp, c_vp, c_vp, c_vp, c_i64, c_f32, c_f32, c_f32, c_f32, c_f32, c_vp, c_f32,
+                                                c_i32, c_vp]),
+    "c2v_next_dropout_key": (ctypes.c_int, [c_vp, c_vp, c_vp]),
     "c2v_adam_step_sharded": (ctypes.c_int, [c_vp, c_vp, c_vp, _P(c_vp), _P(c_vp), c_i32, c_vp, c_vp, c_i64, c_i64, c_vp, c_i64,
                                              c_f32, c_f32, c_f32, c_f32, c_f32, c_i64, c_f32, c_vp]),
     "c2v_adam_step_sharded_bulk": (ctypes.c_int, [c_vp, _P(c_vp), _P(c_vp), c_i32, c_vp, c_vp, c_i64, c_i64, c_f32, c_f32, c_f32,

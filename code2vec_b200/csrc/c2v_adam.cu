@@ -24,18 +24,25 @@ __device__ __forceinline__ float adam_grad(float g, float gscale, float wd, floa
     return fmaf(wd, p, gs) + fmaf(g, gscale, -gs);
 }
 
+// DEV_SCALARS (c2v_adam_step_capturable): step_size and inv_sqrt_bc2 are read from dev_scalars[0..1], where
+// adam_step_count_kernel left them, instead of the launch parameters.
+template <bool DEV_SCALARS = false>
 __global__ void __launch_bounds__(256)
 adam_step_kernel(float4 *__restrict__ p, float4 *__restrict__ g, float4 *__restrict__ m, float4 *__restrict__ v,
                  long long n4, float *__restrict__ pt, float *__restrict__ gt, float *__restrict__ mt, float *__restrict__ vt,
                  int tail, float step_size, float one_minus_b1, float b2, float one_minus_b2, float inv_sqrt_bc2, float eps,
-                 float wd, float gscale, int zero_grad)
+                 float wd, float gscale, int zero_grad, const float *__restrict__ dev_scalars)
 {
+    if (DEV_SCALARS) { step_size = dev_scalars[0]; inv_sqrt_bc2 = dev_scalars[1]; }
     auto upd = [&](float &pp, float &gg, float &mm, float &vv) {
         const float gr = adam_grad(gg, gscale, wd, pp);
         mm = mm + (gr - mm) * one_minus_b1;                 // exp_avg.lerp_(grad, 1 - beta1)
         vv = vv * b2 + one_minus_b2 * gr * gr;              // exp_avg_sq.mul_(beta2).addcmul_(grad, grad, value=1 - beta2)
         const float denom = sqrtf(vv) * inv_sqrt_bc2 + eps;
-        pp = pp - step_size * (mm / denom);                 // param.addcdiv_(exp_avg, denom, value=-step_size)
+        // param.addcdiv_(exp_avg, denom, value=-step_size).  One fused multiply-add, written out for DEV_SCALARS: there
+        // the compiler left some products unfused, and the update would round differently from the by-value kernel's
+        if (DEV_SCALARS) pp = fmaf(-step_size, mm / denom, pp);
+        else pp = pp - step_size * (mm / denom);
         if (zero_grad) gg = 0.0f;
     };
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
@@ -51,6 +58,18 @@ adam_step_kernel(float4 *__restrict__ p, float4 *__restrict__ g, float4 *__restr
         pt[i] = P; mt[i] = M; vt[i] = V;
         if (zero_grad) gt[i] = G;
     }
+}
+
+// The step count of c2v_adam_step_capturable: state = {int64 step; float step_size; float inv_sqrt_bc2}.  The bias
+// corrections use c2v_adam_step's host expressions, in double.
+__global__ void adam_step_count_kernel(long long *state, float lr, float beta1, float beta2)
+{
+    const long long t = state[0] + 1;
+    state[0] = t;
+    const double bc1 = 1.0 - pow((double)beta1, (double)t), bc2 = 1.0 - pow((double)beta2, (double)t);
+    float *f = reinterpret_cast<float *>(state + 1);
+    f[0] = (float)((double)lr / bc1);
+    f[1] = (float)(1.0 / sqrt(bc2));
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -288,22 +307,26 @@ using namespace c2v;
 
 static bool misaligned(const void *ptr, uintptr_t a) { return (reinterpret_cast<uintptr_t>(ptr) & (a - 1)) != 0; }
 
-extern "C" int c2v_adam_step(float *param, float *grad, float *exp_avg, float *exp_avg_sq, int64_t n, float lr,
-                             float beta1, float beta2, float eps, float weight_decay, int64_t step, float grad_scale,
-                             int32_t zero_grad, void *stream)
+static bool adam_buffers_ok(const char *fn, const float *param, const float *grad, const float *exp_avg,
+                            const float *exp_avg_sq, int64_t n)
 {
-    if (!param || !grad || !exp_avg || !exp_avg_sq || n < 1 || step < 1) {
-        set_error("c2v_adam_step: bad argument");
-        return C2V_EINVAL;
+    if (!param || !grad || !exp_avg || !exp_avg_sq || n < 1) {
+        set_error("%s: bad argument", fn);
+        return false;
     }
     if ((reinterpret_cast<uintptr_t>(param) | reinterpret_cast<uintptr_t>(grad) | reinterpret_cast<uintptr_t>(exp_avg) |
          reinterpret_cast<uintptr_t>(exp_avg_sq)) & 15) {
-        set_error("c2v_adam_step: buffers must be 16-byte aligned");
-        return C2V_EINVAL;
+        set_error("%s: buffers must be 16-byte aligned", fn);
+        return false;
     }
-    const double bc1 = 1.0 - pow((double)beta1, (double)step), bc2 = 1.0 - pow((double)beta2, (double)step);
-    const float step_size = (float)((double)lr / bc1);
-    const float inv_sqrt_bc2 = (float)(1.0 / sqrt(bc2));
+    return true;
+}
+
+// the flat update kernel; dev_scalars != NULL: its DEV_SCALARS instantiation
+static int launch_adam_flat(float *param, float *grad, float *exp_avg, float *exp_avg_sq, int64_t n, float step_size,
+                            float beta1, float beta2, float inv_sqrt_bc2, float eps, float weight_decay, float grad_scale,
+                            int32_t zero_grad, const float *dev_scalars, cudaStream_t st)
+{
     const long long n4 = n / 4;
     const int tail = (int)(n % 4);
     int dev = 0, sms = 0;
@@ -312,12 +335,45 @@ extern "C" int c2v_adam_step(float *param, float *grad, float *exp_avg, float *e
     long long blocks = (n4 + 255) / 256;
     if (blocks > (long long)sms * 16) blocks = (long long)sms * 16;
     if (blocks < 1) blocks = 1;
-    adam_step_kernel<<<(unsigned)blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+    (dev_scalars ? adam_step_kernel<true> : adam_step_kernel<false>)<<<(unsigned)blocks, 256, 0, st>>>(
         reinterpret_cast<float4 *>(param), reinterpret_cast<float4 *>(grad), reinterpret_cast<float4 *>(exp_avg),
         reinterpret_cast<float4 *>(exp_avg_sq), n4, param + n4 * 4, grad + n4 * 4, exp_avg + n4 * 4, exp_avg_sq + n4 * 4, tail,
-        step_size, 1.0f - beta1, beta2, 1.0f - beta2, inv_sqrt_bc2, eps, weight_decay, grad_scale, zero_grad);
+        step_size, 1.0f - beta1, beta2, 1.0f - beta2, inv_sqrt_bc2, eps, weight_decay, grad_scale, zero_grad, dev_scalars);
     C2V_LAUNCH_OK("adam_step_kernel");
     return C2V_OK;
+}
+
+extern "C" int c2v_adam_step(float *param, float *grad, float *exp_avg, float *exp_avg_sq, int64_t n, float lr,
+                             float beta1, float beta2, float eps, float weight_decay, int64_t step, float grad_scale,
+                             int32_t zero_grad, void *stream)
+{
+    if (!adam_buffers_ok("c2v_adam_step", param, grad, exp_avg, exp_avg_sq, n)) return C2V_EINVAL;
+    if (step < 1) {
+        set_error("c2v_adam_step: bad argument");
+        return C2V_EINVAL;
+    }
+    const double bc1 = 1.0 - pow((double)beta1, (double)step), bc2 = 1.0 - pow((double)beta2, (double)step);
+    const float step_size = (float)((double)lr / bc1);
+    const float inv_sqrt_bc2 = (float)(1.0 / sqrt(bc2));
+    return launch_adam_flat(param, grad, exp_avg, exp_avg_sq, n, step_size, beta1, beta2, inv_sqrt_bc2, eps, weight_decay,
+                            grad_scale, zero_grad, nullptr, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int c2v_adam_step_capturable(float *param, float *grad, float *exp_avg, float *exp_avg_sq, int64_t n, float lr,
+                                        float beta1, float beta2, float eps, float weight_decay, void *step_state,
+                                        float grad_scale, int32_t zero_grad, void *stream)
+{
+    if (!adam_buffers_ok("c2v_adam_step_capturable", param, grad, exp_avg, exp_avg_sq, n)) return C2V_EINVAL;
+    if (!step_state || (reinterpret_cast<uintptr_t>(step_state) & 7)) {
+        set_error("c2v_adam_step_capturable: step_state must be an 8-byte aligned device buffer of 16 bytes");
+        return C2V_EINVAL;
+    }
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    long long *state = static_cast<long long *>(step_state);
+    adam_step_count_kernel<<<1, 1, 0, st>>>(state, lr, beta1, beta2);
+    C2V_LAUNCH_OK("adam_step_count_kernel");
+    return launch_adam_flat(param, grad, exp_avg, exp_avg_sq, n, 0.0f, beta1, beta2, 0.0f, eps, weight_decay, grad_scale,
+                            zero_grad, reinterpret_cast<const float *>(state + 1), st);
 }
 
 extern "C" int c2v_adam_step_sharded(const float *param_local, float *param_multicast, const float *grad_multicast,

@@ -131,6 +131,51 @@ EncodeWorkspace carve_encode_workspace(const c2v_dims *d, int B, int L, void *ba
     return carve_encode_workspace_n(d, B, (long long)B * L, base, nullptr);
 }
 
+// c2v_dropout.training: bit 0 = dropout on, C2V_DROPOUT_SEED_ON_DEVICE = `seed` is the device address of the key.
+// Checked before any CUDA call.
+static bool dropout_ok(const char *fn, const c2v_dropout *drop)
+{
+    if (!drop) return true;
+    if (drop->training & ~(1 | C2V_DROPOUT_SEED_ON_DEVICE)) {
+        set_error("%s: unknown dropout flag bits 0x%x", fn, (unsigned)drop->training);
+        return false;
+    }
+    if ((drop->training & C2V_DROPOUT_SEED_ON_DEVICE) && (drop->seed == 0 || (drop->seed & 7))) {
+        set_error("%s: C2V_DROPOUT_SEED_ON_DEVICE needs the 8-byte aligned device address of the key in `seed`", fn);
+        return false;
+    }
+    return true;
+}
+
+// the dropout fields of EncodeArgs (model.py:26-29): dropout runs when bit 0 is set and 0 < p < 1
+static void set_dropout(EncodeArgs &a, const c2v_dropout *drop)
+{
+    a.drop_p = 0.0f; a.drop_scale = 1.0f; a.seed = 0; a.seed_dev = nullptr;
+    if (drop && (drop->training & 1) && drop->p > 0.0f && drop->p < 1.0f) {
+        a.drop_p = drop->p; a.drop_scale = 1.0f / (1.0f - drop->p);
+        if (drop->training & C2V_DROPOUT_SEED_ON_DEVICE)
+            a.seed_dev = reinterpret_cast<const unsigned long long *>(static_cast<uintptr_t>(drop->seed));
+        else
+            a.seed = drop->seed;
+    }
+}
+
+// splitmix64 (Steele, Lea and Flood 2014): the output for the generator state x
+__device__ __forceinline__ unsigned long long splitmix64(unsigned long long x)
+{
+    unsigned long long z = x + 0x9E3779B97F4A7C15ull;
+    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+    return z ^ (z >> 31);
+}
+
+__global__ void next_dropout_key_kernel(long long *state, unsigned long long *key)
+{
+    const long long counter = state[1];
+    *key = splitmix64((unsigned long long)state[0] + (unsigned long long)counter);
+    state[1] = counter + 1;
+}
+
 }  // namespace c2v
 
 using namespace c2v;
@@ -186,6 +231,7 @@ static int encode_forward_impl(const char *fn, const c2v_dims *d, const c2v_para
         set_error("%s: NULL parameter pointer", fn);
         return C2V_EINVAL;
     }
+    if (!dropout_ok(fn, drop)) return C2V_EINVAL;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     int *row_bag = nullptr;
     EncodeWorkspace ws = carve_encode_workspace_n(d, B, N, workspace, offsets ? &row_bag : nullptr);
@@ -224,10 +270,7 @@ static int encode_forward_impl(const char *fn, const c2v_dims *d, const c2v_para
     a.Et = d->terminal_embed; a.Ep = d->path_embed; a.H = d->encode;
     a.D = 2 * a.Et + a.Ep;
     a.L = L; a.N = N;
-    a.drop_p = 0.0f; a.drop_scale = 1.0f; a.seed = 0;
-    if (drop && drop->training && drop->p > 0.0f && drop->p < 1.0f) {   // model.py:26-29
-        a.drop_p = drop->p; a.drop_scale = 1.0f / (1.0f - drop->p); a.seed = drop->seed;
-    }
+    set_dropout(a, drop);
     a.attention = attention;
     a.stash_x = x_stash;
     a.flags = 0;
@@ -908,6 +951,7 @@ static int encode_backward_impl(const c2v_dims *d, const c2v_params *p, const in
         set_error("c2v_encode_backward: NULL gradient pointer");
         return C2V_EINVAL;
     }
+    if (!dropout_ok("c2v_encode_backward", drop)) return C2V_EINVAL;
     EncodeArgs a;
     memset(&a, 0, sizeof(a));
     a.starts = reinterpret_cast<const long long *>(starts);
@@ -919,10 +963,7 @@ static int encode_backward_impl(const c2v_dims *d, const c2v_params *p, const in
     a.Et = d->terminal_embed; a.Ep = d->path_embed; a.H = d->encode;
     a.D = 2 * a.Et + a.Ep;
     a.L = L; a.N = N;
-    a.drop_p = 0.0f; a.drop_scale = 1.0f;
-    if (drop && drop->training && drop->p > 0.0f && drop->p < 1.0f) {
-        a.drop_p = drop->p; a.drop_scale = 1.0f / (1.0f - drop->p); a.seed = drop->seed;
-    }
+    set_dropout(a, drop);
     a.bag_off = reinterpret_cast<const long long *>(offsets);
     a.n_bags = B;
     return launch_encode_backward(d, p, a, B, code_vector, attention, d_code_vector, d_attention,
@@ -1026,6 +1067,18 @@ int c2v_encode_backward_packed_sparse(const c2v_dims *d, const c2v_params *p, co
     if (!row_slots_ok("c2v_encode_backward_packed_sparse", slots, grads)) return C2V_EINVAL;
     return encode_backward_impl(d, p, starts, paths, ends, offsets, B, N, L, drop, code_vector, attention, x_stash,
                                 d_code_vector, d_attention, grads, workspace, workspace_bytes, phase, stream, slots);
+}
+
+int c2v_next_dropout_key(int64_t *rng_state, uint64_t *key_out, void *stream)
+{
+    if (!rng_state || !key_out || (reinterpret_cast<uintptr_t>(rng_state) & 7) || (reinterpret_cast<uintptr_t>(key_out) & 7)) {
+        set_error("c2v_next_dropout_key: rng_state and key_out must be 8-byte aligned device pointers");
+        return C2V_EINVAL;
+    }
+    next_dropout_key_kernel<<<1, 1, 0, static_cast<cudaStream_t>(stream)>>>(reinterpret_cast<long long *>(rng_state),
+                                                                            reinterpret_cast<unsigned long long *>(key_out));
+    C2V_LAUNCH_OK("next_dropout_key_kernel");
+    return C2V_OK;
 }
 
 }  // extern "C"

@@ -96,7 +96,7 @@ __device__ __forceinline__ void load_wrow_chunk(const float *__restrict__ W, int
 }
 
 // SPARSE: compact embedding gradients as in backward_dc_tc_kernel (slot maps in sl, a parameter behind the others)
-template <bool VEC, bool PACKED = false, bool SPARSE = false>
+template <bool VEC, bool PACKED = false, bool SPARSE = false, bool SEED_DEV = false>
 __global__ void __launch_bounds__(THREADS)
 backward_rows_kernel(const EncodeArgs a, const BackwardArgs b, const int Hs, const c2v_row_slots sl)
 {
@@ -164,7 +164,7 @@ backward_rows_kernel(const EncodeArgs a, const BackwardArgs b, const int Hs, con
                     xh[k] = (xr[c] - mean) * rstd;
                     tt[k] = tanh_accurate(fmaf(xh[k], a.ln_g[c], a.ln_b[c]));
                     if (a.drop_p > 0.0f) {
-                        if ((k & 3) == 0) dbits = dropout_bits(a.seed, drow, c >> 2);      // columns c .. c+3
+                        if ((k & 3) == 0) dbits = dropout_bits(dropout_key<SEED_DEV>(a), drow, c >> 2);      // columns c .. c+3
                         const unsigned w = (k & 3) == 0 ? dbits.x : (k & 3) == 1 ? dbits.y : (k & 3) == 2 ? dbits.z : dbits.w;
                         dm[k] = dropout_mul(w, a.drop_p, a.drop_scale);
                     }
@@ -326,7 +326,7 @@ backward_rows_kernel(const EncodeArgs a, const BackwardArgs b, const int Hs, con
 // in registers for the whole launch, one Philox block serves four columns, and padded contexts (attention weight
 // exactly 0) cost one zero store.  encode_size % 4 == 0, <= 256.
 // ------------------------------------------------------------------------------------
-template <int NG, bool PACKED = false>                        // 128-column groups: 1 (encode_size <= 128) or 2
+template <int NG, bool PACKED = false, bool SEED_DEV = false> // 128-column groups: 1 (encode_size <= 128) or 2
 __global__ void __launch_bounds__(256, NG == 1 ? 4 : 2)
 backward_rows_lite_kernel(const EncodeArgs a, const BackwardArgs b)
 {
@@ -395,7 +395,7 @@ backward_rows_lite_kernel(const EncodeArgs a, const BackwardArgs b)
 #pragma unroll
         for (int g = 0; g < NG; ++g) {
             uint4 bits = make_uint4(0u, 0u, 0u, 0u);
-            if (on[g] && a.drop_p > 0.0f) bits = dropout_bits(a.seed, drow, g * 32 + lane);
+            if (on[g] && a.drop_p > 0.0f) bits = dropout_bits(dropout_key<SEED_DEV>(a), drow, g * 32 + lane);
             const float gam[4] = {g4[g].x, g4[g].y, g4[g].z, g4[g].w}, bet[4] = {b4[g].x, b4[g].y, b4[g].z, b4[g].w};
             const unsigned bw[4] = {bits.x, bits.y, bits.z, bits.w};
 #pragma unroll
@@ -641,8 +641,12 @@ int launch_encode_backward(const c2v_dims *d, const c2v_params *p, const EncodeA
     int dev = 0, sms = 0;
     C2V_CUDA_OK(cudaGetDevice(&dev));
     C2V_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    const bool dev_key = a.drop_p > 0.0f && a.seed_dev;       // C2V_DROPOUT_SEED_ON_DEVICE: the SEED_DEV instantiations
     if (x_stash && dc_tc && (a.H & 3) == 0) {                  // no GEMM left in this kernel: one warp per row
-        if (a.H <= 128) (packed ? backward_rows_lite_kernel<1, true> : backward_rows_lite_kernel<1>)<<<sms * 16, 256, 0, st>>>(a, b);
+        if (dev_key) {
+            if (a.H <= 128) (packed ? backward_rows_lite_kernel<1, true, true> : backward_rows_lite_kernel<1, false, true>)<<<sms * 16, 256, 0, st>>>(a, b);
+            else (packed ? backward_rows_lite_kernel<2, true, true> : backward_rows_lite_kernel<2, false, true>)<<<sms * 8, 256, 0, st>>>(a, b);
+        } else if (a.H <= 128) (packed ? backward_rows_lite_kernel<1, true> : backward_rows_lite_kernel<1>)<<<sms * 16, 256, 0, st>>>(a, b);
         else (packed ? backward_rows_lite_kernel<2, true> : backward_rows_lite_kernel<2>)<<<sms * 8, 256, 0, st>>>(a, b);
         C2V_LAUNCH_OK("backward_rows_lite_kernel");
         if (phase == 1) {                                       // path sub-vector + dW; start / end follow in phase 2
@@ -660,10 +664,15 @@ int launch_encode_backward(const c2v_dims *d, const c2v_params *p, const EncodeA
     }
     {
     const bool sparse = !dc_tc && slots && (slots->terminal || slots->path);     // (with dc_tc K3c scatters)
-    auto kern = sparse ? (packed ? (vec ? backward_rows_kernel<true, true, true> : backward_rows_kernel<false, true, true>)
-                                 : (vec ? backward_rows_kernel<true, false, true> : backward_rows_kernel<false, false, true>))
-                       : (packed ? (vec ? backward_rows_kernel<true, true> : backward_rows_kernel<false, true>)
-                                 : (vec ? backward_rows_kernel<true> : backward_rows_kernel<false>));
+    auto kern = dev_key
+        ? (sparse ? (packed ? (vec ? backward_rows_kernel<true, true, true, true> : backward_rows_kernel<false, true, true, true>)
+                            : (vec ? backward_rows_kernel<true, false, true, true> : backward_rows_kernel<false, false, true, true>))
+                  : (packed ? (vec ? backward_rows_kernel<true, true, false, true> : backward_rows_kernel<false, true, false, true>)
+                            : (vec ? backward_rows_kernel<true, false, false, true> : backward_rows_kernel<false, false, false, true>)))
+        : (sparse ? (packed ? (vec ? backward_rows_kernel<true, true, true> : backward_rows_kernel<false, true, true>)
+                            : (vec ? backward_rows_kernel<true, false, true> : backward_rows_kernel<false, false, true>))
+                  : (packed ? (vec ? backward_rows_kernel<true, true> : backward_rows_kernel<false, true>)
+                            : (vec ? backward_rows_kernel<true> : backward_rows_kernel<false>)));
     c2v_row_slots sl = {nullptr, nullptr};
     if (sparse) sl = *slots;
     C2V_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));

@@ -110,6 +110,9 @@ struct EncodeArgs {
     const long long *bag_off;
     const int *row_bag;
     int n_bags;
+    // C2V_DROPOUT_SEED_ON_DEVICE: the dropout key is *seed_dev, loaded at run time by the SEED_DEV instantiations (so that
+    // a captured CUDA graph draws a fresh key at every replay); NULL otherwise.  Behind every other field, like bag_off.
+    const unsigned long long *seed_dev;
 };
 
 #ifdef __CUDACC__
@@ -134,6 +137,13 @@ template <bool PACKED>
 __device__ __forceinline__ long long dropout_row(const EncodeArgs &a, long long row, long long bag)
 {
     return PACKED ? bag * a.L + (row - bag_first_row<true>(a, bag)) : row;
+}
+// The Philox key of the dropout mask: the launch parameter, or (SEED_DEV) the key the caller keeps in device memory.  Read
+// after pdl_wait(): the kernel that wrote the key may be the one this launch overlaps.
+template <bool SEED_DEV>
+__device__ __forceinline__ unsigned long long dropout_key(const EncodeArgs &a)
+{
+    return SEED_DEV ? *a.seed_dev : a.seed;
 }
 #endif
 int launch_row_bag(const long long *bag_off, int B, long long N, int *row_bag, cudaStream_t st);

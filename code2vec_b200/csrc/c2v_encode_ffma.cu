@@ -42,7 +42,7 @@ int launch_transpose_w(const float *W, float *Wt, int H, int D, int Hs, cudaStre
 // ------------------------------------------------------------------------------------
 // K1a
 // ------------------------------------------------------------------------------------
-template <bool VEC, bool PACKED = false>
+template <bool VEC, bool PACKED = false, bool SEED_DEV = false>
 __global__ void __launch_bounds__(THREADS)
 encode_ffma_kernel(const EncodeArgs a, const int Hs)
 {
@@ -86,7 +86,7 @@ encode_ffma_kernel(const EncodeArgs a, const int Hs)
             float u = 0.0f;
             for (int c = lane; c < H; c += 32) {
                 float y = tanh_accurate((xr[c] - mean) * rstd * a.ln_g[c] + a.ln_b[c]);
-                if (a.drop_p > 0.0f) y *= dropout_mask_at(a.seed, drow, c, a.drop_p, a.drop_scale);
+                if (a.drop_p > 0.0f) y *= dropout_mask_at(dropout_key<SEED_DEV>(a), drow, c, a.drop_p, a.drop_scale);
                 xr[c] = y;
                 u = fmaf(y, a.attn[c], u);
             }
@@ -146,8 +146,11 @@ int launch_encode_ffma(const EncodeArgs &a, cudaStream_t st)
         set_error("encode_ffma: encode_size %d needs %d B of shared memory (> 227 KB)", a.H, lay.total);
         return C2V_EUNSUPPORTED;
     }
-    auto kern = a.bag_off ? (vec ? encode_ffma_kernel<true, true> : encode_ffma_kernel<false, true>)
-                          : (vec ? encode_ffma_kernel<true> : encode_ffma_kernel<false>);
+    auto kern = (a.drop_p > 0.0f && a.seed_dev)
+                    ? (a.bag_off ? (vec ? encode_ffma_kernel<true, true, true> : encode_ffma_kernel<false, true, true>)
+                                 : (vec ? encode_ffma_kernel<true, false, true> : encode_ffma_kernel<false, false, true>))
+                    : (a.bag_off ? (vec ? encode_ffma_kernel<true, true> : encode_ffma_kernel<false, true>)
+                                 : (vec ? encode_ffma_kernel<true> : encode_ffma_kernel<false>));
     C2V_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, lay.total));
     int occ = 1;
     C2V_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, THREADS, lay.total));

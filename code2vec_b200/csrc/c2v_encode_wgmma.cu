@@ -133,7 +133,7 @@ int launch_split_w_tcgen05(const c2v_dims *d, const float *W, EncodeWorkspace &w
 // ------------------------------------------------------------------------------------
 // the kernel
 // ------------------------------------------------------------------------------------
-template <bool DROPOUT, int HV, bool PACKED = false>
+template <bool DROPOUT, int HV, bool PACKED = false, bool SEED_DEV = false>
 __global__ void __launch_bounds__(WgCfg<(HV > 128)>::THREADS, 1)
 encode_wgmma_kernel(const EncodeArgs a)
 {
@@ -260,7 +260,7 @@ encode_wgmma_kernel(const EncodeArgs a)
                     float y0 = tanh_from_scaled(fmaf(fmaf(acc[4 * j + 2 * h], nrm[h], shift[h]), gm.x, bt.x));
                     float y1 = tanh_from_scaled(fmaf(fmaf(acc[4 * j + 2 * h + 1], nrm[h], shift[h]), gm.y, bt.y));
                     if (DROPOUT) {
-                        const uint4 bits = dropout_bits(a.seed, PACKED ? dropout_row<true>(a, row[h], bag_r[h]) : row[h], c >> 2);
+                        const uint4 bits = dropout_bits(dropout_key<SEED_DEV>(a), PACKED ? dropout_row<true>(a, row[h], bag_r[h]) : row[h], c >> 2);
                         y0 *= dropout_mul((m4 & 1) ? bits.z : bits.x, a.drop_p, a.drop_scale);
                         y1 *= dropout_mul((m4 & 1) ? bits.w : bits.y, a.drop_p, a.drop_scale);
                     }
@@ -401,13 +401,16 @@ static int launch_wg(void (*kern)(const EncodeArgs), const EncodeArgs &a, cudaSt
 template <bool PACKED>
 static int launch_encode_wg(const EncodeArgs &a, cudaStream_t st)
 {
-    const bool drop = a.drop_p > 0.0f;
+    const bool drop = a.drop_p > 0.0f, dev_key = drop && a.seed_dev;
     if (a.H == 256)
-        return launch_wg<true>(drop ? encode_wgmma_kernel<true, 256, PACKED> : encode_wgmma_kernel<false, 256, PACKED>, a, st);
+        return launch_wg<true>(dev_key ? encode_wgmma_kernel<true, 256, PACKED, true>
+                               : drop ? encode_wgmma_kernel<true, 256, PACKED> : encode_wgmma_kernel<false, 256, PACKED>, a, st);
     if (a.H == 128)
-        return launch_wg<false>(drop ? encode_wgmma_kernel<true, 128, PACKED> : encode_wgmma_kernel<false, 128, PACKED>, a, st);
+        return launch_wg<false>(dev_key ? encode_wgmma_kernel<true, 128, PACKED, true>
+                                : drop ? encode_wgmma_kernel<true, 128, PACKED> : encode_wgmma_kernel<false, 128, PACKED>, a, st);
     if (a.H == 100)
-        return launch_wg<false>(drop ? encode_wgmma_kernel<true, 100, PACKED> : encode_wgmma_kernel<false, 100, PACKED>, a, st);
+        return launch_wg<false>(dev_key ? encode_wgmma_kernel<true, 100, PACKED, true>
+                                : drop ? encode_wgmma_kernel<true, 100, PACKED> : encode_wgmma_kernel<false, 100, PACKED>, a, st);
     set_error("encode_wgmma_kernel: encode_size %d not supported (100, 128 or 256)", a.H);
     return C2V_EUNSUPPORTED;
 }

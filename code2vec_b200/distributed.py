@@ -76,9 +76,13 @@ class FlatAdam:
     """torch.optim.Adam(model.parameters(), lr, betas, weight_decay) (main.py:138) as ONE kernel launch per step
     (`c2v_adam_step`): parameters, like the gradients of `bucket`, become views into one flat buffer; the step reads
     p, g, m, v once, writes p, m, v and leaves the gradient zeroed for the next backward (main.py:171), folding the
-    1/world of the data-parallel mean into the read.  Dense, same update rule and operation order as torch's Adam."""
+    1/world of the data-parallel mean into the read.  Dense, same update rule and operation order as torch's Adam.
 
-    def __init__(self, bucket, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0):
+    capturable=True (torch.optim.Adam's flag): the step count lives on the device (`step_state`, see
+    c2v_adam_step_capturable) and every step, eager or inside a CUDA graph, runs the capturable kernels; `t` is then not
+    kept (read `step_count()`).  With capturable=False a step cannot be captured."""
+
+    def __init__(self, bucket, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, capturable=False):
         self.bucket = bucket
         self.lr, self.betas, self.eps, self.weight_decay = float(lr), (float(betas[0]), float(betas[1])), float(eps), float(weight_decay)
         flat = torch.empty_like(bucket.flat)
@@ -92,20 +96,33 @@ class FlatAdam:
         self.exp_avg = torch.zeros_like(flat)
         self.exp_avg_sq = torch.zeros_like(flat)
         self.t = 0
+        self.capturable = bool(capturable)
+        self.step_state = _step_state(flat.device) if self.capturable else None
+
+    def step_count(self):
+        """the number of steps taken (synchronises in capturable mode)"""
+        return int(self.step_state[0]) if self.capturable else self.t
 
     def step(self, grad_scale=1.0, zero_grad=True):
         import ctypes
         from . import _lib
         lib = _lib.load()
-        self.t += 1
+        _check_capturable(self.capturable, "FlatAdam")
         P = lambda t: ctypes.c_void_p(t.data_ptr())
         dev = self.flat_param.device
         with torch.cuda.device(dev):
-            rc = lib.c2v_adam_step(P(self.flat_param), P(self.bucket.flat), P(self.exp_avg), P(self.exp_avg_sq),
-                                   self.flat_param.numel(), self.lr, self.betas[0], self.betas[1], self.eps,
-                                   self.weight_decay, self.t, float(grad_scale), 1 if zero_grad else 0,
-                                   ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
-        _lib.check(rc, "c2v_adam_step")
+            stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            if self.capturable:
+                rc = lib.c2v_adam_step_capturable(P(self.flat_param), P(self.bucket.flat), P(self.exp_avg), P(self.exp_avg_sq),
+                                                  self.flat_param.numel(), self.lr, self.betas[0], self.betas[1], self.eps,
+                                                  self.weight_decay, P(self.step_state), float(grad_scale),
+                                                  1 if zero_grad else 0, stream)
+            else:
+                self.t += 1
+                rc = lib.c2v_adam_step(P(self.flat_param), P(self.bucket.flat), P(self.exp_avg), P(self.exp_avg_sq),
+                                       self.flat_param.numel(), self.lr, self.betas[0], self.betas[1], self.eps,
+                                       self.weight_decay, self.t, float(grad_scale), 1 if zero_grad else 0, stream)
+        _lib.check(rc, "c2v_adam_step_capturable" if self.capturable else "c2v_adam_step")
         # the kernel wrote through raw pointers: tell autograd (and the weight-image caches of the model, which key on
         # Tensor._version) that every parameter changed, as an in-place torch op would
         for p in self.bucket.params:
@@ -113,6 +130,18 @@ class FlatAdam:
 
     def zero_grad(self):
         self.bucket.zero()
+
+
+def _step_state(device):
+    """the device step-state of c2v_adam_step_capturable: {int64 step; float step_size; float inv_sqrt_bc2}, step 0"""
+    return torch.zeros(2, dtype=torch.int64, device=device)
+
+
+def _check_capturable(capturable, name):
+    from .functional import capturing
+    if capturing() and not capturable:
+        raise RuntimeError(f"{name}.step() is being captured into a CUDA graph, but the optimizer keeps its step count on "
+                           f"the host, so every replay would repeat the captured step: construct it with capturable=True")
 
 
 def sharded_layout(n_early, numel, world, rank):
@@ -158,7 +187,7 @@ class ShardedFlatAdam:
     """
 
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, group=None, transport="auto",
-                 early=()):
+                 early=(), capturable=False):
         params = [p for p in params if p.requires_grad]
         if not params:
             raise ValueError("no trainable parameters")
@@ -168,6 +197,10 @@ class ShardedFlatAdam:
         self.group = group
         self.world = dist.get_world_size(group) if dist.is_available() and dist.is_initialized() else 1
         self.rank = dist.get_rank(group) if self.world > 1 else 0
+        if capturable and self.world > 1:
+            raise NotImplementedError("ShardedFlatAdam(capturable=True) supports one process only: the data-parallel step "
+                                      f"uses cross-GPU barriers and a side stream (world size {self.world})")
+        self.capturable = bool(capturable)
         self.lr, self.betas, self.eps, self.weight_decay = float(lr), (float(betas[0]), float(betas[1])), float(eps), float(weight_decay)
         dev, dt = self.params[0].device, self.params[0].dtype
         if dt != torch.float32:
@@ -200,6 +233,7 @@ class ShardedFlatAdam:
         self.exp_avg = torch.zeros(self.state_numel, dtype=dt, device=dev)
         self.exp_avg_sq = torch.zeros(self.state_numel, dtype=dt, device=dev)
         self.t, self.cur = 0, 0
+        self.step_state = _step_state(dev) if self.capturable else None
         self._early_done = False
         self._side = torch.cuda.Stream(dev) if (dev.type == "cuda" and len(self.regions) > 1) else None
         self._point_grads(0)
@@ -290,6 +324,13 @@ class ShardedFlatAdam:
         m, v = state if state is not None else (self.exp_avg, self.exp_avg_sq)
         dev = p_slice.device
         with torch.cuda.device(dev):
+            if self.capturable:                               # (world 1 only)
+                rc = lib.c2v_adam_step_capturable(P(p_slice), P(g_slice), P(m), P(v), p_slice.numel(), self.lr, self.betas[0],
+                                                  self.betas[1], self.eps, self.weight_decay, P(self.step_state), 1.0,
+                                                  1 if zero_grad else 0,
+                                                  ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
+                _lib.check(rc, "c2v_adam_step_capturable")
+                return
             rc = lib.c2v_adam_step(P(p_slice), P(g_slice), P(m), P(v), p_slice.numel(), self.lr,
                                    self.betas[0], self.betas[1], self.eps, self.weight_decay, self.t, 1.0 / self.world,
                                    1 if zero_grad else 0, ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
@@ -364,8 +405,9 @@ class ShardedFlatAdam:
     def step(self):
         """reduce this step's gradients over the ranks (mean), Adam, parameters identical everywhere afterwards; the
         other bucket is left zeroed and becomes the target of the next backward (main.py:171 + :175)."""
+        _check_capturable(self.capturable, "ShardedFlatAdam")
         cur, nxt = self.cur, 1 - self.cur
-        if not self._early_done:
+        if not self._early_done and not self.capturable:
             self.t += 1
         if self.world == 1:                                      # one launch, gradient zeroed in the same pass, no swap
             self._adam_slice(self.flat_param, self.buckets[cur], zero_grad=True)
@@ -412,8 +454,11 @@ def ddp_step(model, optimizer, bucket, starts, paths, ends, label, loss_fn):
     fused = isinstance(optimizer, FlatAdam)
     if not fused:
         bucket.zero()                       # (FlatAdam leaves the bucket zeroed at the end of its step)
-    outputs, code_vector, attention = model.forward(starts, paths, ends, label)
-    loss = loss_fn(outputs, label)
+    if loss_fn is None:                     # fused loss (Code2Vec.forward_loss)
+        loss = model.forward_loss(starts, paths, ends, label)[0]
+    else:
+        outputs, code_vector, attention = model.forward(starts, paths, ends, label)
+        loss = loss_fn(outputs, label)
     loss.backward()
     if fused:
         bucket.allreduce(average=False)     # plain sum; the 1/world is folded into the optimizer's gradient read

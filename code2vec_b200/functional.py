@@ -72,12 +72,46 @@ NO_PDL = 0x200
 GRAD_ABSMAX_READY = 0x400
 
 
+def capturing():
+    """True while the current CUDA stream is being captured into a CUDA graph"""
+    return torch.cuda.is_available() and torch.cuda.is_current_stream_capturing()
+
+
+def capture_flags(algo):
+    """`algo` of a library call made under capture: plain stream-ordered launches (no programmatic dependent launch)"""
+    return int(algo) | NO_PDL if capturing() else int(algo)
+
+
+def next_dropout_key(rng_state):
+    """A fresh int64 [1] device tensor holding the next dropout key of rng_state (int64 [2] {base, counter} on the
+    device): c2v_next_dropout_key, enqueued on the current stream (capturable)."""
+    lib = _lib.load()
+    dev = rng_state.device
+    with torch.cuda.device(dev):
+        key = torch.empty(1, dtype=torch.int64, device=dev)
+        _lib.check(lib.c2v_next_dropout_key(_ptr(rng_state), _ptr(key), _stream(dev)), "c2v_next_dropout_key")
+    return key
+
+
+def _dropout(drop_p, training, seed):
+    """c2v_dropout: `seed` is an int (the key, by value) or an int64 [1] device tensor holding it
+    (C2V_DROPOUT_SEED_ON_DEVICE; the caller keeps the tensor alive until the kernels have run)"""
+    if isinstance(seed, torch.Tensor):
+        return Dropout(float(drop_p), (1 if training else 0) | _lib.DROPOUT_SEED_ON_DEVICE, seed.data_ptr())
+    return Dropout(float(drop_p), 1 if training else 0, int(seed))
+
+
 class PrepCache:
     """A persistent workspace whose derived weight images (split / transposed copies of a weight
     matrix) are rebuilt only when the weight changed: keyed on (data_ptr, _version, size)."""
 
     def __init__(self, mirror_errors=False):
         self.buf, self.key = None, None
+        # CUDA graphs: a replay neither bumps version counters nor knows whether the weights changed since the capture, so
+        # a call under capture rebuilds the images (no REUSE_PREP), and once the owner has captured a training step the
+        # counters are not trusted at all (trust_versions = False).  A graph keeps the raw address of the workspace it
+        # was captured with: graph_bufs keeps every such buffer alive even after a larger one replaces it.
+        self.trust_versions, self.graph_bufs = True, []
         # encode workspaces: a pinned host word the finalize kernel adds its out-of-range index count to
         # (c2v_workspace_set_status_mirror), polled by raise_deferred() at the next call on this cache
         self.mirror_errors, self.err = mirror_errors, None       # (pinned memory needs the driver: allocated on first use)
@@ -85,6 +119,10 @@ class PrepCache:
     def get(self, nbytes, device, weight):
         key = (weight.data_ptr(), weight._version, str(device))
         fresh = self.buf is None or self.buf.numel() < nbytes or self.buf.device != device
+        cap = capturing()
+        if fresh and cap:
+            raise RuntimeError("a persistent workspace would be allocated under CUDA-graph capture: run the same call once "
+                               "eagerly at this batch shape before capturing it")
         if fresh:
             self.buf = _empty((nbytes,), torch.uint8, device)
             if self.mirror_errors:
@@ -94,8 +132,10 @@ class PrepCache:
                 with torch.cuda.device(device):
                     _lib.check(lib.c2v_workspace_set_status_mirror(_ptr(self.buf), ctypes.c_void_p(self.err.data_ptr()),
                                                                    _stream(device)), "c2v_workspace_set_status_mirror")
-        reuse = (not fresh) and key == self.key
+        reuse = (not fresh) and key == self.key and self.trust_versions and not cap
         self.key = key
+        if cap and not any(b is self.buf for b in self.graph_bufs):
+            self.graph_bufs.append(self.buf)
         return self.buf, reuse
 
     def raise_deferred(self, synchronize=False):
@@ -132,7 +172,8 @@ def encode_forward(dims, params, starts, paths, ends, drop_p=0.0, training=False
                 algo = int(algo) | REUSE_PREP
         else:
             ws = _empty((nbytes,), torch.uint8, dev)
-        drop = Dropout(float(drop_p), 1 if training else 0, int(seed))
+        drop = _dropout(drop_p, training, seed)
+        algo = capture_flags(algo)
         xs = _empty((B * L, dims.encode), torch.float32, dev) if stash else None
         rc = lib.c2v_encode_forward_stash(ctypes.byref(dims), ctypes.byref(params), _ptr(starts), _ptr(paths), _ptr(ends),
                                           B, L, ctypes.byref(drop), _ptr(cv), _ptr(att), _ptr(xs), _ptr(ws), ws.numel(),
@@ -232,6 +273,9 @@ def encode_forward_packed(dims, params, bags, drop_p=0.0, training=False, seed=0
     """encode_forward for a PackedBags batch -> (code_vector [B,H], attention [N]) (+ x_stash [N, H] with stash=True).
     The code vector of a bag equals the [B, L] result of the same bag up to fp32 summation order; packed context j of bag
     b draws the dropout mask of padded row b * L + j."""
+    if capturing():
+        raise RuntimeError("PackedBags batches cannot be captured into a CUDA graph: their context count N changes from "
+                           "batch to batch; capture padded [B, L] batches")
     lib = _lib.load()
     _need_cuda(bags.starts, bags.paths, bags.ends, bags.offsets)
     B, N, L = bags.B, bags.N, bags.L
@@ -246,7 +290,7 @@ def encode_forward_packed(dims, params, bags, drop_p=0.0, training=False, seed=0
                 algo = int(algo) | REUSE_PREP
         else:
             ws = _empty((nbytes,), torch.uint8, dev)
-        drop = Dropout(float(drop_p), 1 if training else 0, int(seed))
+        drop = _dropout(drop_p, training, seed)
         xs = _empty((N, dims.encode), torch.float32, dev) if stash else None
         rc = lib.c2v_encode_forward_packed(ctypes.byref(dims), ctypes.byref(params), _ptr(bags.starts), _ptr(bags.paths),
                                            _ptr(bags.ends), _ptr(bags.offsets), B, N, L, ctypes.byref(drop), _ptr(cv),
@@ -269,6 +313,7 @@ def _label_ws(dims, B, dev, algo, cache, weight, nbytes=None, absmax_ready=False
     workspace, or None if not fresh (the backward calls then run on the CUDA cores)."""
     if nbytes is None:
         nbytes = _lib.load().c2v_label_workspace_bytes(ctypes.byref(dims), B)
+    algo = capture_flags(algo)
     if cache is not None and weight is not None:
         ws, reuse = cache.get(nbytes, dev, weight)
         return ws, int(algo) | (REUSE_PREP if reuse else 0) | (GRAD_ABSMAX_READY if absmax_ready else 0)
@@ -574,7 +619,7 @@ def encode_backward(dims, params, starts, paths, ends, cv, att, d_cv, d_att, sha
                       _ptr(g["ln_weight"]), _ptr(g["ln_bias"]), _ptr(g["attention"]))
         nbytes = lib.c2v_encode_backward_workspace_bytes(ctypes.byref(dims), B, L)
         ws = _empty((nbytes,), torch.uint8, dev)
-        drop = Dropout(float(drop_p), 1 if training else 0, int(seed))
+        drop = _dropout(drop_p, training, seed)
         # contiguous copies (if any were needed) are bound to locals so that they outlive the launch
         cv = _f32c(cv, "code_vector"); att = _f32c(att, "attention")
         d_cv = _f32c(d_cv, "d_code_vector")
@@ -607,7 +652,7 @@ def encode_backward_packed(dims, params, bags, cv, att, d_cv, d_att, shapes, dro
                       _ptr(g["ln_weight"]), _ptr(g["ln_bias"]), _ptr(g["attention"]))
         nbytes = lib.c2v_encode_backward_packed_workspace_bytes(ctypes.byref(dims), B, N)
         ws = _empty((nbytes,), torch.uint8, dev)
-        drop = Dropout(float(drop_p), 1 if training else 0, int(seed))
+        drop = _dropout(drop_p, training, seed)
         cv = _f32c(cv, "code_vector"); att = _f32c(att, "attention")
         d_cv = _f32c(d_cv, "d_code_vector")
         d_att = _f32c(d_att, "d_attention") if d_att is not None else None

@@ -70,6 +70,7 @@ class _EncodeFn(torch.autograd.Function):
             # kept with the graph (freed with it), so that a backward with retain_graph=True can run again
             ctx.row_maps = (maps, counts, ready)
         ctx.save_for_backward(emb_t, emb_p, W, ln_g, ln_b, attn, starts, paths, ends, cv, att)
+        # seed: an int, or (Code2Vec.use_device_rng) the device tensor holding this forward's key, which the backward reads
         ctx.cfg = (dims, drop_p, training, seed)
         ctx.cache = cache
         return cv, att
@@ -263,6 +264,8 @@ class Code2Vec(nn.Module):
         # sparse embedding gradients (opt-in: terminal_embedding.sparse / path_embedding.sparse, as on nn.Embedding)
         self._enc_cache.sparse_indices = {}
         self._sparse_hooks = None
+        # use_device_rng(): int64 [2] {base, counter} on the device, from which every training forward draws its key
+        self._rng_base, self._rng_state = None, None
 
     # -- helpers ---------------------------------------------------------------------------
     def _dims(self):
@@ -275,6 +278,25 @@ class Code2Vec(nn.Module):
         # torch.manual_seed (main.py:120) makes runs repeatable
         self._dropout_calls += 1
         return int(torch.randint(0, 2 ** 62, (1,)).item())
+
+    def _next_device_key(self, device):
+        """use_device_rng: a fresh int64 [1] key buffer for one training forward, written on the device"""
+        self._dropout_calls += 1
+        if self._rng_state is None or self._rng_state.device != device:
+            if CF.capturing():
+                raise RuntimeError("use_device_rng: run one training forward eagerly on this device before capturing")
+            self._rng_state = torch.tensor([self._rng_base, 0], dtype=torch.int64, device=device)
+        return CF.next_dropout_key(self._rng_state)
+
+    def use_device_rng(self, seed=None):
+        """From now on every training forward draws its dropout key on the device, key k = splitmix64(base + k)
+        (c2v_next_dropout_key), so that a training step captured into a CUDA graph draws a fresh mask at every replay.
+        Eager steps and replays launch the same kernels and continue one key sequence.  base = seed, or when seed is None
+        a draw from torch's CPU generator (torch.manual_seed keeps runs repeatable).  The masks differ from those of the
+        host-drawn keys, reproducibly.  Returns self."""
+        self._rng_base = int(seed) if seed is not None else int(torch.randint(0, 2 ** 62, (1,)).item())
+        self._rng_state = None
+        return self
 
     def _head(self):
         """-> (W_out, b_out) of the label head; the angular-margin head has no bias"""
@@ -290,8 +312,23 @@ class Code2Vec(nn.Module):
         dims = self._dims()
         training = self.training and self.input_dropout is not None
         drop_p = float(self.option.dropout_prob) if training else 0.0
-        seed = self._next_seed() if training else 0
         sparse = (bool(self.terminal_embedding.sparse), bool(self.path_embedding.sparse))
+        if CF.capturing():
+            if any(sparse) and torch.is_grad_enabled():
+                raise RuntimeError("sparse embedding gradients cannot be captured into a CUDA graph: their backward waits "
+                                   "on the host for the number of rows a batch touches")
+            if torch.is_grad_enabled():
+                # a replayed optimizer step bumps no version counter: from now on this module's weight images are rebuilt
+                # at every call (no REUSE_PREP), eagerly as under capture
+                self._enc_cache.trust_versions = self._lab_cache.trust_versions = False
+        seed = 0
+        if training and self._rng_base is not None:
+            seed = self._next_device_key(starts.device)                 # (a PackedBags batch has .device too)
+        elif training:
+            if CF.capturing():
+                raise RuntimeError("a training forward with dropout draws its key on the host and would replay the same mask "
+                                   "at every replay of a CUDA graph: call Code2Vec.use_device_rng() before capturing it")
+            seed = self._next_seed()
         if any(sparse):
             self._watch_sparse_grads()
         code_vector, attention = _EncodeFn.apply(
@@ -355,6 +392,8 @@ class Code2Vec(nn.Module):
     def check_indices(self):
         """Synchronise and raise IndexError if any forward so far saw an index outside the embedding tables
         (`forward` itself raises it one call late, without synchronising: see functional.PrepCache.raise_deferred)."""
+        if CF.capturing():
+            raise RuntimeError("check_indices() synchronises the device and cannot run under CUDA-graph capture")
         self._enc_cache.raise_deferred(synchronize=True)
 
     # Every entry point below also takes a functional.PackedBags batch in place of `starts`, with paths = ends = None: the

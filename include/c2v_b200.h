@@ -111,13 +111,25 @@ typedef struct c2v_grads {
 
 /* Dropout after tanh (model.py:26-29, :60-61): keep-prob 1-p, survivors scaled by
  * 1/(1-p).  The mask is a counter-based hash of (seed, context row, column), so
- * backward regenerates it instead of storing it. training==0 or p outside (0,1)
- * means identity, as in the reference. */
+ * backward regenerates it instead of storing it. Bit 0 of `training` clear or p outside (0,1)
+ * means identity, as in the reference.
+ * training | C2V_DROPOUT_SEED_ON_DEVICE: `seed` holds the device address of a uint64 key (8-byte aligned) that the
+ * kernels load when they run instead of taking the key as a launch parameter, so that a captured CUDA graph can draw a
+ * new key at every replay (c2v_next_dropout_key); the mask for a key value is the same either way.  Every entry point that
+ * takes a c2v_dropout returns C2V_EINVAL, before any CUDA call, for other bits or for this bit with a NULL address. */
+#define C2V_DROPOUT_SEED_ON_DEVICE 2
 typedef struct c2v_dropout {
     float p;
     int32_t training;
     uint64_t seed;
 } c2v_dropout;
+
+/* Device-side dropout keys: rng_state int64 [2] = {base, counter} (device); one single-thread kernel writes
+ * *key_out = splitmix64(base + counter) and increments counter, where splitmix64(x) is the output of Steele, Lea and
+ * Flood's SplitMix64 generator in state x: z = x + 0x9E3779B97F4A7C15, z = (z ^ z >> 30) * 0xBF58476D1CE4E5B9,
+ * z = (z ^ z >> 27) * 0x94D049BB133111EB, key = z ^ z >> 31 (mod 2^64).  key_out: uint64 (device); both pointers 8-byte
+ * aligned.  Nothing is read on the host, so the call can be captured into a CUDA graph. */
+int c2v_next_dropout_key(int64_t *rng_state, uint64_t *key_out, void *stream);
 
 int c2v_abi_version(void);
 const char *c2v_last_error(void);
@@ -516,6 +528,14 @@ int c2v_build_batch_vars_packed(const int64_t *offsets, const int32_t *contexts,
 int c2v_adam_step(float *param, float *grad, float *exp_avg, float *exp_avg_sq, int64_t n, float lr,
                   float beta1, float beta2, float eps, float weight_decay, int64_t step, float grad_scale,
                   int32_t zero_grad, void *stream);
+/* c2v_adam_step with the step count on the device, for CUDA-graph capture (torch.optim.Adam(capturable=True)):
+ * step_state (device, 8-byte aligned) = {int64 step; float step_size; float inv_sqrt_bc2}.  A single-thread kernel
+ * increments step, then stores step_size = lr / (1 - beta1^step) and inv_sqrt_bc2 = 1 / sqrt(1 - beta2^step), computed
+ * in double as c2v_adam_step computes them on the host; the update kernel reads the two.  lr, the betas, eps,
+ * weight_decay and grad_scale are launch parameters (fixed in a captured graph).  step starts at 0. */
+int c2v_adam_step_capturable(float *param, float *grad, float *exp_avg, float *exp_avg_sq, int64_t n, float lr,
+                             float beta1, float beta2, float eps, float weight_decay, void *step_state, float grad_scale,
+                             int32_t zero_grad, void *stream);
 
 /* The same optimizer for data-parallel training, fused with its collective (the reference's
  * one all_reduce per step becomes one kernel per rank): for the rank's slice [slice_begin, slice_begin + slice_n) of the flat buffers the kernel
