@@ -218,19 +218,23 @@ encode_wgmma_kernel(const EncodeArgs a)
                 row[h] = (long long)tile * C::ROWS + 64 * g + 16 * w4 + (lane >> 2) + 8 * h;
                 in_range[h] = row[h] < a.N;
                 if (PACKED) bag_r[h] = in_range[h] ? bag_of_row<true>(a, row[h]) : 0;     // rows past N: any valid bag, unused
-                // LayerNorm (model.py:55-56), one pass: sum and sum of squares together; padding columns are exactly 0.
-                // var = E[x^2] - mean^2 in fp32: relative error ~2^-24 (1 + mean^2 / var), far inside the 1e-4 budget.
+                // LayerNorm (model.py:55-56) in two passes over the accumulator registers, as the CUDA-core encode and
+                // the backward compute it: the one-pass E[x^2] - mean^2 loses ~2^-24 mean^2 / var relative, which misses
+                // the 1e-4 bar once |mean| / std reaches a few tens.  Padding columns (c >= HV) are exactly 0 and stay
+                // out of the sum of squares.
                 float s = 0.f, q = 0.f;
 #pragma unroll
-                for (int j = 0; j < C::HP / 8; ++j) {
-                    const float x0 = acc[4 * j + 2 * h], x1 = acc[4 * j + 2 * h + 1];
-                    s += x0 + x1;
-                    q = fmaf(x0, x0, fmaf(x1, x1, q));
-                }
+                for (int j = 0; j < C::HP / 8; ++j) s += acc[4 * j + 2 * h] + acc[4 * j + 2 * h + 1];
                 s += __shfl_xor_sync(0xffffffffu, s, 1); s += __shfl_xor_sync(0xffffffffu, s, 2);
-                q += __shfl_xor_sync(0xffffffffu, q, 1); q += __shfl_xor_sync(0xffffffffu, q, 2);
                 const float mean = s * inv_h;
-                const float var = fmaxf(fmaf(-mean, mean, q * inv_h), 0.0f) * inv_scale * inv_scale;
+#pragma unroll
+                for (int j = 0; j < C::HP / 8; ++j) {
+                    const bool col = 8 * j + 2 * m4 < HV;
+                    const float d0 = col ? acc[4 * j + 2 * h] - mean : 0.f, d1 = col ? acc[4 * j + 2 * h + 1] - mean : 0.f;
+                    q = fmaf(d0, d0, fmaf(d1, d1, q));
+                }
+                q += __shfl_xor_sync(0xffffffffu, q, 1); q += __shfl_xor_sync(0xffffffffu, q, 2);
+                const float var = q * inv_h * inv_scale * inv_scale;
                 nrm[h] = inv_scale / sqrtf(var + C2V_LN_EPS);
                 shift[h] = -mean * nrm[h];
             }
@@ -292,10 +296,12 @@ encode_wgmma_kernel(const EncodeArgs a)
                     const float e0 = seg0 ? __expf(z[0] - m) : 0.0f, e1 = seg1 ? __expf(z[1] - m) : 0.0f;
                     const size_t slot = (size_t)(vt + bag);
                     float *pv = a.ws.part_v + slot * a.H;
+                    // a row of another bag is selected out, not multiplied by 0: its h may be NaN (an inf / NaN
+                    // embedding entry), and 0 * NaN would spread into this bag's code vector
 #pragma unroll
                     for (int j = 0; j < C::HP / 8; ++j) {
-                        float v0 = fmaf(e0, acc[4 * j], e1 * acc[4 * j + 2]);
-                        float v1 = fmaf(e0, acc[4 * j + 1], e1 * acc[4 * j + 3]);
+                        float v0 = fmaf(e0, seg0 ? acc[4 * j] : 0.0f, seg1 ? e1 * acc[4 * j + 2] : 0.0f);
+                        float v1 = fmaf(e0, seg0 ? acc[4 * j + 1] : 0.0f, seg1 ? e1 * acc[4 * j + 3] : 0.0f);
 #pragma unroll
                         for (int o = 4; o < 32; o <<= 1) {
                             v0 += __shfl_xor_sync(0xffffffffu, v0, o);

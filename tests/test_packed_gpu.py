@@ -26,7 +26,7 @@ from code2vec_b200.model import Code2Vec
 from gpu_util import random_params
 from oracle import oracle
 from philox_ref import dropout_mask
-from test_train_step_gpu import _reference, _rho, _scales
+from fp64_judge import reference as _reference, rho as _rho, scales as _scales
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device("cuda:0")

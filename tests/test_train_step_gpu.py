@@ -28,7 +28,7 @@ import torch.nn.functional as F
 from bench import WORKLOADS, synth_params, synth_pool
 from code2vec_b200.distributed import ShardedFlatAdam, ddp_step
 from code2vec_b200.model import Code2Vec
-from oracle import oracle
+from fp64_judge import reference, rho, scales
 from philox_ref import dropout_mask
 
 pytestmark = pytest.mark.gpu
@@ -149,109 +149,6 @@ def _batches(w, data, dev):
     return out
 
 
-# ---- the references ----------------------------------------------------------------------------------------------------
-def _reference(params, batch, mask, angular, dtype):
-    """oracle.torch_forward + mean NLL in `dtype` with autograd -> dict of everything the checks read"""
-    s, pth, e, lab = batch
-    p = {k: v.detach().to(dtype).requires_grad_() for k, v in params.items()}
-    taps = {}
-    ang = {"margin": MARGIN, "inverse_temp": INV_TEMP} if angular else None
-    out, cv, att = oracle.torch_forward(p, s, pth, e, lab, angular=ang, dropmask=mask.to(dtype), taps=taps)
-    for t in taps.values():
-        t.retain_grad()
-    loss = F.nll_loss(F.log_softmax(out, dim=1), lab)
-    loss.backward()
-    r = {"loss": loss.detach(), "logits": out.detach(), "cv": cv.detach(), "att": att.detach(),
-         "grads": {k: v.grad for k, v in p.items()}, "taps": {k: (v.detach(), v.grad) for k, v in taps.items()},
-         "params": {k: v.detach() for k, v in p.items()}}
-    del out, cv, att, loss, p, taps
-    return r
-
-
-def _scales(r, batch, mask, angular):
-    """S for every checked quantity: its last sum / contraction in fp64 on absolute values"""
-    s, pth, e, lab = batch
-    P = r["params"]
-    B, L = s.shape
-    x, dX = r["taps"]["x"]
-    ln, dY = r["taps"]["ln"]
-    _, dz = r["taps"]["z"]
-    H = x.shape[-1]
-    N = B * L
-    Wi = P["input_linear.weight"]
-    Et, Ep = P["terminal_embedding.weight"].shape[1], P["path_embedding.weight"].shape[1]
-    S = {}
-    adX = dX.reshape(N, H).abs()
-    # input_linear: dW = dX^T C
-    aC = torch.cat((P["terminal_embedding.weight"][s.reshape(-1)].abs(), P["path_embedding.weight"][pth.reshape(-1)].abs(),
-                    P["terminal_embedding.weight"][e.reshape(-1)].abs()), dim=1)
-    S["input_linear.weight"] = adX.t() @ aC
-    del aC
-    # embedding tables: the scatter of dC = dX W by (starts, paths, ends)
-    A = adX @ Wi.abs()
-    S["terminal_embedding.weight"] = torch.zeros_like(P["terminal_embedding.weight"]).index_add_(
-        0, s.reshape(-1), A[:, :Et]).index_add_(0, e.reshape(-1), A[:, Et + Ep:])
-    S["path_embedding.weight"] = torch.zeros_like(P["path_embedding.weight"]).index_add_(0, pth.reshape(-1), A[:, Et:Et + Ep])
-    del A, adX
-    # LayerNorm affine: d gamma = sum dy * y_hat, d beta = sum dy
-    xv = x.reshape(N, H)
-    y_hat = (xv - xv.mean(1, keepdim=True)) / torch.sqrt(xv.var(1, unbiased=False, keepdim=True) + 1e-5)
-    S["input_layer_norm.weight"] = (dY.reshape(N, H) * y_hat).abs().sum(0)
-    S["input_layer_norm.bias"] = dY.reshape(N, H).abs().sum(0)
-    del y_hat
-    # attention: d a = sum over contexts of (dz * mask) h;  code vector: sum_l att h;  attention: the softmax normaliser
-    h = torch.tanh(ln) * mask.double()
-    valid = (s > 0).double()
-    S["attention_parameter"] = torch.einsum("bl,blh->h", (dz * valid).abs(), h.abs())
-    S["cv"] = torch.einsum("bl,blh->bh", r["att"], h.abs())
-    S["att"] = r["att"].clone()
-    del h
-    cv, logits = r["cv"], r["logits"]
-    if angular:
-        W = P["output_linear"]
-        wnorm = W.norm(dim=1, keepdim=True).clamp_min(1e-12)
-        wn = W / wnorm
-        cvn = F.normalize(cv)
-        cos, Gc = r["taps"]["cos"]
-        # cos = cvn . wn^T;  dW = (dwn - (dwn . wn) wn) / |w| with dwn = Gc^T cvn
-        Ac = Gc.abs().t() @ cvn.abs()
-        S["output_linear"] = (Ac + wn.abs() * (Ac * wn.abs()).sum(1, keepdim=True)) / wnorm
-        # d cv = (dcvn - (dcvn . cvn) cvn) / |cv| with dcvn = Gc wn
-        Ad = Gc.abs() @ wn.abs()
-        S["dcv"] = (Ad + cvn.abs() * (Ad * cvn.abs()).sum(1, keepdim=True)) / cv.norm(dim=1, keepdim=True).clamp_min(1e-12)
-        del Ac, Ad
-        Sl = INV_TEMP * (cvn.abs() @ wn.abs().t())
-        # at the label column (cos > 0) the logit is s * phi(cos): phi' = cos m + sin m * cos / sin
-        c = cos.gather(1, lab[:, None])
-        sin = torch.sqrt((1.0 - c * c).clamp_min(1e-12))
-        amp = torch.where(c > 0, math.cos(MARGIN) + math.sin(MARGIN) * c.abs() / sin, torch.ones_like(c))
-        Sl.scatter_(1, lab[:, None], Sl.gather(1, lab[:, None]) * amp)
-    else:
-        G = r["taps"]["logits"][1]
-        S["output_linear.weight"] = G.abs().t() @ cv.abs()
-        S["output_linear.bias"] = G.abs().sum(0)
-        S["dcv"] = G.abs() @ P["output_linear.weight"].abs()
-        Sl = cv.abs() @ P["output_linear.weight"].abs().t() + P["output_linear.bias"].abs()
-    S["logits"] = Sl
-    lse = torch.logsumexp(logits, 1)
-    S["loss"] = (lse.abs() + logits.gather(1, lab[:, None])[:, 0].abs()).mean()
-    return S
-
-
-def _rho(a, ref, S, name, zero_violations):
-    """max |a - ref| / S over S > 0; where S == 0, `a` must be exactly 0 (recorded in zero_violations)"""
-    a = a.double()
-    nz = S > 0
-    d = (a - ref).abs()
-    if not bool(nz.all()):
-        bad = int(((a != 0) & ~nz).sum())
-        if bad:
-            zero_violations.append(f"{name}: {bad} elements nonzero where S = 0")
-    if not bool(nz.any()):
-        return 0.0
-    return float((d[nz] / S[nz]).max())
-
-
 # ---- the case ----------------------------------------------------------------------------------------------------------
 def _ulp32(x):
     _, ex = torch.frexp(x.float())
@@ -368,12 +265,12 @@ def _run_case(case):
         for k, msg in _check_adam(snap, opt.flat_param, opt.exp_avg, opt.exp_avg_sq, snap["t"]).items():
             failures.append(f"step {step} Adam {k}: {msg}")
 
-        r32 = _reference(params, batch, mask, angular, torch.float32)
+        r32 = reference(params, batch, mask, angular, torch.float32, MARGIN, INV_TEMP)
         r32 = {"loss": r32["loss"], "logits": r32["logits"], "cv": r32["cv"], "att": r32["att"], "grads": r32["grads"],
                "dcv": r32["taps"]["cv"][1]}
         torch.cuda.empty_cache()
-        r64 = _reference(params, batch, mask, angular, torch.float64)
-        S = _scales(r64, batch, mask, angular)
+        r64 = reference(params, batch, mask, angular, torch.float64, MARGIN, INV_TEMP)
+        S = scales(r64, batch, mask, angular, MARGIN, INV_TEMP)
         dxm = r64["taps"]["x"][1].abs().amax(-1).reshape(-1)
         G = (r64["taps"]["cos"] if angular else r64["taps"]["logits"])[1].abs()
         spread = {"dx_range_log2": math.log2(float(dxm.max() / dxm[dxm > 0].min())),
@@ -383,12 +280,12 @@ def _run_case(case):
         zv = []
         # stage by stage: code vector and attention, the logits / loss / prediction, then the gradients
         for name in ("cv", "att"):
-            note(step, name, _rho(captured[name], r64[name], S[name], name, zv),
-                 _rho(r32[name], r64[name], S[name], name + " (fp32 torch)", []))
-        rl32 = _rho(r32["logits"], r64["logits"], S["logits"], "logits (fp32 torch)", [])
+            note(step, name, rho(captured[name], r64[name], S[name], name, zv),
+                 rho(r32[name], r64[name], S[name], name + " (fp32 torch)", []))
+        rl32 = rho(r32["logits"], r64["logits"], S["logits"], "logits (fp32 torch)", [])
         if fused:
-            note(step, "loss", _rho(captured["loss"], r64["loss"], S["loss"], "loss", zv),
-                 _rho(r32["loss"], r64["loss"], S["loss"], "", []))
+            note(step, "loss", rho(captured["loss"], r64["loss"], S["loss"], "loss", zv),
+                 rho(r32["loss"], r64["loss"], S["loss"], "", []))
             lg = r64["logits"]
             mx64, am64 = lg.max(1)
             am = captured["am"]
@@ -401,14 +298,14 @@ def _run_case(case):
             if n_wrong:
                 failures.append(f"step {step}: {n_wrong} rows whose pred_label is not an fp64 maximum")
         else:
-            note(step, "logits", _rho(captured["logits"], r64["logits"], S["logits"], "logits", zv), rl32)
-            note(step, "loss", _rho(loss_k, r64["loss"], S["loss"], "loss", zv),
-                 _rho(r32["loss"], r64["loss"], S["loss"], "", []))
-        note(step, "dcv", _rho(captured["dcv"], r64["taps"]["cv"][1], S["dcv"], "dcv", zv),
-             _rho(r32["dcv"], r64["taps"]["cv"][1], S["dcv"], "", []))
+            note(step, "logits", rho(captured["logits"], r64["logits"], S["logits"], "logits", zv), rl32)
+            note(step, "loss", rho(loss_k, r64["loss"], S["loss"], "loss", zv),
+                 rho(r32["loss"], r64["loss"], S["loss"], "", []))
+        note(step, "dcv", rho(captured["dcv"], r64["taps"]["cv"][1], S["dcv"], "dcv", zv),
+             rho(r32["dcv"], r64["taps"]["cv"][1], S["dcv"], "", []))
         for name in names:
-            note(step, name, _rho(g_k[name], r64["grads"][name], S[name], name, zv),
-                 _rho(r32["grads"][name], r64["grads"][name], S[name], "", []))
+            note(step, name, rho(g_k[name], r64["grads"][name], S[name], name, zv),
+                 rho(r32["grads"][name], r64["grads"][name], S[name], "", []))
         failures += [f"step {step} {v}" for v in zv]
         del r32, r64, S, mask, params, g_k
         snap.clear()

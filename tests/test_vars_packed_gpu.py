@@ -17,7 +17,7 @@ from gpu_util import random_params
 from philox_ref import dropout_mask
 from test_batch_builder_gpu import GV, _var_corpus
 from test_packed_gpu import DEV, DROPOUT, EVAL_TOL, _model, _padded_positions, _step
-from test_train_step_gpu import _reference, _rho, _scales
+from fp64_judge import reference as _reference, rho as _rho, scales as _scales
 from test_vars_packed_abi import unit_counts
 
 pytestmark = pytest.mark.gpu
