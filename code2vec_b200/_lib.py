@@ -153,6 +153,8 @@ SYMBOLS = {
                                                      c_vp, c_vp, c_vp, c_vp, c_i32, _P(c_i64)]),
     "c2v_session_wait": (ctypes.c_int, [c_vp, c_i64]),
     "c2v_launch_count": (c_i64, []),
+    "c2v_set_deterministic": (ctypes.c_int, [c_i32]),
+    "c2v_get_deterministic": (ctypes.c_int, []),
     "c2v_profile_enable": (ctypes.c_int, [c_i32]),
     "c2v_profile_read": (ctypes.c_int, [_P(ctypes.c_double), _P(c_i64)]),
     "c2v_corpus_parse_buffer": (ctypes.c_int, [ctypes.c_char_p, c_sz, c_i32, _P(c_vp)]),

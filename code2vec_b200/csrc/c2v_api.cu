@@ -52,8 +52,9 @@ int label_w_image(const c2v_dims *d, const float *Wout, int B, void *ws, size_t 
                   const uint8_t **img, const float **hdr, unsigned **scratch, const uint8_t **cv_img);
 int launch_label_backward_tc(const c2v_dims *d, const float *cv, const float *G, int B, const uint8_t *w_img,
                              const float *w_hdr, float *d_cv, float *d_w, float *d_b, unsigned *scratch, cudaStream_t st,
-                             bool absmax_ready, const uint8_t *cv_img);
+                             bool absmax_ready, const uint8_t *cv_img, float *dcv_slabs);
 size_t label_tcgen05_workspace_bytes(const c2v_dims *d, int B);
+void set_deterministic(bool on);
 bool label_ws_holds_dlogits_of(const void *ws, const float *cv, int B);
 
 // ---- profiling hook (c2v_profile_enable / c2v_profile_read) ----------------------------
@@ -183,6 +184,14 @@ using namespace c2v;
 extern "C" {
 
 int c2v_abi_version(void) { return C2V_ABI_VERSION; }
+
+int c2v_set_deterministic(int32_t on)
+{
+    set_deterministic(on != 0);
+    return C2V_OK;
+}
+
+int c2v_get_deterministic(void) { return deterministic() ? 1 : 0; }
 const char *c2v_last_error(void) { return g_err; }
 int64_t c2v_launch_count(void) { return __atomic_load_n(&g_launches, __ATOMIC_RELAXED); }
 
@@ -419,8 +428,10 @@ int c2v_workspace_set_status_mirror(void *workspace, int64_t *pinned_host_word, 
 size_t c2v_label_workspace_bytes(const c2v_dims *d, int32_t B)
 {
     if (!dims_ok(d) || B < 1) return 0;
-    // split fp16 images of cv and W_out for the tcgen05 label GEMM (unused by the FFMA path)
-    return align_up(label_tcgen05_workspace_bytes(d, B), 1024);
+    // split fp16 images of cv and W_out for the tcgen05 label GEMM (unused by the FFMA path); deterministic mode: then
+    // the label splits' d code_vector slabs of c2v_label_backward_ws
+    return align_up(label_tcgen05_workspace_bytes(d, B), 1024) +
+           (deterministic() ? align_up((size_t)kDetLabelSplits * B * d->encode * 4, 1024) : 0);
 }
 
 // What every tensor-core label entry point does once its own argument checks have passed: apply the flags of `algo`
@@ -621,7 +632,8 @@ int c2v_label_topk_supported(const c2v_dims *d, int32_t B, int32_t k)
 size_t c2v_label_topk_workspace_bytes(const c2v_dims *d, int32_t B, int32_t k)
 {
     if (!dims_ok(d) || B < 1 || k < 1 || k > C2V_TOPK_MAX || k > d->label_count) return 0;
-    return align_up(label_topk_workspace_bytes(d, B, k), 1024);
+    const size_t topk = align_up(label_topk_workspace_bytes(d, B, k), 1024), label = c2v_label_workspace_bytes(d, B);
+    return topk > label ? topk : label;       // (larger in deterministic mode only)
 }
 
 // argument checks shared by c2v_label_topk / c2v_angular_topk, all before any CUDA call
@@ -851,6 +863,10 @@ int c2v_loss_argmax(const float *outputs, const int64_t *label, int32_t B, int64
         set_error("c2v_loss_argmax: loss / d_outputs need label");
         return C2V_EINVAL;
     }
+    if (deterministic() && loss && (!argmax || !maxval)) {
+        set_error("c2v_loss_argmax: the deterministic loss needs argmax and maxval (its per-bag terms pass through maxval)");
+        return C2V_EINVAL;
+    }
     return launch_loss_argmax(outputs, reinterpret_cast<const long long *>(label), B, C, loss,
                               reinterpret_cast<long long *>(argmax), maxval, d_outputs,
                               static_cast<cudaStream_t>(stream));
@@ -908,8 +924,17 @@ int c2v_label_backward_ws(const c2v_dims *d, const c2v_params *p, const float *c
     // after c2v_label_dlogits on this workspace (the flag's contract: same code_vector, nothing in between) the workspace also
     // holds max |d_outputs| and the fp16 image of code_vector: the backward reads both instead of recomputing them
     const bool from_dlogits = (algo & C2V_FLAG_GRAD_ABSMAX_READY) != 0 && label_ws_holds_dlogits_of(workspace, code_vector, B);
+    float *dcv_slabs = nullptr;
+    if (deterministic() && d_code_vector) {
+        const size_t need = c2v_label_workspace_bytes(d, B);
+        if (workspace_bytes < need) {
+            set_error("c2v_label_backward_ws: workspace too small for the deterministic mode: %zu < %zu", workspace_bytes, need);
+            return C2V_EWORKSPACE;
+        }
+        dcv_slabs = reinterpret_cast<float *>(static_cast<char *>(workspace) + align_up(label_tcgen05_workspace_bytes(d, B), 1024));
+    }
     return launch_label_backward_tc(d, code_vector, d_outputs, B, img, hdr, d_code_vector, d_output_weight, d_output_bias,
-                                    scratch, st, from_dlogits, from_dlogits ? cv_img : nullptr);
+                                    scratch, st, from_dlogits, from_dlogits ? cv_img : nullptr, dcv_slabs);
 }
 
 size_t c2v_encode_backward_workspace_bytes(const c2v_dims *d, int32_t B, int32_t L)

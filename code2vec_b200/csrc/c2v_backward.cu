@@ -29,10 +29,13 @@ int launch_transpose_w(const float *W, float *Wt, int H, int D, int Hs, cudaStre
 bool backward_dw_tc_ok(const EncodeArgs &a);
 bool backward_dc_tc_ok(const EncodeArgs &a);
 size_t backward_dc_tc_workspace_bytes();
+// dc_rows / dw_slabs (deterministic mode, else NULL): dC rows stored to dc_rows [N, D] instead of scattered; dW from per-CTA
+// slabs added in CTA order
 int launch_backward_dc_tc(const EncodeArgs &a, const float *W, const float *dx, const unsigned *dx_absmax, void *ws,
                           float *g_emb_t, float *g_emb_p, cudaStream_t st, int sv_mask, bool build_image,
-                          const c2v_row_slots *slots);
-int launch_backward_dw_tc(const EncodeArgs &a, const float *dx, const unsigned *dx_absmax, float *dW, cudaStream_t st);
+                          const c2v_row_slots *slots, float *dc_rows);
+int launch_backward_dw_tc(const EncodeArgs &a, const float *dx, const unsigned *dx_absmax, float *dW, cudaStream_t st,
+                          float *dw_slabs);
 
 struct BackwardArgs {
     const float *cv, *att, *d_cv, *d_att, *sb;   // sb[b] = sum_j att[b,j] d_att[b,j] (or null)
@@ -42,6 +45,9 @@ struct BackwardArgs {
     const float *W;                              // [H, D] row-major (B operand of dC = dX . W)
     float *dx;                                   // [N, H]
     float *g_emb_t, *g_emb_p, *g_attn, *g_ln_g, *g_ln_b;
+    // deterministic mode (else NULL): dc_rows [N, D] receives every context's dC row (plain stores instead of the scatter),
+    // ln_part [gridDim.x][3][H] every CTA's d attention / d gamma / d beta (instead of one atomic per column per CTA)
+    float *dc_rows, *ln_part;
 };
 
 constexpr int MAXC = 8;   // columns per lane: encode_size <= 256
@@ -96,7 +102,8 @@ __device__ __forceinline__ void load_wrow_chunk(const float *__restrict__ W, int
 }
 
 // SPARSE: compact embedding gradients as in backward_dc_tc_kernel (slot maps in sl, a parameter behind the others)
-template <bool VEC, bool PACKED = false, bool SPARSE = false, bool SEED_DEV = false>
+// DET: deterministic mode (b.dc_rows / b.ln_part instead of atomics)
+template <bool VEC, bool PACKED = false, bool SPARSE = false, bool SEED_DEV = false, bool DET = false>
 __global__ void __launch_bounds__(THREADS)
 backward_rows_kernel(const EncodeArgs a, const BackwardArgs b, const int Hs, const c2v_row_slots sl)
 {
@@ -271,6 +278,11 @@ backward_rows_kernel(const EncodeArgs a, const BackwardArgs b, const int Hs, con
                     const int c = cb * NB + g * 64 + tx * 4;
                     if (c >= D) continue;
                     const float v0 = acc[i][g * 4], v1 = acc[i][g * 4 + 1], v2 = acc[i][g * 4 + 2], v3 = acc[i][g * 4 + 3];
+                    if constexpr (DET) {                             // the row, stored as it is
+                        const float vv[4] = {v0, v1, v2, v3};
+                        for (int q = 0; q < 4 && c + q < D; ++q) b.dc_rows[(size_t)(row0 + r) * D + c + q] = vv[q];
+                        continue;
+                    }
                     if (v0 == 0.0f && v1 == 0.0f && v2 == 0.0f && v3 == 0.0f) continue;   // padded contexts
                     if (VEC) {
                         float *dst;
@@ -314,6 +326,7 @@ backward_rows_kernel(const EncodeArgs a, const BackwardArgs b, const int Hs, con
         const int which = i / H, c = i % H;
         float s = 0.0f;
         for (int w = 0; w < 8; ++w) s += red[(which * 8 + w) * H + c];
+        if (DET) { b.ln_part[((size_t)blockIdx.x * 3 + which) * H + c] = s; continue; }
         float *dst = which == 0 ? b.g_attn : which == 1 ? b.g_ln_g : b.g_ln_b;
         if (s != 0.0f) atomicAdd(dst + c, s);
     }
@@ -326,7 +339,7 @@ backward_rows_kernel(const EncodeArgs a, const BackwardArgs b, const int Hs, con
 // in registers for the whole launch, one Philox block serves four columns, and padded contexts (attention weight
 // exactly 0) cost one zero store.  encode_size % 4 == 0, <= 256.
 // ------------------------------------------------------------------------------------
-template <int NG, bool PACKED = false, bool SEED_DEV = false> // 128-column groups: 1 (encode_size <= 128) or 2
+template <int NG, bool PACKED = false, bool SEED_DEV = false, bool DET = false> // 128-column groups: 1 (encode_size <= 128) or 2
 __global__ void __launch_bounds__(256, NG == 1 ? 4 : 2)
 backward_rows_lite_kernel(const EncodeArgs a, const BackwardArgs b)
 {
@@ -467,6 +480,7 @@ backward_rows_lite_kernel(const EncodeArgs a, const BackwardArgs b)
         if (c >= H) continue;
         float sum = 0.0f;
         for (int w = 0; w < 8; ++w) sum += red[((which * 8 + w) * MAXC + k) * 32 + l];
+        if (DET) { b.ln_part[((size_t)blockIdx.x * 3 + which) * H + c] = sum; continue; }
         float *dst = which == 0 ? b.g_attn : which == 1 ? b.g_ln_g : b.g_ln_b;
         if (sum != 0.0f) atomicAdd(dst + c, sum);
     }
@@ -475,7 +489,8 @@ backward_rows_lite_kernel(const EncodeArgs a, const BackwardArgs b)
 // dW[h][d] += sum over this CTA's rows of dx[row][h] * c[row][d]
 constexpr int DW_T = 64, DW_R = 16;
 __global__ void __launch_bounds__(256)
-backward_dw_kernel(const EncodeArgs a, const float *__restrict__ dx, float *__restrict__ dW, const long long rows_per_cta)
+backward_dw_kernel(const EncodeArgs a, const float *__restrict__ dx, float *__restrict__ dW, const long long rows_per_cta,
+                   float *__restrict__ slabs)
 {
     __shared__ float As[DW_R][DW_T + 4];
     __shared__ float Bs[DW_R][DW_T + 4];
@@ -534,13 +549,15 @@ backward_dw_kernel(const EncodeArgs a, const float *__restrict__ dx, float *__re
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             const int d = d0 + tx * 4 + j;
-            if (d < D && acc[i][j] != 0.0f) atomicAdd(dW + (size_t)h * D + d, acc[i][j]);
+            if (d >= D) continue;
+            if (slabs) slabs[((size_t)blockIdx.z * a.H + h) * D + d] = acc[i][j];     // deterministic mode: this split's slab
+            else if (acc[i][j] != 0.0f) atomicAdd(dW + (size_t)h * D + d, acc[i][j]);
         }
     }
 }
 
 // N context rows; a packed batch adds its row -> bag map (int32 [N]) at the end
-size_t encode_backward_workspace_bytes_n(const c2v_dims *d, int B, long long N, bool packed)
+static size_t backward_base_bytes(const c2v_dims *d, int B, long long N, bool packed)
 {
     const size_t H = d->encode, D = 2 * (size_t)d->terminal_embed + d->path_embed;
     const size_t Hs = (H + 3) / 4 * 4;
@@ -548,9 +565,57 @@ size_t encode_backward_workspace_bytes_n(const c2v_dims *d, int B, long long N, 
            align_up(backward_dc_tc_workspace_bytes(), 1024) + (packed ? align_up((size_t)N * 4, 1024) : 0);
 }
 
+// deterministic mode, behind the base layout: dC rows [N, D] | dW slabs [kDetSlabs][H][D] | d attention / gamma / beta
+// slabs [kDetRowSlabs][3][H] | the embedding reduction's keys and partials
+struct DetBackwardLayout {
+    size_t dc, dw, ln, emb, total;
+};
+static DetBackwardLayout det_backward_layout(const c2v_dims *d, long long N, size_t base)
+{
+    const size_t H = d->encode, D = 2 * (size_t)d->terminal_embed + d->path_embed;
+    const int E = d->terminal_embed > d->path_embed ? d->terminal_embed : d->path_embed;
+    DetBackwardLayout l;
+    size_t o = base;
+    l.dc = o; o += align_up((size_t)N * D * 4, 1024);
+    l.dw = o; o += align_up((size_t)kDetSlabs * H * D * 4, 1024);
+    l.ln = o; o += align_up((size_t)kDetRowSlabs * 3 * H * 4, 1024);
+    l.emb = o; o += align_up(det_embed_workspace_bytes(N, E), 1024);
+    l.total = o;
+    return l;
+}
+
+size_t encode_backward_workspace_bytes_n(const c2v_dims *d, int B, long long N, bool packed)
+{
+    const size_t base = backward_base_bytes(d, B, N, packed);
+    return deterministic() ? det_backward_layout(d, N, base).total : base;
+}
+
 size_t encode_backward_workspace_bytes(const c2v_dims *d, int B, int L)
 {
     return encode_backward_workspace_bytes_n(d, B, (long long)B * L, false);
+}
+
+// deterministic mode: the embedding gradients of the tables whose dC sub-vectors are in the dC rows buffer
+static int det_tables(const EncodeArgs &a, const float *att, const float *dc, const c2v_grads *g, const c2v_row_slots *slots,
+                      bool path, bool terminal, char *ws, const DetBackwardLayout &l, cudaStream_t st)
+{
+    const size_t emb_bytes = l.total - l.emb;
+    if (path) {
+        const int rc = launch_det_embed_grads(a, att, dc, true, g->path_embedding, slots ? slots->path : nullptr, ws + l.emb,
+                                              emb_bytes, st);
+        if (rc != C2V_OK) return rc;
+    }
+    if (terminal)
+        return launch_det_embed_grads(a, att, dc, false, g->terminal_embedding, slots ? slots->terminal : nullptr, ws + l.emb,
+                                      emb_bytes, st);
+    return C2V_OK;
+}
+
+// deterministic mode: d attention / d gamma / d beta = the sum of the n_slabs CTA slabs, in CTA order (overwritten)
+static int det_ln_grads(const float *ln_part, int n_slabs, int H, const c2v_grads *g, cudaStream_t st)
+{
+    float *const out[3] = {g->attention, g->ln_weight, g->ln_bias};
+    return launch_det_slab_sum3(ln_part, n_slabs, (size_t)3 * H, (size_t)H, 3, out, false, st);
 }
 
 int launch_encode_backward(const c2v_dims *d, const c2v_params *p, const EncodeArgs &a_in, int B,
@@ -563,15 +628,18 @@ int launch_encode_backward(const c2v_dims *d, const c2v_params *p, const EncodeA
     // dW gathers rows of BOTH embedding tables, so it must run before a caller may start updating path_embedding between
     // the phases; phase 2 reads only dx, the W^T image and the indices.  Only the tensor-core path with a stashed x
     // splits; every other path does everything in phase 1.
+    // Deterministic mode (c2v_set_deterministic) keeps the same kernels and phases; the dC kernels store rows that
+    // launch_det_embed_grads then sums per table row, and dW / d attention / d gamma / d beta come from per-CTA slabs.
     EncodeArgs a = a_in;
     if (a.H > 32 * MAXC) {
         set_error("encode backward supports encode_size <= %d (got %d)", 32 * MAXC, a.H);
         return C2V_EUNSUPPORTED;
     }
     const bool packed = a.bag_off != nullptr;
+    const bool det = deterministic();
     const size_t need = encode_backward_workspace_bytes_n(d, B, a.N, packed);
     if (ws_bytes < need) {
-        set_error("backward workspace too small: %zu < %zu", ws_bytes, need);
+        set_error("backward workspace too small: %zu < %zu%s", ws_bytes, need, det ? " (deterministic mode)" : "");
         return C2V_EWORKSPACE;
     }
     const int Hs = (a.H + 3) / 4 * 4;
@@ -583,6 +651,10 @@ int launch_encode_backward(const c2v_dims *d, const c2v_params *p, const EncodeA
     unsigned *dx_absmax = reinterpret_cast<unsigned *>(base + o); o += 1024;
     void *dc_ws = base + o; o += align_up(backward_dc_tc_workspace_bytes(), 1024);
     int *row_bag = packed ? reinterpret_cast<int *>(base + o) : nullptr;
+    const DetBackwardLayout dl = det_backward_layout(d, a.N, backward_base_bytes(d, B, a.N, packed));
+    float *dc_rows = det ? reinterpret_cast<float *>(base + dl.dc) : nullptr;
+    float *dw_slabs = det ? reinterpret_cast<float *>(base + dl.dw) : nullptr;
+    float *ln_part = det ? reinterpret_cast<float *>(base + dl.ln) : nullptr;
     {
         const char *dc_env0 = getenv("C2V_BACKWARD_DC"), *dw_env0 = getenv("C2V_BACKWARD_DW");
         const bool split_ok = x_stash && (a.H & 3) == 0 && backward_dc_tc_ok(a) && backward_dw_tc_ok(a) &&
@@ -590,8 +662,10 @@ int launch_encode_backward(const c2v_dims *d, const c2v_params *p, const EncodeA
         if (phase == 2) {
             if (!split_ok) return C2V_OK;                       // phase 1 already did everything
             a.n_tiles = (int)((a.N + TM - 1) / TM);
-            return launch_backward_dc_tc(a, p->input_linear, dx, dx_absmax, dc_ws, g->terminal_embedding, g->path_embedding, st,
-                                         5, false, slots);
+            const int rc = launch_backward_dc_tc(a, p->input_linear, dx, dx_absmax, dc_ws, g->terminal_embedding,
+                                                 g->path_embedding, st, 5, false, slots, dc_rows);
+            if (rc != C2V_OK || !det) return rc;
+            return det_tables(a, attention, dc_rows, g, slots, false, true, base, dl, st);
         }
         if (phase == 1 && !split_ok) phase = 0;
     }
@@ -617,6 +691,7 @@ int launch_encode_backward(const c2v_dims *d, const c2v_params *p, const EncodeA
     b.W = p->input_linear; b.dx = dx;
     b.g_emb_t = g->terminal_embedding; b.g_emb_p = g->path_embedding;
     b.g_attn = g->attention; b.g_ln_g = g->ln_weight; b.g_ln_b = g->ln_bias;
+    b.dc_rows = dc_rows; b.ln_part = ln_part;
     if (d_att && packed) {
         bag_dot_packed_kernel<<<B, 32, 0, st>>>(attention, d_att, a.bag_off, a.N, sb);
         C2V_LAUNCH_OK("bag_dot_packed_kernel");
@@ -626,10 +701,12 @@ int launch_encode_backward(const c2v_dims *d, const c2v_params *p, const EncodeA
         C2V_LAUNCH_OK("bag_dot_kernel");
         b.sb = sb;
     }
-    // the three small gradients are overwritten (header contract): zero, then accumulate
-    C2V_CUDA_OK(cudaMemsetAsync(g->attention, 0, (size_t)a.H * 4, st));
-    C2V_CUDA_OK(cudaMemsetAsync(g->ln_weight, 0, (size_t)a.H * 4, st));
-    C2V_CUDA_OK(cudaMemsetAsync(g->ln_bias, 0, (size_t)a.H * 4, st));
+    if (!det) {
+        // the three small gradients are overwritten (header contract): zero, then accumulate
+        C2V_CUDA_OK(cudaMemsetAsync(g->attention, 0, (size_t)a.H * 4, st));
+        C2V_CUDA_OK(cudaMemsetAsync(g->ln_weight, 0, (size_t)a.H * 4, st));
+        C2V_CUDA_OK(cudaMemsetAsync(g->ln_bias, 0, (size_t)a.H * 4, st));
+    }
 
     const FfmaSmem lay = ffma_smem_layout(Hs);
     int smem = lay.total;
@@ -643,28 +720,50 @@ int launch_encode_backward(const c2v_dims *d, const c2v_params *p, const EncodeA
     C2V_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     const bool dev_key = a.drop_p > 0.0f && a.seed_dev;       // C2V_DROPOUT_SEED_ON_DEVICE: the SEED_DEV instantiations
     if (x_stash && dc_tc && (a.H & 3) == 0) {                  // no GEMM left in this kernel: one warp per row
-        if (dev_key) {
-            if (a.H <= 128) (packed ? backward_rows_lite_kernel<1, true, true> : backward_rows_lite_kernel<1, false, true>)<<<sms * 16, 256, 0, st>>>(a, b);
-            else (packed ? backward_rows_lite_kernel<2, true, true> : backward_rows_lite_kernel<2, false, true>)<<<sms * 8, 256, 0, st>>>(a, b);
-        } else if (a.H <= 128) (packed ? backward_rows_lite_kernel<1, true> : backward_rows_lite_kernel<1>)<<<sms * 16, 256, 0, st>>>(a, b);
-        else (packed ? backward_rows_lite_kernel<2, true> : backward_rows_lite_kernel<2>)<<<sms * 8, 256, 0, st>>>(a, b);
+        int grid = a.H <= 128 ? sms * 16 : sms * 8;
+        if (det && grid > kDetRowSlabs) grid = kDetRowSlabs;
+        if (det) {
+            if (a.H <= 128)
+                (dev_key ? (packed ? backward_rows_lite_kernel<1, true, true, true> : backward_rows_lite_kernel<1, false, true, true>)
+                         : (packed ? backward_rows_lite_kernel<1, true, false, true> : backward_rows_lite_kernel<1, false, false, true>))
+                    <<<grid, 256, 0, st>>>(a, b);
+            else
+                (dev_key ? (packed ? backward_rows_lite_kernel<2, true, true, true> : backward_rows_lite_kernel<2, false, true, true>)
+                         : (packed ? backward_rows_lite_kernel<2, true, false, true> : backward_rows_lite_kernel<2, false, false, true>))
+                    <<<grid, 256, 0, st>>>(a, b);
+        } else if (dev_key) {
+            if (a.H <= 128) (packed ? backward_rows_lite_kernel<1, true, true> : backward_rows_lite_kernel<1, false, true>)<<<grid, 256, 0, st>>>(a, b);
+            else (packed ? backward_rows_lite_kernel<2, true, true> : backward_rows_lite_kernel<2, false, true>)<<<grid, 256, 0, st>>>(a, b);
+        } else if (a.H <= 128) (packed ? backward_rows_lite_kernel<1, true> : backward_rows_lite_kernel<1>)<<<grid, 256, 0, st>>>(a, b);
+        else (packed ? backward_rows_lite_kernel<2, true> : backward_rows_lite_kernel<2>)<<<grid, 256, 0, st>>>(a, b);
         C2V_LAUNCH_OK("backward_rows_lite_kernel");
+        if (det && (rc = det_ln_grads(ln_part, grid, a.H, g, st)) != C2V_OK) return rc;
         if (phase == 1) {                                       // path sub-vector + dW; start / end follow in phase 2
-            rc = launch_backward_dc_tc(a, p->input_linear, dx, dx_absmax, dc_ws, g->terminal_embedding, g->path_embedding, st, 2, true, slots);
+            rc = launch_backward_dc_tc(a, p->input_linear, dx, dx_absmax, dc_ws, g->terminal_embedding, g->path_embedding, st, 2, true,
+                                       slots, dc_rows);
             if (rc != C2V_OK) return rc;
-            return launch_backward_dw_tc(a, dx, dx_absmax, g->input_linear, st);
+            if (det && (rc = det_tables(a, attention, dc_rows, g, slots, true, false, base, dl, st)) != C2V_OK) return rc;
+            return launch_backward_dw_tc(a, dx, dx_absmax, g->input_linear, st, dw_slabs);
         }
-        rc = launch_backward_dc_tc(a, p->input_linear, dx, dx_absmax, dc_ws, g->terminal_embedding, g->path_embedding, st, 7, true, slots);
+        rc = launch_backward_dc_tc(a, p->input_linear, dx, dx_absmax, dc_ws, g->terminal_embedding, g->path_embedding, st, 7, true,
+                                   slots, dc_rows);
         if (rc != C2V_OK) return rc;
+        if (det && (rc = det_tables(a, attention, dc_rows, g, slots, true, true, base, dl, st)) != C2V_OK) return rc;
         const char *dw_env2 = getenv("C2V_BACKWARD_DW");
         if (backward_dw_tc_ok(a) && !(dw_env2 && !strcmp(dw_env2, "ffma")))
-            return launch_backward_dw_tc(a, dx, dx_absmax, g->input_linear, st);
+            return launch_backward_dw_tc(a, dx, dx_absmax, g->input_linear, st, dw_slabs);
         a.n_tiles = (int)((a.N + TM - 1) / TM);
         goto dw_ffma;
     }
     {
-    const bool sparse = !dc_tc && slots && (slots->terminal || slots->path);     // (with dc_tc K3c scatters)
-    auto kern = dev_key
+    // (with dc_tc K3c scatters; in deterministic mode nothing is scattered here)
+    const bool sparse = !dc_tc && !det && slots && (slots->terminal || slots->path);
+    auto kern = det
+        ? (dev_key ? (packed ? (vec ? backward_rows_kernel<true, true, false, true, true> : backward_rows_kernel<false, true, false, true, true>)
+                             : (vec ? backward_rows_kernel<true, false, false, true, true> : backward_rows_kernel<false, false, false, true, true>))
+                   : (packed ? (vec ? backward_rows_kernel<true, true, false, false, true> : backward_rows_kernel<false, true, false, false, true>)
+                             : (vec ? backward_rows_kernel<true, false, false, false, true> : backward_rows_kernel<false, false, false, false, true>)))
+        : dev_key
         ? (sparse ? (packed ? (vec ? backward_rows_kernel<true, true, true, true> : backward_rows_kernel<false, true, true, true>)
                             : (vec ? backward_rows_kernel<true, false, true, true> : backward_rows_kernel<false, false, true, true>))
                   : (packed ? (vec ? backward_rows_kernel<true, true, false, true> : backward_rows_kernel<false, true, false, true>)
@@ -680,28 +779,34 @@ int launch_encode_backward(const c2v_dims *d, const c2v_params *p, const EncodeA
     C2V_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, THREADS, smem));
     if (occ < 1) occ = 1;
     int grid = a.n_tiles < sms * occ ? a.n_tiles : sms * occ;
+    if (det && grid > kDetRowSlabs) grid = kDetRowSlabs;
     kern<<<grid, THREADS, smem, st>>>(a, b, Hs, sl);
     C2V_LAUNCH_OK("backward_rows_kernel");
+    if (det && (rc = det_ln_grads(ln_part, grid, a.H, g, st)) != C2V_OK) return rc;
     if (dc_tc) {
-        rc = launch_backward_dc_tc(a, p->input_linear, dx, dx_absmax, dc_ws, g->terminal_embedding, g->path_embedding, st, 7, true, slots);
+        rc = launch_backward_dc_tc(a, p->input_linear, dx, dx_absmax, dc_ws, g->terminal_embedding, g->path_embedding, st, 7, true,
+                                   slots, dc_rows);
         if (rc != C2V_OK) return rc;
     }
+    if (det && (rc = det_tables(a, attention, dc_rows, g, slots, true, true, base, dl, st)) != C2V_OK) return rc;
 
     // dW = dX^T . C: tensor cores when the shape allows (c2v_backward_dw_tc.cu), C2V_BACKWARD_DW=ffma forces the CUDA cores
     const char *dw_env = getenv("C2V_BACKWARD_DW");
     if (backward_dw_tc_ok(a) && !(dw_env && !strcmp(dw_env, "ffma")))
-        return launch_backward_dw_tc(a, dx, dx_absmax, g->input_linear, st);
+        return launch_backward_dw_tc(a, dx, dx_absmax, g->input_linear, st, dw_slabs);
     }
 dw_ffma:
     const int gx = (a.D + DW_T - 1) / DW_T, gy = (a.H + DW_T - 1) / DW_T;
     long long split = (8LL * sms) / (gx * gy);
     if (split < 1) split = 1;
+    if (det && split > kDetSlabs) split = kDetSlabs;
     long long rows_per = (a.N + split - 1) / split;
     rows_per = (rows_per + DW_R - 1) / DW_R * DW_R;
     if (rows_per < DW_R) rows_per = DW_R;
     const long long gz = (a.N + rows_per - 1) / rows_per;
-    backward_dw_kernel<<<dim3(gx, gy, (unsigned)gz), 256, 0, st>>>(a, dx, g->input_linear, rows_per);
+    backward_dw_kernel<<<dim3(gx, gy, (unsigned)gz), 256, 0, st>>>(a, dx, g->input_linear, rows_per, dw_slabs);
     C2V_LAUNCH_OK("backward_dw_kernel");
+    if (det) return launch_det_slab_sum(dw_slabs, (int)gz, (size_t)a.H * a.D, (size_t)a.H * a.D, g->input_linear, true, st);
     return C2V_OK;
 }
 

@@ -90,7 +90,9 @@ split_wt_kernel(const float *__restrict__ W, int H, int E, int n_hb, int n_db, c
 // SPARSE: a table whose slot map in sl is not NULL gets its gradient in compact form, row r of the table adding into row
 // sl.<table>[r] of the [U, E] buffer passed as its gradient (sparse embedding gradients, c2v_sparse_rows).  The slot maps
 // are a parameter of their own behind all the others, so that the dense instantiation keeps its parameter layout.
-template <bool SPARSE = false>
+// DET (deterministic mode): g_emb_t is the [N, 3E] dC rows buffer; every in-range row's dC is stored there as it is
+// (zeros included) and launch_det_embed_grads sums it into the tables.
+template <bool SPARSE = false, bool DET = false>
 __global__ void __launch_bounds__(dct::THREADS, 1)
 backward_dc_tc_kernel(const EncodeArgs a, const float *__restrict__ dx, const unsigned *__restrict__ dx_absmax,
                       const uint8_t *__restrict__ wt_img, const float *__restrict__ wt_hdr,
@@ -256,6 +258,20 @@ backward_dc_tc_kernel(const EncodeArgs a, const float *__restrict__ dx, const un
                 // acc[4j + 2h + b] is row[h], column 8j + 2 (lane & 3) + b of the window: a lane quad adds 32 contiguous
                 // bytes of one embedding row per instruction
                 float *tab = sv == 1 ? g_emb_p : g_emb_t;
+                if constexpr (DET) {
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        if (!in_range[h]) continue;
+                        float *dst = g_emb_t + (size_t)row[h] * (3 * a.Et) + sv * a.Et + db * dct::E;
+#pragma unroll
+                        for (int j = 0; j < 16; ++j) {
+                            const int c = 8 * j + 2 * m4;
+                            if (db * dct::E + c < a.Et)
+                                *reinterpret_cast<float2 *>(dst + c) = make_float2(acc[4 * j + 2 * h] * inv, acc[4 * j + 2 * h + 1] * inv);
+                        }
+                    }
+                    continue;
+                }
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
                     if (!in_range[h]) continue;
@@ -286,7 +302,7 @@ size_t backward_dc_tc_workspace_bytes() { return 1024 + 4 * dct::IMG_BYTES; }   
 // ws: [0, 1024) header {1/scale, scale} | W^T images [db][hb]
 int launch_backward_dc_tc(const EncodeArgs &a_in, const float *W, const float *dx, const unsigned *dx_absmax, void *ws,
                           float *g_emb_t, float *g_emb_p, cudaStream_t st, int sv_mask, bool build_image,
-                          const c2v_row_slots *slots)
+                          const c2v_row_slots *slots, float *dc_rows)
 {
     EncodeArgs a = a_in;
     a.n_tiles = (int)((a.N + dct::ROWS - 1) / dct::ROWS);
@@ -305,8 +321,9 @@ int launch_backward_dc_tc(const EncodeArgs &a_in, const float *W, const float *d
     int dev = 0, sms = 0;
     C2V_CUDA_OK(cudaGetDevice(&dev));
     C2V_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    const bool sparse = slots && (slots->terminal || slots->path);
-    auto kern = sparse ? backward_dc_tc_kernel<true> : backward_dc_tc_kernel<false>;
+    const bool sparse = !dc_rows && slots && (slots->terminal || slots->path);
+    auto kern = dc_rows ? backward_dc_tc_kernel<false, true> : sparse ? backward_dc_tc_kernel<true> : backward_dc_tc_kernel<false>;
+    if (dc_rows) g_emb_t = dc_rows;
     C2V_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, dct::SMEM_BYTES));
     int grid = sms / n_db;                                 // one CTA per SM over the d windows
     if (grid > a.n_tiles) grid = a.n_tiles;

@@ -40,6 +40,8 @@ constexpr int SMEM_A_OFF = 0, SMEM_B_OFF = 2 * A_STAGE, SMEM_BAR_OFF = SMEM_B_OF
 constexpr int SMEM_BYTES = SMEM_BAR_OFF + 128 + 1024;
 }  // namespace dwt
 
+// DET (deterministic mode): dW is the slab array [gridDim.x][H][3E]; CTA x stores its window of the partial to slab x
+template <bool DET = false>
 __global__ void __launch_bounds__(dwt::THREADS, 1)
 backward_dw_tc_kernel(const EncodeArgs a, const float *__restrict__ dx, const unsigned *__restrict__ dx_absmax,
                       float *__restrict__ dW, const int n_db)
@@ -216,7 +218,10 @@ backward_dw_tc_kernel(const EncodeArgs a, const float *__restrict__ dx, const un
 #pragma unroll
                     for (int j = 0; j < 8; ++j) {
                         const int d = db * 128 + 64 * kb + 8 * j + 2 * (lane & 3);
-                        if (h < a.H && d < E)                                                   // dW is [H][3E]
+                        if (DET && h < a.H && d < E)
+                            *reinterpret_cast<float2 *>(dW + ((size_t)blockIdx.x * a.H + h) * (3 * E) + sv * E + d) =
+                                make_float2(acc[kb][4 * j + 2 * hh] * inv, acc[kb][4 * j + 2 * hh + 1] * inv);
+                        else if (h < a.H && d < E)                                              // dW is [H][3E]
                             red_add_v2(dW + (size_t)h * (3 * E) + sv * E + d, acc[kb][4 * j + 2 * hh] * inv, acc[kb][4 * j + 2 * hh + 1] * inv);
                     }
                 }
@@ -229,20 +234,25 @@ bool backward_dw_tc_ok(const EncodeArgs &a) {
            (long long)a.T * a.Et * 4 < (1ll << 32) && (long long)a.P * a.Et * 4 < (1ll << 32);
 }
 
-int launch_backward_dw_tc(const EncodeArgs &a_in, const float *dx, const unsigned *dx_absmax, float *dW, cudaStream_t st)
+int launch_backward_dw_tc(const EncodeArgs &a_in, const float *dx, const unsigned *dx_absmax, float *dW, cudaStream_t st,
+                          float *dw_slabs)
 {
     EncodeArgs a = a_in;
     a.n_tiles = (int)((a.N + dwt::ROWS - 1) / dwt::ROWS);
     int dev = 0, sms = 0;
     C2V_CUDA_OK(cudaGetDevice(&dev));
     C2V_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    C2V_CUDA_OK(cudaFuncSetAttribute(backward_dw_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dwt::SMEM_BYTES));
+    auto kern = dw_slabs ? backward_dw_tc_kernel<true> : backward_dw_tc_kernel<false>;
+    C2V_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, dwt::SMEM_BYTES));
     const int n_hb = (a.H + dwt::H - 1) / dwt::H, n_db = (a.Et + dwt::E - 1) / dwt::E;
     int grid = sms / (3 * n_hb * n_db);                    // one CTA per SM over all windows
     if (grid > a.n_tiles) grid = a.n_tiles;
+    if (dw_slabs && grid > kDetSlabs) grid = kDetSlabs;
     if (grid < 1) grid = 1;
-    backward_dw_tc_kernel<<<dim3(grid, 3 * n_hb * n_db), dwt::THREADS, dwt::SMEM_BYTES, st>>>(a, dx, dx_absmax, dW, n_db);
+    kern<<<dim3(grid, 3 * n_hb * n_db), dwt::THREADS, dwt::SMEM_BYTES, st>>>(a, dx, dx_absmax, dw_slabs ? dw_slabs : dW, n_db);
     C2V_LAUNCH_OK("backward_dw_tc_kernel");
+    if (dw_slabs)          // every CTA of every window has at least one row tile (grid <= n_tiles): all slabs are written
+        return launch_det_slab_sum(dw_slabs, grid, (size_t)a.H * a.D, (size_t)a.H * a.D, dW, true, st);
     return C2V_OK;
 }
 

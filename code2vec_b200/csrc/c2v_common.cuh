@@ -148,6 +148,30 @@ __device__ __forceinline__ unsigned long long dropout_key(const EncodeArgs &a)
 #endif
 int launch_row_bag(const long long *bag_off, int B, long long N, int *row_bag, cudaStream_t st);
 
+// ---------------------------------------------------------------------------------
+// deterministic mode (c2v_set_deterministic, per host thread): every float sum of the training step runs in a fixed
+// order instead of through atomics (c2v_deterministic.cu)
+// ---------------------------------------------------------------------------------
+bool deterministic();
+constexpr int kDetSlabs = 64;          // per-CTA partial slabs of dW (tensor-core CTAs per window / CUDA-core row splits)
+constexpr int kDetRowSlabs = 512;      // per-CTA partials of d attention / d gamma / d beta (caps the row kernels' grids)
+constexpr int kDetLabelSplits = 32;    // label splits of d code_vector on the tensor cores
+// out[i] (+)= sum over s = 0 .. n_slabs-1, in that order, of src[s * slab_stride + i], i < n
+int launch_det_slab_sum(const float *src, int n_slabs, size_t slab_stride, size_t n, float *out, bool accumulate,
+                        cudaStream_t st);
+// the same over n_out * seg columns, column i going to out[i / seg][i % seg] (n_out <= 3), in one launch
+int launch_det_slab_sum3(const float *src, int n_slabs, size_t slab_stride, size_t seg, int n_out, float *const *out,
+                         bool accumulate, cudaStream_t st);
+// workspace of launch_det_embed_grads for N context rows (tables of up to `vocab` rows, rows up to E floats)
+size_t det_embed_workspace_bytes(long long N, int E);
+// Embedding-table gradient from the per-context rows dc [N, D] (D = 2 Et + Ep: start | path | end sub-vectors):
+// terminal (path = false) sums columns [0, Et) of row r into row starts[r] and [Et + Ep, D) into row ends[r], path sums
+// [Et, Et + Ep) into row paths[r]; contexts with attention exactly 0 are left out (their rows are 0).  Sorted keys
+// row << bits | entry, fixed-size chunks summed in key order, chunk partials of rows that span chunks summed in chunk
+// order; one write per row: grad[row] += sum, or grad[slot[row]] += sum with a slot map.
+int launch_det_embed_grads(const EncodeArgs &a, const float *att, const float *dc, bool path, float *grad, const int *slot,
+                           void *ws, size_t ws_bytes, cudaStream_t st);
+
 int launch_prepare_weights(const c2v_dims *d, const float *W, EncodeWorkspace &ws, bool tcgen05,
                            cudaStream_t st);
 int launch_encode_ffma(const EncodeArgs &a, cudaStream_t st);

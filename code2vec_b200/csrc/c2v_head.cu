@@ -78,7 +78,7 @@ int launch_sgemm(int M, int N, int K, const float *A, long long a_sm, long long 
     const int gx = (N + GT - 1) / GT, gy = (M + GT - 1) / GT;
     // few output tiles but a long reduction (d_cv = d_out . W_out: 32 tiles, K = label_count): split K
     int splits = 1;
-    if (gx * gy < 128 && K >= 1024) {
+    if (gx * gy < 128 && K >= 1024 && !deterministic()) {      // (split-K adds its partials with atomics)
         splits = 592 / (gx * gy);
         if (splits > K / 256) splits = K / 256;
         if (splits < 1) splits = 1;
@@ -207,10 +207,45 @@ angular_dcos_kernel(float *__restrict__ g, const float *__restrict__ cosv, const
         if (label[b] == c && co > 0.0f) dcos *= cos_m + sin_m * co / sqrtf(1.0f - co * co);
         g[i] = dcos * inv_cv[b] * inv_w[c];
         pc = dcos * co;
-        if (pc != 0.0f) atomicAdd(colsum + c, pc);
+        if (colsum && pc != 0.0f) atomicAdd(colsum + c, pc);
     }
+    if (!rowsum) return;                                   // deterministic mode: the sums come from angular_sums_kernel
     pc = warp_sum(pc);
     if ((threadIdx.x & 31) == 0 && pc != 0.0f) atomicAdd(rowsum + b, pc);
+}
+// deterministic mode: the same two correction sums of dcos * cos, before angular_dcos_kernel overwrites d_out, in a fixed
+// order.  Blocks [0, B): row b, 256 threads striding over the classes, then a fixed tree; blocks [B, B + ceil(C / 256)):
+// one column per thread, rows in order.
+__global__ void __launch_bounds__(256)
+angular_sums_kernel(const float *__restrict__ g, const float *__restrict__ cosv, const long long *__restrict__ label, int B,
+                    long long C, float cos_m, float sin_m, float inv_temp, float *__restrict__ rowsum, float *__restrict__ colsum)
+{
+    __shared__ float red[256];
+    auto term = [&](int b, long long c) {
+        const size_t i = (size_t)b * C + c;
+        const float co = cosv[i];
+        float dcos = g[i] * inv_temp;
+        if (label[b] == c && co > 0.0f) dcos *= cos_m + sin_m * co / sqrtf(1.0f - co * co);
+        return dcos * co;
+    };
+    if ((int)blockIdx.x < B) {
+        const int b = blockIdx.x;
+        float s = 0.0f;
+        for (long long c = threadIdx.x; c < C; c += 256) s += term(b, c);
+        red[threadIdx.x] = s;
+        __syncthreads();
+        for (int o = 128; o > 0; o >>= 1) {
+            if ((int)threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
+            __syncthreads();
+        }
+        if (threadIdx.x == 0) rowsum[b] = red[0];
+        return;
+    }
+    const long long c = (long long)(blockIdx.x - B) * 256 + threadIdx.x;
+    if (c >= C) return;
+    float s = 0.0f;
+    for (int b = 0; b < B; ++b) s += term(b, c);
+    colsum[c] = s;
 }
 __global__ void angular_fix_rows_kernel(float *__restrict__ d, const float *__restrict__ x, const float *__restrict__ inv,
                                         const float *__restrict__ sums, long long rows, int H)
@@ -228,9 +263,17 @@ int launch_angular_backward(const c2v_dims *d, const c2v_params *p, const float 
     const int H = d->encode;
     const long long C = d->label_count;
     float *rowsum = sums, *colsum = sums + B;
-    C2V_CUDA_OK(cudaMemsetAsync(sums, 0, (size_t)(B + C) * sizeof(float), st));
+    const bool det = deterministic();
+    if (det) {
+        angular_sums_kernel<<<(unsigned)(B + (C + 255) / 256), 256, 0, st>>>(d_out_inplace, cosine, label, B, C, cosf(margin),
+                                                                             sinf(margin), inverse_temp, rowsum, colsum);
+        C2V_LAUNCH_OK("angular_sums_kernel");
+    } else {
+        C2V_CUDA_OK(cudaMemsetAsync(sums, 0, (size_t)(B + C) * sizeof(float), st));
+    }
     angular_dcos_kernel<<<dim3((unsigned)((C + 255) / 256), (unsigned)B), 256, 0, st>>>(
-        d_out_inplace, cosine, inv_cv, inv_w, label, B, C, cosf(margin), sinf(margin), inverse_temp, rowsum, colsum);
+        d_out_inplace, cosine, inv_cv, inv_w, label, B, C, cosf(margin), sinf(margin), inverse_temp, det ? nullptr : rowsum,
+        det ? nullptr : colsum);
     C2V_LAUNCH_OK("angular_dcos_kernel");
     int rc = C2V_OK;
     if (d_cv) {
@@ -257,7 +300,7 @@ int launch_angular_backward(const c2v_dims *d, const c2v_params *p, const float 
 __global__ void __launch_bounds__(256)
 loss_argmax_kernel(const float *__restrict__ out, const long long *__restrict__ label, int B,
                    long long C, float *__restrict__ loss, long long *__restrict__ argmax,
-                   float *__restrict__ maxval, float *__restrict__ d_out)
+                   float *__restrict__ maxval, float *__restrict__ d_out, int det)
 {
     __shared__ float s_val[8];
     __shared__ long long s_idx[8];
@@ -294,7 +337,8 @@ loss_argmax_kernel(const float *__restrict__ out, const long long *__restrict__ 
     if (tid == 0) {
         if (argmax) argmax[b] = am;
         if (maxval) maxval[b] = mx;
-        if (loss && label) atomicAdd(loss, (mx + logf(s) - r[label[b]]) / (float)B);
+        if (loss && label && det) maxval[b] = (mx + logf(s) - r[label[b]]) / (float)B;   // loss_sum_kernel restores maxval
+        else if (loss && label) atomicAdd(loss, (mx + logf(s) - r[label[b]]) / (float)B);
     }
     if (d_out && label) {
         const float inv = 1.0f / s, invB = 1.0f / (float)B;
@@ -305,12 +349,39 @@ loss_argmax_kernel(const float *__restrict__ out, const long long *__restrict__ 
     }
 }
 
+// deterministic mode: maxval [B] holds the per-bag loss terms; one CTA sums them in a fixed order (strided per thread,
+// then a fixed tree) and puts the row maxima back (the logit at the arg-max, -inf for a row without one, as the scan has)
+__global__ void __launch_bounds__(256)
+loss_sum_kernel(const float *__restrict__ out, int B, long long C, const long long *__restrict__ argmax,
+                float *__restrict__ maxval, float *__restrict__ loss)
+{
+    __shared__ float red[256];
+    float s = 0.0f;
+    for (int b = threadIdx.x; b < B; b += 256) {
+        s += maxval[b];
+        const long long am = argmax[b];
+        maxval[b] = am >= 0 && am < C ? out[(size_t)b * C + am] : -INFINITY;
+    }
+    red[threadIdx.x] = s;
+    __syncthreads();
+    for (int o = 128; o > 0; o >>= 1) {
+        if ((int)threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) *loss = red[0];
+}
+
 int launch_loss_argmax(const float *out, const long long *label, int B, long long C, float *loss,
                        long long *argmax, float *maxval, float *d_out, cudaStream_t st)
 {
-    if (loss) C2V_CUDA_OK(cudaMemsetAsync(loss, 0, sizeof(float), st));
-    loss_argmax_kernel<<<B, 256, 0, st>>>(out, label, B, C, loss, argmax, maxval, d_out);
+    const bool det = deterministic() && loss && label;          // (the entry point checked argmax / maxval)
+    if (loss && !det) C2V_CUDA_OK(cudaMemsetAsync(loss, 0, sizeof(float), st));
+    loss_argmax_kernel<<<B, 256, 0, st>>>(out, label, B, C, loss, argmax, maxval, d_out, det ? 1 : 0);
     C2V_LAUNCH_OK("loss_argmax_kernel");
+    if (det) {
+        loss_sum_kernel<<<1, 256, 0, st>>>(out, B, C, argmax, maxval, loss);
+        C2V_LAUNCH_OK("loss_sum_kernel");
+    }
     return C2V_OK;
 }
 

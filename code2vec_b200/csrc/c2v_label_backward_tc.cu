@@ -284,7 +284,8 @@ constexpr int SMEM_A_OFF = 0;
 static inline int lb2_stages(int nkb) { return nkb <= 2 ? 3 : 2; }
 static inline int lb2_smem_bytes(int nkb) { return lb2_stages(nkb) * (lb2::A_STAGE + nkb * 2 * lb2::B_HALF) + 128 + 1024; }
 
-template <int NKB>
+// DET (deterministic mode): d_cv is the slab array [n_split][B][H]; label split sp stores its partial to slab sp
+template <int NKB, bool DET = false>
 __global__ void __launch_bounds__(lbt::THREADS, 1)
 label_dcv_tc_kernel(const float *__restrict__ G, int B, long long C, int H, const uint8_t *__restrict__ w_img,
                     const float *__restrict__ w_hdr, const unsigned *__restrict__ g_absmax, int n_split,
@@ -431,12 +432,15 @@ label_dcv_tc_kernel(const float *__restrict__ G, int B, long long C, int H, cons
                     const int b = bt * 128 + 64 * g + 16 * w4 + (lane >> 2) + 8 * hh;
                     if (b >= B) continue;
                     float *dst = d_cv + (size_t)b * H;
+                    if (DET) dst += (size_t)(kb0 / kblocks_per_split) * B * H;
 #pragma unroll
                     for (int kb = 0; kb < NKB; ++kb)
 #pragma unroll
                         for (int j = 0; j < 8; ++j) {
                             const int h = 64 * kb + 8 * j + 2 * m4;
-                            if (h < H) red_add_v2(dst + h, acc[kb][4 * j + 2 * hh] * inv, acc[kb][4 * j + 2 * hh + 1] * inv);
+                            if (DET && h < H)
+                                *reinterpret_cast<float2 *>(dst + h) = make_float2(acc[kb][4 * j + 2 * hh] * inv, acc[kb][4 * j + 2 * hh + 1] * inv);
+                            else if (h < H) red_add_v2(dst + h, acc[kb][4 * j + 2 * hh] * inv, acc[kb][4 * j + 2 * hh + 1] * inv);
                         }
                 }
             }
@@ -452,7 +456,7 @@ bool label_backward_tc_ok(const c2v_dims *d)
 // scratch: 256 B (word 0: bits of max |G|).  w_img / w_hdr: the label workspace's cached W_out image and header (valid).
 int launch_label_backward_tc(const c2v_dims *d, const float *cv, const float *G, int B, const uint8_t *w_img,
                              const float *w_hdr, float *d_cv, float *d_w, float *d_b, unsigned *scratch, cudaStream_t st,
-                             bool absmax_ready, const uint8_t *cv_img)
+                             bool absmax_ready, const uint8_t *cv_img, float *dcv_slabs)
 {
     const int H = d->encode, nkb = (H + 63) / 64;
     const long long C = d->label_count;
@@ -478,23 +482,29 @@ int launch_label_backward_tc(const c2v_dims *d, const float *cv, const float *G,
         C2V_LAUNCH_OK("label_dw_tc_kernel");
     }
     if (d_cv) {
-        C2V_CUDA_OK(cudaMemsetAsync(d_cv, 0, (size_t)B * H * sizeof(float), st));
+        if (!dcv_slabs) C2V_CUDA_OK(cudaMemsetAsync(d_cv, 0, (size_t)B * H * sizeof(float), st));
         const int smem = lb2_smem_bytes(nkb);
         void (*kern)(const float *, int, long long, int, const uint8_t *, const float *, const unsigned *, int, long long, float *,
-                     int) = nkb == 1 ? label_dcv_tc_kernel<1> : nkb == 2 ? label_dcv_tc_kernel<2>
-                          : nkb == 3 ? label_dcv_tc_kernel<3> : label_dcv_tc_kernel<4>;
+                     int) = dcv_slabs ? (nkb == 1 ? label_dcv_tc_kernel<1, true> : nkb == 2 ? label_dcv_tc_kernel<2, true>
+                                         : nkb == 3 ? label_dcv_tc_kernel<3, true> : label_dcv_tc_kernel<4, true>)
+                                      : (nkb == 1 ? label_dcv_tc_kernel<1> : nkb == 2 ? label_dcv_tc_kernel<2>
+                                         : nkb == 3 ? label_dcv_tc_kernel<3> : label_dcv_tc_kernel<4>);
         C2V_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
         const int n_bt = (B + 127) / 128;
         const long long n_kblocks = (C + 63) / 64;
         long long n_split = (2LL * sms + n_bt - 1) / n_bt;            // ~2 items per SM
         if (n_split > n_kblocks) n_split = n_kblocks;
+        if (dcv_slabs && n_split > kDetLabelSplits) n_split = kDetLabelSplits;
         if (n_split < 1) n_split = 1;
         const long long per = (n_kblocks + n_split - 1) / n_split;
         n_split = (n_kblocks + per - 1) / per;
         const long long n_items = (long long)n_bt * n_split;
         const int grid = (int)(n_items < sms ? n_items : sms);
-        kern<<<grid, lbt::THREADS, smem, st>>>(G, B, C, H, w_img, w_hdr, scratch, (int)n_split, per, d_cv, lb2_stages(nkb));
+        kern<<<grid, lbt::THREADS, smem, st>>>(G, B, C, H, w_img, w_hdr, scratch, (int)n_split, per, dcv_slabs ? dcv_slabs : d_cv,
+                                               lb2_stages(nkb));
         C2V_LAUNCH_OK("label_dcv_tc_kernel");
+        if (dcv_slabs)     // every split owns at least one label block: all n_split slabs are written
+            return launch_det_slab_sum(dcv_slabs, (int)n_split, (size_t)B * H, (size_t)B * H, d_cv, false, st);
     }
     return C2V_OK;
 }

@@ -12,6 +12,8 @@ the minimum: bags are independent, so the forward shards with no collective; onl
 torch.distributed is only plumbing here (process group, the collective); launch one process per GPU with
 `python -m torch.distributed.run --nproc-per-node N --master-addr 127.0.0.1 ...`.
 """
+import warnings
+
 import torch
 import torch.distributed as dist
 
@@ -162,6 +164,22 @@ def sharded_layout(n_early, numel, world, rank):
     return regions, slices, o
 
 
+def nvls_allowed(transport, world):
+    """Whether ShardedFlatAdam's transport="auto" may pick "nvls" for a group of `world` ranks.  Under
+    torch.use_deterministic_algorithms(True) at world size > 1 it may not: the in-switch reduction (multimem.ld_reduce)
+    has no documented summation order.  An explicit "nvls" then raises RuntimeError, or warns (UserWarning) with
+    warn_only=True and stays.  "p2p" sums the ranks in a fixed order and "nccl" is left to NCCL: both are unchanged."""
+    if world <= 1 or not torch.are_deterministic_algorithms_enabled():
+        return True
+    if transport == "nvls":
+        msg = ('ShardedFlatAdam: transport "nvls" reduces the gradients in the NVSwitch in no documented order, so it is '
+               'not deterministic; torch.use_deterministic_algorithms(True) is set: use transport="p2p" (or "auto")')
+        if not torch.is_deterministic_algorithms_warn_only_enabled():
+            raise RuntimeError(msg)
+        warnings.warn(msg, UserWarning)
+    return False
+
+
 class ShardedFlatAdam:
     """Data-parallel Adam with the optimizer state sharded over the ranks and the gradient reduction fused into the
     optimizer kernel.  Same update rule, dense, as
@@ -212,6 +230,7 @@ class ShardedFlatAdam:
         self.regions, self.slices, self.state_numel = sharded_layout(n_early, self.numel, self.world, self.rank)
         self.padded = sum(n for _, n in self.regions)
         self._auto = transport == "auto"
+        self._auto_nvls = nvls_allowed(transport, self.world)
         self.transport, self._hdl = self._allocate(transport, dev)
         self._grad_views = ([], [])
         self.flat_param.zero_()
@@ -288,7 +307,7 @@ class ShardedFlatAdam:
                 mc = all(int(h.multicast_ptr) != 0 for h in hdls)
                 if want == "nvls" and not mc:
                     raise RuntimeError("this process group has no NVSwitch multicast support")
-                return ("nvls" if (mc and want != "p2p") else "p2p"), hdls
+                return ("nvls" if (mc and (want == "nvls" or (want == "auto" and self._auto_nvls))) else "p2p"), hdls
             except Exception:
                 if want in ("nvls", "p2p"):
                     raise
@@ -406,6 +425,8 @@ class ShardedFlatAdam:
         """reduce this step's gradients over the ranks (mean), Adam, parameters identical everywhere afterwards; the
         other bucket is left zeroed and becomes the target of the next backward (main.py:171 + :175)."""
         _check_capturable(self.capturable, "ShardedFlatAdam")
+        if self.transport == "nvls":             # the switch may have been turned on after the construction chose "nvls"
+            nvls_allowed("nvls", self.world)
         cur, nxt = self.cur, 1 - self.cur
         if not self._early_done and not self.capturable:
             self.t += 1

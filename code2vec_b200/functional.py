@@ -2,6 +2,7 @@
 All arithmetic happens inside libc2v_b200.so."""
 import ctypes
 import os
+import threading
 
 import torch
 
@@ -21,6 +22,21 @@ def _empty(shape, dtype, device):
         if t.numel():
             t.reshape(-1).view(torch.uint8).fill_(255)
     return t
+
+
+_det = threading.local()
+
+
+def sync_deterministic():
+    """Set the library's deterministic mode (c2v_set_deterministic) of the calling thread from
+    torch.are_deterministic_algorithms_enabled(); the library is called only when the value changed.  The mode is per host
+    thread and autograd runs backwards on threads of its own, so every training-path wrapper calls this before it sizes a
+    workspace.  Returns the mode."""
+    on = torch.are_deterministic_algorithms_enabled()
+    if getattr(_det, "on", False) != on:
+        _lib.load().c2v_set_deterministic(1 if on else 0)
+        _det.on = on
+    return on
 
 
 def _ptr(t):
@@ -311,6 +327,7 @@ def _label_ws(dims, B, dev, algo, cache, weight, nbytes=None, absmax_ready=False
     """-> (workspace, algo with its flags) of a label-head call.  With a cache (and its weight, W_out) the cache's persistent
     workspace, plus REUSE_PREP while its W_out image is current and GRAD_ABSMAX_READY if absmax_ready.  Without one a fresh
     workspace, or None if not fresh (the backward calls then run on the CUDA cores)."""
+    sync_deterministic()
     if nbytes is None:
         nbytes = _lib.load().c2v_label_workspace_bytes(ctypes.byref(dims), B)
     algo = capture_flags(algo)
@@ -441,6 +458,7 @@ def _topk(fn, dims, params, cv, k, want_probs, algo, cache, weight, *head_args):
         prob = _empty((B, k), torch.float32, dev) if want_probs else None
         ws = None                    # a call the library will refuse must not mark the cache's weight image as current
         if (int(algo) & 0xff) != _lib.ALGO_FFMA and label_topk_supported(dims, B, k):
+            sync_deterministic()                 # (the size depends on the mode)
             nbytes = lib.c2v_label_topk_workspace_bytes(ctypes.byref(dims), B, k)
             ws, algo = _label_ws(dims, B, dev, algo, cache, weight, nbytes=nbytes)
         cv = _f32c(cv, "code_vector")
@@ -539,6 +557,7 @@ def angular_forward_train(dims, params, cv, label, margin, inverse_temp):
 def angular_backward(dims, params, cv, label, margin, inverse_temp, cos, inv, d_out, need_cv=True, need_w=True):
     """-> (d_code_vector, d_output_weight); d_out is consumed (overwritten)"""
     lib = _lib.load()
+    sync_deterministic()
     B = cv.shape[0]
     dev = cv.device
     with torch.cuda.device(dev):
@@ -557,6 +576,7 @@ def angular_backward(dims, params, cv, label, margin, inverse_temp, cos, inv, d_
 def loss_argmax(outputs, label=None, want_grad=False):
     """main.py:251-264 + main.py:285 -> (loss 0-d or None, argmax [B], maxval [B], d_outputs or None)"""
     lib = _lib.load()
+    sync_deterministic()
     _need_cuda(outputs)
     B, C = outputs.shape
     dev = outputs.device
@@ -611,6 +631,7 @@ def encode_backward(dims, params, starts, paths, ends, cv, att, d_cv, d_att, sha
     for this batch, None for a dense table; grads_out then holds the zero-filled compact [U, E] buffer of every table
     with a slot map (c2v_encode_backward_sparse)."""
     lib = _lib.load()
+    sync_deterministic()
     B, L = starts.shape
     dev = starts.device
     with torch.cuda.device(dev):
@@ -644,6 +665,7 @@ def encode_backward_packed(dims, params, bags, cv, att, d_cv, d_att, shapes, dro
                            grads_out=None, x_stash=None, between_phases=None, slots=None):
     """encode_backward for a PackedBags batch: att / d_att [N], x_stash [N, H] from encode_forward_packed(stash=True)."""
     lib = _lib.load()
+    sync_deterministic()
     B, N, L = bags.B, bags.N, bags.L
     dev = bags.device
     with torch.cuda.device(dev):

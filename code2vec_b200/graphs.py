@@ -49,7 +49,8 @@ class _Graphed:
             return self._run(*inputs)                    # e.g. the ragged last batch of an epoch: eagerly
         if self.graph is not None:
             if self._settings() != self._frozen:
-                raise RuntimeError(f"{type(self).__name__}: hyper-parameters or model.training changed since the capture "
+                raise RuntimeError(f"{type(self).__name__}: hyper-parameters, model.training or "
+                                   "torch.are_deterministic_algorithms_enabled() changed since the capture "
                                    f"({self._frozen} -> {self._settings()}); build a new {type(self).__name__}")
             for s, t in zip(self.static_in, inputs):
                 s.copy_(t, non_blocking=True)
@@ -106,7 +107,8 @@ class GraphedTrainStep(_Graphed):
         else:
             hyper = tuple(tuple((k, v) for k, v in sorted(g.items()) if k != "params" and not isinstance(v, torch.Tensor))
                           for g in o.param_groups)
-        return (self.model.training, hyper)
+        # the deterministic mode selects other kernels and workspace sizes than the captured ones
+        return (self.model.training, torch.are_deterministic_algorithms_enabled(), hyper)
 
     def _run(self, starts, paths, ends, label):
         model, opt = self.model, self.optimizer

@@ -217,6 +217,25 @@ class _LabelLossFn(torch.autograd.Function):
         return d_cv, d_w, d_b, None, None, None, None, None
 
 
+class _LossArgmaxFn(torch.autograd.Function):
+    """mean NLL of log_softmax + torch.max over materialised logits [B, C] (main.py:251-264, main.py:285) in one library
+    call (c2v_loss_argmax), whose d loss / d logits comes out of the same pass.  forward_loss's fallback takes it under
+    torch.use_deterministic_algorithms: the library sums the loss in a fixed order there, and torch's NLLLoss on CUDA has no
+    deterministic implementation."""
+
+    @staticmethod
+    def forward(ctx, outputs, label):
+        loss, am, mx, d_out = CF.loss_argmax(outputs.detach(), label, want_grad=True)
+        ctx.save_for_backward(d_out)
+        ctx.mark_non_differentiable(am, mx)
+        return loss, am, mx
+
+    @staticmethod
+    def backward(ctx, d_loss, _d_am, _d_mx):
+        d_out, = ctx.saved_tensors
+        return d_out * d_loss, None
+
+
 class Code2Vec(nn.Module):
     """the code2vec model (H100-native drop-in for model.py:15-105)"""
 
@@ -410,13 +429,15 @@ class Code2Vec(nn.Module):
         1) and is autograd-connected; the [b, C] logits are never written.  Both label heads: with
         option.angular_margin_loss the loss, arg-max and max are those of the angular-margin logits (model.py:71-80).
         Shapes the fused kernel does not take, and algo="ffma", fall back to forward()'s head + eager log_softmax / NLL +
-        torch.max."""
+        torch.max; under torch.use_deterministic_algorithms(True) to forward()'s head + c2v_loss_argmax."""
         code_vector, attention, dims = self._encode(starts, paths, ends)
         if self.algo != _lib.ALGO_FFMA and CF.label_loss_supported(dims, code_vector.shape[0]):
             o = self.option
             angular = (o.angular_margin, o.inverse_temp) if o.angular_margin_loss else None
             loss, am, mx = _LabelLossFn.apply(code_vector, *self._head(), label, dims, self._label_algo, self._lab_cache,
                                               angular)
+        elif torch.are_deterministic_algorithms_enabled():
+            loss, am, mx = _LossArgmaxFn.apply(self._head_logits(code_vector, label, dims), label)
         else:
             loss, am, mx = self._eager_loss(self._head_logits(code_vector, label, dims), label)
         return loss, am, mx, code_vector, attention

@@ -134,6 +134,26 @@ int c2v_next_dropout_key(int64_t *rng_state, uint64_t *key_out, void *stream);
 int c2v_abi_version(void);
 const char *c2v_last_error(void);
 
+/* Deterministic mode, per host thread like c2v_last_error (off by default): while it is on, the calls of a single-GPU
+ * training step give bit-identical results on repeated runs with the same inputs, shapes, library build and GPU model
+ * (what torch.use_deterministic_algorithms promises; not across GPU models or batch shapes).  Every float sum that is
+ * otherwise accumulated with atomics runs in a fixed order instead:
+ *   c2v_encode_backward* (all layouts, dense and sparse): the dC kernels store each context's dC row [N, 2E_t + E_p] to
+ *     the workspace, and a sort of (table row, context) keys plus a chunked segmented sum writes each embedding row once
+ *     (grad[row] += sum, so accumulation into existing gradients still works); dW, d attention, d gamma and d beta come
+ *     from per-CTA partials added in CTA order.  The phases keep their contract.
+ *   c2v_label_backward_ws (tensor cores): d_code_vector from per-split partials added in split order.
+ *   c2v_label_backward, c2v_label_logits* and c2v_angular_* on the CUDA cores: no split-K; c2v_angular_backward's row
+ *     and column sums in a fixed order.
+ *   c2v_loss_argmax: per-bag loss terms and an ordered sum (argmax and maxval must then be given when loss is).
+ * The other calls are deterministic either way.  While it is on, c2v_encode_backward_workspace_bytes,
+ * c2v_encode_backward_packed_workspace_bytes, c2v_label_workspace_bytes and c2v_label_topk_workspace_bytes return the
+ * larger sizes this mode needs (the dC rows alone are N (2E_t + E_p) * 4 bytes), and the calls check for them.  With it
+ * off nothing changes: same kernels, launches, workspace sizes and results.  Nothing is read on the host, so every call
+ * stays capturable into a CUDA graph. */
+int c2v_set_deterministic(int32_t on);
+int c2v_get_deterministic(void);
+
 /* Device facts the host side sizes grids with. */
 typedef struct c2v_device_info {
     int32_t cc_major, cc_minor, sm_count, reserved;
