@@ -44,6 +44,16 @@ class RowSlots(ctypes.Structure):
     _fields_ = [("terminal", c_vp), ("path", c_vp)]
 
 
+REDUCTION_MEAN, REDUCTION_SUM, REDUCTION_NONE = 0, 1, 2      # C2V_REDUCTION_*
+REDUCTIONS = {"mean": REDUCTION_MEAN, "sum": REDUCTION_SUM, "none": REDUCTION_NONE}
+
+
+class LossOptions(ctypes.Structure):
+    """c2v_loss_options: the criterion of the fused loss (include/c2v_b200.h)"""
+    _fields_ = [("class_weight", c_vp), ("ignore_index", c_i64), ("label_smoothing", c_f32), ("reduction", c_i32),
+                ("row_grad", c_vp)]
+
+
 class DeviceInfo(ctypes.Structure):
     _fields_ = [("cc_major", c_i32), ("cc_minor", c_i32), ("sm_count", c_i32), ("reserved", c_i32),
                 ("global_mem_bytes", c_i64), ("smem_per_block_optin", c_i64)]
@@ -94,6 +104,15 @@ SYMBOLS = {
                                                c_vp, c_vp, c_vp, c_sz, c_i32, c_vp]),
     "c2v_angular_dlogits": (ctypes.c_int, [_P(Dims), _P(Params), c_vp, c_vp, c_vp, c_vp, c_i32, c_f32, c_f32, c_f32, c_vp, c_vp,
                                            c_vp, c_sz, c_i32, c_vp]),
+    "c2v_label_loss_opts_workspace_bytes": (c_sz, [_P(Dims), c_i32]),
+    "c2v_label_loss_argmax_opts": (ctypes.c_int, [_P(Dims), _P(Params), c_vp, c_vp, c_i32, _P(LossOptions), c_vp, c_vp, c_vp,
+                                                  c_vp, c_vp, c_vp, c_vp, c_sz, c_i32, c_vp]),
+    "c2v_label_dlogits_opts": (ctypes.c_int, [_P(Dims), _P(Params), c_vp, c_vp, c_vp, c_vp, c_i32, _P(LossOptions), c_f32, c_vp,
+                                              c_vp, c_vp, c_sz, c_i32, c_vp]),
+    "c2v_angular_loss_argmax_opts": (ctypes.c_int, [_P(Dims), _P(Params), c_vp, c_vp, c_i32, c_f32, c_f32, _P(LossOptions),
+                                                    c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_sz, c_i32, c_vp]),
+    "c2v_angular_dlogits_opts": (ctypes.c_int, [_P(Dims), _P(Params), c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_f32, c_f32,
+                                                _P(LossOptions), c_f32, c_vp, c_vp, c_vp, c_sz, c_i32, c_vp]),
     "c2v_angular_backward_ws": (ctypes.c_int, [_P(Dims), _P(Params), c_vp, c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_sz, c_i32,
                                                c_vp]),
     "c2v_angular_logits": (ctypes.c_int, [_P(Dims), _P(Params), c_vp, c_vp, c_i32, c_f32, c_f32, c_vp, c_vp]),
@@ -122,6 +141,7 @@ SYMBOLS = {
     "c2v_adam_step_sharded_bulk": (ctypes.c_int, [c_vp, _P(c_vp), _P(c_vp), c_i32, c_vp, c_vp, c_i64, c_i64, c_f32, c_f32, c_f32,
                                                   c_f32, c_f32, c_i64, c_f32, c_i32, c_vp]),
     "c2v_loss_argmax": (ctypes.c_int, [c_vp, c_vp, c_i32, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "c2v_loss_argmax_opts": (ctypes.c_int, [c_vp, c_vp, c_i32, c_i64, _P(LossOptions), c_vp, c_vp, c_vp, c_vp, c_vp]),
     "c2v_label_backward": (ctypes.c_int, [_P(Dims), _P(Params), c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp]),
     "c2v_label_backward_ws": (ctypes.c_int, [_P(Dims), _P(Params), c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_sz, c_i32, c_vp]),
     "c2v_encode_backward_workspace_bytes": (c_sz, [_P(Dims), c_i32, c_i32]),

@@ -37,6 +37,8 @@ int launch_angular_backward(const c2v_dims *d, const c2v_params *p, const float 
                             float *d_out_inplace, float *d_cv, float *d_w, float *sums, cudaStream_t st);
 int launch_loss_argmax(const float *out, const long long *label, int B, long long C, float *loss,
                        long long *argmax, float *maxval, float *d_out, cudaStream_t st);
+int launch_loss_argmax_opts(const float *out, const long long *label, int B, long long C, const LossOptArgs &o, float *loss,
+                            long long *argmax, float *maxval, float *d_out, cudaStream_t st);
 int launch_row_inv_norm(const float *X, long long rows, int H, float *inv, cudaStream_t st);
 int launch_angular_project(float *d, const float *x, const float *inv, long long rows, int H, cudaStream_t st);
 int launch_colsum(const float *X, int B, long long C, float *out, cudaStream_t st);
@@ -585,6 +587,168 @@ int c2v_angular_dlogits(const c2v_dims *d, const c2v_params *p, const float *cod
                       &la);
 }
 
+// ---- criterion options (c2v_loss_options) ------------------------------------------------------------------------------
+// o != NULL -> *out; every check before any CUDA call.  dlogits: the call that needs row_grad for reduction none.
+static int loss_opts_ok(const char *fn, const c2v_loss_options *o, bool dlogits, LossOptArgs *out)
+{
+    if (!(o->label_smoothing >= 0.0f && o->label_smoothing <= 1.0f)) {          // (false for NaN)
+        set_error("%s: label_smoothing %g is not in [0, 1]", fn, (double)o->label_smoothing);
+        return C2V_EINVAL;
+    }
+    if (o->reduction != C2V_REDUCTION_MEAN && o->reduction != C2V_REDUCTION_SUM && o->reduction != C2V_REDUCTION_NONE) {
+        set_error("%s: unknown reduction %d", fn, o->reduction);
+        return C2V_EINVAL;
+    }
+    if ((uintptr_t)o->class_weight % alignof(float) != 0) {
+        set_error("%s: class_weight is not 4-byte aligned", fn);
+        return C2V_EINVAL;
+    }
+    if (dlogits && o->reduction == C2V_REDUCTION_NONE && !o->row_grad) {
+        set_error("%s: reduction none needs row_grad", fn);
+        return C2V_EINVAL;
+    }
+    *out = LossOptArgs{};
+    out->weight = o->class_weight; out->ignore_index = o->ignore_index; out->eps = o->label_smoothing;
+    out->reduction = o->reduction; out->row_grad = dlogits ? o->row_grad : nullptr;
+    return C2V_OK;
+}
+
+size_t c2v_label_loss_opts_workspace_bytes(const c2v_dims *d, int32_t B)
+{
+    if (!dims_ok(d) || B < 1) return 0;
+    return align_up(c2v_label_workspace_bytes(d, B), 1024) + label_loss_opts_bytes(d, B);
+}
+
+// the checks every fused loss call with options adds to those of the call it extends
+static int loss_opts_call_ok(const char *fn, const c2v_dims *d, int32_t B, const c2v_loss_options *options, float *coef,
+                             void *workspace, size_t workspace_bytes, LossOptArgs *oa)
+{
+    int rc = loss_opts_ok(fn, options, false, oa);
+    if (rc != C2V_OK) return rc;
+    if (!coef) { set_error("%s: coef is NULL", fn); return C2V_EINVAL; }
+    const size_t need = c2v_label_loss_opts_workspace_bytes(d, B);
+    if (!workspace || workspace_bytes < need) {
+        set_error("%s: workspace too small: %zu < %zu", fn, workspace ? workspace_bytes : (size_t)0, need);
+        return C2V_EWORKSPACE;
+    }
+    oa->coef = coef;
+    oa->part = static_cast<uint8_t *>(workspace) + align_up(c2v_label_workspace_bytes(d, B), 1024);
+    return C2V_OK;
+}
+
+int c2v_label_loss_argmax_opts(const c2v_dims *d, const c2v_params *p, const float *code_vector, const int64_t *label,
+                               int32_t B, const c2v_loss_options *options, float *outputs, float *loss, float *lse,
+                               float *coef, int64_t *argmax, float *maxval, void *workspace, size_t workspace_bytes,
+                               int32_t algo, void *stream)
+{
+    if (!options)
+        return c2v_label_loss_argmax(d, p, code_vector, label, B, outputs, loss, lse, argmax, maxval, workspace,
+                                     workspace_bytes, algo, stream);
+    if (!dims_ok(d)) return C2V_EINVAL;
+    if (!p || !p->output_weight || !code_vector || !label || B < 1 || d->label_count < 1 || (!loss && !lse)) {
+        set_error("c2v_label_loss_argmax_opts: bad argument");
+        return C2V_EINVAL;
+    }
+    LossOptArgs oa;
+    int rc = loss_opts_call_ok("c2v_label_loss_argmax_opts", d, B, options, coef, workspace, workspace_bytes, &oa);
+    if (rc != C2V_OK) return rc;
+    if (!c2v_label_loss_supported(d, B)) {
+        set_error("c2v_label_loss_argmax_opts: the fused loss needs encode_size %% 4 == 0, <= 256 and B <= 2048 (got %d, %d); "
+                  "use c2v_label_logits + c2v_loss_argmax_opts", d->encode, B);
+        return C2V_EUNSUPPORTED;
+    }
+    LabelLossArgs la = {};
+    la.label = reinterpret_cast<const long long *>(label); la.loss = loss; la.lse_out = lse; la.opts = &oa;
+    return label_gemm(d, p, code_vector, B, outputs, argmax, maxval, workspace, workspace_bytes, algo, stream, &la);
+}
+
+int c2v_label_dlogits_opts(const c2v_dims *d, const c2v_params *p, const float *code_vector, const int64_t *label,
+                           const float *lse, const float *coef, int32_t B, const c2v_loss_options *options, float scale,
+                           const float *scale_device, float *d_outputs, void *workspace, size_t workspace_bytes,
+                           int32_t algo, void *stream)
+{
+    if (!options)
+        return c2v_label_dlogits(d, p, code_vector, label, lse, B, scale, scale_device, d_outputs, workspace, workspace_bytes,
+                                 algo, stream);
+    if (!dims_ok(d)) return C2V_EINVAL;
+    if (!p || !p->output_weight || !code_vector || !label || !lse || !coef || !d_outputs || B < 1 || d->label_count < 1) {
+        set_error("c2v_label_dlogits_opts: bad argument");
+        return C2V_EINVAL;
+    }
+    LossOptArgs oa;
+    const int rc = loss_opts_ok("c2v_label_dlogits_opts", options, true, &oa);
+    if (rc != C2V_OK) return rc;
+    if (!label_tcgen05_shape_ok(d)) {
+        set_error("c2v_label_dlogits_opts: needs encode_size %% 4 == 0 and <= 256 (got %d)", d->encode);
+        return C2V_EUNSUPPORTED;
+    }
+    oa.coef = const_cast<float *>(coef);                     // (read only in the dlogits mode)
+    LabelLossArgs la = {};
+    la.label = reinterpret_cast<const long long *>(label); la.dlogits_lse = lse; la.dscale = scale; la.dscale_ptr = scale_device;
+    la.opts = &oa;
+    return label_gemm(d, p, code_vector, B, d_outputs, nullptr, nullptr, workspace, workspace_bytes, algo | C2V_FLAG_NO_PDL,
+                      stream, &la);
+}
+
+int c2v_angular_loss_argmax_opts(const c2v_dims *d, const c2v_params *p, const float *code_vector, const int64_t *label,
+                                 int32_t B, float margin, float inverse_temp, const c2v_loss_options *options,
+                                 float *outputs, float *loss, float *lse, float *coef, int64_t *argmax, float *maxval,
+                                 float *inv_norms, void *workspace, size_t workspace_bytes, int32_t algo, void *stream)
+{
+    if (!options)
+        return c2v_angular_loss_argmax(d, p, code_vector, label, B, margin, inverse_temp, outputs, loss, lse, argmax, maxval,
+                                       inv_norms, workspace, workspace_bytes, algo, stream);
+    if (!dims_ok(d)) return C2V_EINVAL;
+    if (!p || !p->output_weight || !code_vector || !label || !inv_norms || B < 1 || d->label_count < 1 || (!loss && !lse)) {
+        set_error("c2v_angular_loss_argmax_opts: bad argument (NULL pointer, B < 1 or neither loss nor lse)");
+        return C2V_EINVAL;
+    }
+    LossOptArgs oa;
+    int rc = loss_opts_call_ok("c2v_angular_loss_argmax_opts", d, B, options, coef, workspace, workspace_bytes, &oa);
+    if (rc != C2V_OK) return rc;
+    if (!c2v_label_loss_supported(d, B)) {
+        set_error("c2v_angular_loss_argmax_opts: the fused loss needs encode_size %% 4 == 0, <= 256 and B <= 2048 (got %d, "
+                  "%d); use c2v_angular_forward_train + c2v_loss_argmax_opts", d->encode, B);
+        return C2V_EUNSUPPORTED;
+    }
+    rc = angular_inv_norms(d, p, code_vector, B, inv_norms, stream);
+    if (rc != C2V_OK) return rc;
+    LabelLossArgs la = {};
+    la.label = reinterpret_cast<const long long *>(label); la.loss = loss; la.lse_out = lse; la.opts = &oa;
+    la.inv_norms = inv_norms; la.cos_m = cosf(margin); la.sin_m = sinf(margin); la.inverse_temp = inverse_temp;
+    return label_gemm(d, p, code_vector, B, outputs, argmax, maxval, workspace, workspace_bytes, algo, stream, &la);
+}
+
+int c2v_angular_dlogits_opts(const c2v_dims *d, const c2v_params *p, const float *code_vector, const int64_t *label,
+                             const float *lse, const float *coef, const float *inv_norms, int32_t B, float margin,
+                             float inverse_temp, const c2v_loss_options *options, float scale, const float *scale_device,
+                             float *d_dot, void *workspace, size_t workspace_bytes, int32_t algo, void *stream)
+{
+    if (!options)
+        return c2v_angular_dlogits(d, p, code_vector, label, lse, inv_norms, B, margin, inverse_temp, scale, scale_device,
+                                   d_dot, workspace, workspace_bytes, algo, stream);
+    if (!dims_ok(d)) return C2V_EINVAL;
+    if (!p || !p->output_weight || !code_vector || !label || !lse || !coef || !inv_norms || !d_dot || B < 1 ||
+        d->label_count < 1) {
+        set_error("c2v_angular_dlogits_opts: bad argument (NULL pointer or B < 1)");
+        return C2V_EINVAL;
+    }
+    LossOptArgs oa;
+    const int rc = loss_opts_ok("c2v_angular_dlogits_opts", options, true, &oa);
+    if (rc != C2V_OK) return rc;
+    if (!label_tcgen05_shape_ok(d)) {
+        set_error("c2v_angular_dlogits_opts: needs encode_size %% 4 == 0 and <= 256 (got %d)", d->encode);
+        return C2V_EUNSUPPORTED;
+    }
+    oa.coef = const_cast<float *>(coef);
+    LabelLossArgs la = {};
+    la.label = reinterpret_cast<const long long *>(label); la.dlogits_lse = lse; la.dscale = scale; la.dscale_ptr = scale_device;
+    la.inv_norms = inv_norms; la.cos_m = cosf(margin); la.sin_m = sinf(margin); la.inverse_temp = inverse_temp;
+    la.opts = &oa;
+    return label_gemm(d, p, code_vector, B, d_dot, nullptr, nullptr, workspace, workspace_bytes, algo | C2V_FLAG_NO_PDL, stream,
+                      &la);
+}
+
 int c2v_angular_backward_ws(const c2v_dims *d, const c2v_params *p, const float *code_vector, const float *d_dot,
                             const float *inv_norms, int32_t B, float *d_code_vector, float *d_output_weight, void *workspace,
                             size_t workspace_bytes, int32_t algo, void *stream)
@@ -870,6 +1034,22 @@ int c2v_loss_argmax(const float *outputs, const int64_t *label, int32_t B, int64
     return launch_loss_argmax(outputs, reinterpret_cast<const long long *>(label), B, C, loss,
                               reinterpret_cast<long long *>(argmax), maxval, d_outputs,
                               static_cast<cudaStream_t>(stream));
+}
+
+int c2v_loss_argmax_opts(const float *outputs, const int64_t *label, int32_t B, int64_t C,
+                         const c2v_loss_options *options, float *loss, int64_t *argmax, float *maxval, float *d_outputs,
+                         void *stream)
+{
+    if (!options) return c2v_loss_argmax(outputs, label, B, C, loss, argmax, maxval, d_outputs, stream);
+    if (!outputs || !label || B < 1 || C < 1 || (!loss && !d_outputs)) {
+        set_error("c2v_loss_argmax_opts: bad argument (NULL outputs / label, B < 1, C < 1 or neither loss nor d_outputs)");
+        return C2V_EINVAL;
+    }
+    LossOptArgs oa;
+    const int rc = loss_opts_ok("c2v_loss_argmax_opts", options, false, &oa);
+    if (rc != C2V_OK) return rc;
+    return launch_loss_argmax_opts(outputs, reinterpret_cast<const long long *>(label), B, C, oa, loss,
+                                   reinterpret_cast<long long *>(argmax), maxval, d_outputs, static_cast<cudaStream_t>(stream));
 }
 
 int c2v_label_backward(const c2v_dims *d, const c2v_params *p, const float *code_vector,

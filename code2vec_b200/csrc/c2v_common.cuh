@@ -202,7 +202,19 @@ struct LabelLossArgs {
     int topk_k;
     long long *topk_idx;
     float *topk_val, *topk_prob;
+    const struct LossOptArgs *opts;   // criterion options (c2v_*_opts), or NULL: weights 1, mean, no ignore_index
 };
+// criterion options of the loss / dlogits modes, from a checked c2v_loss_options
+struct LossOptArgs {
+    const float *weight;         // [C] class weights or NULL (all 1)
+    long long ignore_index;
+    float eps;                   // label smoothing, in [0, 1]
+    int reduction;               // C2V_REDUCTION_*
+    const float *row_grad;       // dlogits mode, reduction none: [B] upstream gradient of the row losses
+    float *coef;                 // [2 B + 1] row coefficients: written by the loss mode, read by the dlogits mode
+    void *part;                  // loss mode: label_loss_opts_bytes of workspace for the partials
+};
+size_t label_loss_opts_bytes(const c2v_dims *d, int B);
 size_t label_topk_workspace_bytes(const c2v_dims *d, int B, int k);
 float *label_topk_inv_norms(const c2v_dims *d, int B, int k, void *ws);     // where the angular head's inv_norms go
 int launch_label_tcgen05_ex(const c2v_dims *d, const float *cv, int B, const float *Wout, const float *bias,

@@ -385,6 +385,148 @@ int launch_loss_argmax(const float *out, const long long *label, int B, long lon
     return C2V_OK;
 }
 
+// ------------------------------------------------------------------------------------
+// The same with criterion options (c2v_loss_argmax_opts; the definition is in include/c2v_b200.h).  Three launches, every
+// sum in a fixed order: the weighted mean needs den before d_outputs, so a pre-pass over the labels writes the row
+// coefficients coef [2 B + 1] = {a_i = (1 - eps) w_y} {u_i} {den}; then one CTA per row; then the sum over the rows.
+// ------------------------------------------------------------------------------------
+__device__ __forceinline__ float block_sum256(float v, float *red)      // 256 threads, fixed order; red: 8 floats
+{
+    v = warp_sum(v);
+    __syncthreads();                                      // (red may still be read from a previous call)
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+    __syncthreads();
+    float s = 0.0f;
+    for (int w = 0; w < 8; ++w) s += red[w];
+    return s;
+}
+
+__global__ void __launch_bounds__(1024)
+loss_opts_coef_kernel(const long long *__restrict__ label, int B, long long C, const float *__restrict__ weight,
+                      long long ignore_index, float eps, int reduction, float *__restrict__ coef)
+{
+    __shared__ float red[32], s_den;
+    float dacc = 0.0f;
+    for (int b = threadIdx.x; b < B; b += blockDim.x) {
+        const long long y = label[b];
+        const float wy = (y == ignore_index || y < 0 || y >= C) ? 0.0f : (weight ? weight[y] : 1.0f);
+        coef[b] = (1.0f - eps) * wy;
+        dacc += wy;
+    }
+    dacc = warp_sum(dacc);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = dacc;
+    __syncthreads();
+    if (threadIdx.x < 32) {
+        const float den = warp_sum(threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : 0.0f);
+        if (threadIdx.x == 0) { s_den = den; coef[2 * B] = den; }
+    }
+    __syncthreads();
+    const float u = reduction == C2V_REDUCTION_MEAN ? 1.0f / s_den : 1.0f;
+    for (int b = threadIdx.x; b < B; b += blockDim.x) coef[B + b] = label[b] == ignore_index ? 0.0f : u;
+}
+
+// one CTA per row: arg-max, lse, the smoothing sum  sum_j w_j (lse - z_j) = q + W log s  with q = sum_j w_j (max - z_j)
+// (no cancellation), the row's loss term -> rows[b] and, when d_out is given, its gradient row for a unit upstream gradient
+__global__ void __launch_bounds__(256)
+loss_argmax_opts_kernel(const float *__restrict__ out, const long long *__restrict__ label, int B, long long C,
+                        const float *__restrict__ weight, long long ignore_index, float eps_c, const float *__restrict__ coef,
+                        float *__restrict__ rows, long long *__restrict__ argmax, float *__restrict__ maxval,
+                        float *__restrict__ d_out)
+{
+    __shared__ float s_val[8], red[8];
+    __shared__ long long s_idx[8];
+    const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const float *r = out + (size_t)b * C;
+    float mx = -INFINITY; long long am = 0x7fffffffffffffffLL;
+    for (long long c = tid; c < C; c += 256) {
+        const float v = r[c];
+        if (v > mx) { mx = v; am = c; }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const float ov = __shfl_xor_sync(0xffffffffu, mx, o);
+        const long long oi = __shfl_xor_sync(0xffffffffu, am, o);
+        if (ov > mx || (ov == mx && oi < am)) { mx = ov; am = oi; }
+    }
+    if (lane == 0) { s_val[warp] = mx; s_idx[warp] = am; }
+    __syncthreads();
+    mx = s_val[0]; am = s_idx[0];
+    for (int w = 1; w < 8; ++w)
+        if (s_val[w] > mx || (s_val[w] == mx && s_idx[w] < am)) { mx = s_val[w]; am = s_idx[w]; }
+    float s = 0.0f, q = 0.0f, W = 0.0f;
+    for (long long c = tid; c < C; c += 256) {
+        const float v = r[c], w = weight ? weight[c] : 1.0f;
+        s += __expf(v - mx);
+        q = fmaf(w, mx - v, q);
+        W += w;
+    }
+    s = block_sum256(s, red);
+    q = block_sum256(q, red);
+    W = block_sum256(W, red);
+    const float ls = logf(s), lse = mx + ls;
+    const long long y = label[b];
+    const bool ign = y == ignore_index, valid = y >= 0 && y < C;
+    const float a = coef[b], u = coef[B + b];
+    if (tid == 0) {
+        if (argmax) argmax[b] = am;
+        if (maxval) maxval[b] = mx;
+        const float zy = valid ? r[y] : __int_as_float(0x7fffffff);      // no target logit: a NaN row, as without options
+        rows[b] = ign ? 0.0f : fmaf(eps_c, fmaf(W, ls, q), a * (lse - zy));
+    }
+    if (d_out) {
+        const float inv = 1.0f / s;
+        float *g = d_out + (size_t)b * C;
+        for (long long c = tid; c < C; c += 256) {
+            const float p = __expf(r[c] - mx) * inv, w = weight ? weight[c] : 1.0f;
+            g[c] = u * fmaf(eps_c, fmaf(W, p, -w), a * (p - (c == y ? 1.0f : 0.0f)));
+        }
+    }
+}
+
+// loss from the row terms in a fixed order: mean sum / den, sum; none: the rows themselves (written by the row kernel)
+__global__ void __launch_bounds__(256)
+loss_sum_opts_kernel(const float *__restrict__ rows, int B, const float *__restrict__ den, int reduction, float *__restrict__ loss)
+{
+    __shared__ float red[256];
+    float s = 0.0f;
+    for (int b = threadIdx.x; b < B; b += 256) s += rows[b];
+    red[threadIdx.x] = s;
+    __syncthreads();
+    for (int o = 128; o > 0; o >>= 1) {
+        if ((int)threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) *loss = reduction == C2V_REDUCTION_MEAN ? red[0] / *den : red[0];
+}
+
+static int loss_argmax_opts_launches(const float *out, const long long *label, int B, long long C, const LossOptArgs &o,
+                                     float *loss, long long *argmax, float *maxval, float *d_out, float *scratch,
+                                     cudaStream_t st)
+{
+    float *coef = scratch, *rows = scratch + 2 * B + 1;
+    const bool none = o.reduction == C2V_REDUCTION_NONE;
+    loss_opts_coef_kernel<<<1, 1024, 0, st>>>(label, B, C, o.weight, o.ignore_index, o.eps, o.reduction, coef);
+    C2V_LAUNCH_OK("loss_opts_coef_kernel");
+    loss_argmax_opts_kernel<<<B, 256, 0, st>>>(out, label, B, C, o.weight, o.ignore_index, (float)((double)o.eps / (double)C),
+                                               coef, none && loss ? loss : rows, argmax, maxval, d_out);
+    C2V_LAUNCH_OK("loss_argmax_opts_kernel");
+    if (loss && !none) {
+        loss_sum_opts_kernel<<<1, 256, 0, st>>>(rows, B, coef + 2 * B, o.reduction, loss);
+        C2V_LAUNCH_OK("loss_sum_opts_kernel");
+    }
+    return C2V_OK;
+}
+
+int launch_loss_argmax_opts(const float *out, const long long *label, int B, long long C, const LossOptArgs &o, float *loss,
+                            long long *argmax, float *maxval, float *d_out, cudaStream_t st)
+{
+    float *scratch = nullptr;                             // coef [2 B + 1] | rows [B]
+    C2V_CUDA_OK(cudaMallocAsync(&scratch, (size_t)(3 * B + 1) * sizeof(float), st));
+    const int rc = loss_argmax_opts_launches(out, label, B, C, o, loss, argmax, maxval, d_out, scratch, st);
+    cudaFreeAsync(scratch, st);
+    return rc;
+}
+
 // column sums of d_out [B, C] -> d_bias [C]
 __global__ void colsum_kernel(const float *__restrict__ X, int B, long long C, float *__restrict__ out)
 {

@@ -173,6 +173,16 @@ struct LtSim {
     long long qbase;
     long long cap; unsigned long long *pcount; // pairs: every match adds 1 to *pcount (whatever cap is)
 };
+// Criterion options (the OPT instantiations, c2v_*_opts): class weights and label smoothing.  The last parameter, so that
+// the other instantiations keep their parameter layout; they pass it zeroed.
+//   part mode:    per (row, n-tile, 32-column block) (m, sum exp(v - m), q = sum_j w_j (m - v_j), W_b = sum_j w_j) -> part,
+//                 the smoothing partial without cancellation (every term >= 0 for non-negative weights)
+//   dlogits mode: G = (p - [col == label]) A_i + K_i (W p - w_j), A_i = sc u_i a_i, K_i = sc u_i eps / C, with the row
+//                 coefficients a_i = (1 - eps) w[y_i], u_i and W of loss_finalize_opts_kernel (coef [2 B + 1]) and sc the
+//                 upstream gradient (row_grad[i] for reduction none)
+struct LtOpt {
+    float4 *part; const float *weight; const float *coef; const float *row_grad; float eps_c; int B;
+};
 
 // Top-k mode (the label_gemm_v2_kernel<*, true> instantiations): a thread of the epilogue (one row, one column quarter of
 // its CTA's m-tile) keeps the topk_k largest keys  lt_orderable(v) << 32 | ~col  it has seen, sorted descending, in its
@@ -218,6 +228,8 @@ constexpr int SMEM_TAB_OFF = SMEM_STG_OFF + STG_BYTES;
 constexpr int SMEM_BIAS_OFF = SMEM_TAB_OFF + TAB_BYTES;      // [16 warps][32] bias of the current tile
 constexpr int SMEM_BAR_OFF = SMEM_BIAS_OFF + N_EPI_WARPS * 32 * 4;
 constexpr int SMEM_BYTES = SMEM_BAR_OFF + 128 + 1024;
+constexpr int SMEM_W_OFF = SMEM_BAR_OFF + 128;               // OPT only: [16 warps][32] class weights of the current tile
+constexpr int SMEM_BYTES_OPT = SMEM_W_OFF + N_EPI_WARPS * 32 * 4 + 1024;
 }  // namespace lt2
 
 // K2 v2: persistent label GEMM with the arg-max folded in.  The 128 x 128 output tiles are numbered n-tile major /
@@ -234,16 +246,18 @@ constexpr int SMEM_BYTES = SMEM_BAR_OFF + 128 + 1024;
 // SIM (with ANG, lane order, hdr unused): similarity search over a code-vector bank (c2v_knn_*), the value being the cosine
 // itself (see LtSim).  SIM_KNN is the top-k mode with the columns of sm.excl left out; SIM_PAIRS writes every
 // (row, column, cos) with cos >= sm.thr instead.
+// OPT (loss / dlogits modes only, lt2::SMEM_BYTES_OPT of shared memory): the criterion options of LtOpt.
 constexpr int SIM_NONE = 0, SIM_KNN = 1, SIM_PAIRS = 2;
-template <bool ANG, bool TOPK, int SIM = SIM_NONE>
+template <bool ANG, bool TOPK, int SIM = SIM_NONE, bool OPT = false>
 __global__ void __launch_bounds__(lt2::THREADS, 1)
 label_gemm_v2_kernel(const uint8_t *__restrict__ imgA, const uint8_t *__restrict__ imgB,
                      const float *__restrict__ bias, const float *__restrict__ hdr, float *__restrict__ out,
                      int M, long long N, int nkb, int n_mt, long long n_nt, long long n_tiles,
                      unsigned long long *__restrict__ keys, unsigned *__restrict__ ticket,
                      long long *__restrict__ argmax, float *__restrict__ maxval, int dbg, const LtLoss ls, const int per_m,
-                     const LtSim sm)
+                     const LtSim sm, const LtOpt op)
 {
+    static_assert(!OPT || (!TOPK && SIM == SIM_NONE), "criterion options belong to the loss / dlogits modes");
     extern __shared__ unsigned char smem_raw[];
     const uint32_t raw = lt_smem_u32(smem_raw);
     const uint32_t base = (raw + 1023u) & ~1023u;
@@ -319,7 +333,18 @@ label_gemm_v2_kernel(const uint8_t *__restrict__ imgA, const uint8_t *__restrict
             return c2 < N ? __ldg(colv + c2) : 0.0f;
         };
         float bias_next = bias_of(0);
-        unsigned long long *tk_list = nullptr;                // top-k: this thread's list and the upper word of its k-th key
+        // OPT: the class weights of the same columns, fetched the same way (1 without a weight vector, 0 past the last
+        // column, so that the smoothing partials need no column test for W_b)
+        float *sw = OPT ? reinterpret_cast<float *>(smem + lt2::SMEM_W_OFF) + warp * 32 : nullptr;
+        auto weight_of = [&](int i) {
+            if (i >= my_tiles) return 0.0f;
+            const LtTile t2 = tile_of(i);
+            const long long c2 = t2.nt * lt::TN + cq * 32 + lane;
+            return c2 < N ? (op.weight ? __ldg(op.weight + c2) : 1.0f) : 0.0f;
+        };
+        float w_next = 0.0f;
+        if constexpr (OPT) w_next = weight_of(0);
+        unsigned long long *tk_list = nullptr;               // top-k: this thread's list and the upper word of its k-th key
         uint32_t tk_thr = 0;
         if constexpr (TOPK) {
             tk_list = ls.topk + ((size_t)blockIdx.x * 512 + cq * 128 + q * 32 + lane) * ls.topk_k;
@@ -364,8 +389,10 @@ label_gemm_v2_kernel(const uint8_t *__restrict__ imgA, const uint8_t *__restrict
             const int n_rows = (int)(M - row0 < 32 ? M - row0 : 32);
             // bias of this warp's 32 columns: one element per lane -> smem -> broadcast float4 reads
             sbias[lane] = bias_next;
+            if constexpr (OPT) sw[lane] = w_next;
             __syncwarp();
             bias_next = bias_of(i + 1);
+            if constexpr (OPT) w_next = weight_of(i + 1);
             float icv_r = 0.0f;                                        // angular: 1 / |cv| of this thread's row (thread = row)
             if constexpr (ANG) icv_r = row0 + lane < M ? __ldg(ls.icv + row0 + lane) : 0.0f;
             float d[2][16];
@@ -459,7 +486,22 @@ label_gemm_v2_kernel(const uint8_t *__restrict__ imgA, const uint8_t *__restrict
                     const float mb = m * LT_LOG2E;
 #pragma unroll
                     for (int j = 0; j < 32; ++j) ssum += j < n_cols ? lt_ex2(fmaf(v[j], LT_LOG2E, -mb)) : 0.0f;
-                    ls.part[(size_t)(nt * 4 + cq) * ls.Mpad + grow] = make_float2(m, n_cols > 0 ? ssum : 0.0f);
+                    if constexpr (OPT) {
+                        float qs = 0.0f, wb = 0.0f;
+#pragma unroll
+                        for (int j = 0; j < 32; j += 4) {
+                            const float4 w4 = *reinterpret_cast<const float4 *>(sw + j);
+                            const float wj[4] = {w4.x, w4.y, w4.z, w4.w};
+#pragma unroll
+                            for (int u = 0; u < 4; ++u) {
+                                qs += j + u < n_cols ? wj[u] * (m - v[j + u]) : 0.0f;
+                                wb += wj[u];
+                            }
+                        }
+                        op.part[(size_t)(nt * 4 + cq) * ls.Mpad + grow] = make_float4(m, n_cols > 0 ? ssum : 0.0f, qs, wb);
+                    } else {
+                        ls.part[(size_t)(nt * 4 + cq) * ls.Mpad + grow] = make_float2(m, n_cols > 0 ? ssum : 0.0f);
+                    }
                     if (__any_sync(0xffffffffu, tj >= 0 && tj < n_cols)) {
                         // select chain in PTX: written in C++ the compiler turns it into v[tj], a dynamically indexed read
                         // that puts all of v[] in local memory -- 8 x STL.128 per thread and tile in EVERY mode of this
@@ -476,7 +518,35 @@ label_gemm_v2_kernel(const uint8_t *__restrict__ imgA, const uint8_t *__restrict
                 if (!TOPK && ls.lse) {                                                  // dlogits (overwrites v)
                     const float lb = (grow < M ? ls.lse[grow] : 0.0f) * LT_LOG2E;
                     const float sc = ls.dscale_ptr ? ls.dscale * *ls.dscale_ptr : ls.dscale;
-                    if constexpr (!ANG) {
+                    if constexpr (OPT) {
+                        // d logit = (p - [j == y]) A + K (W p - w_j); K == 0 (no smoothing) leaves the first term's bits
+                        const bool in = grow < M;
+                        const float up = op.row_grad ? ls.dscale * (in ? op.row_grad[grow] : 0.0f) : sc;
+                        const float ur = up * (in ? op.coef[op.B + grow] : 0.0f);
+                        const float A = ur * (in ? op.coef[grow] : 0.0f), K = ur * op.eps_c, Wt = op.coef[2 * op.B];
+                        const float tf = ANG && cos_t > 0.0f ? ls.cos_m + ls.sin_m * cos_t / sqrtf(1.0f - cos_t * cos_t) : 1.0f;
+#pragma unroll
+                        for (int j = 0; j < 32; j += 4) {
+                            const float4 w4 = *reinterpret_cast<const float4 *>(sw + j);
+                            const float wj[4] = {w4.x, w4.y, w4.z, w4.w};
+                            float4 iw4 = make_float4(0.f, 0.f, 0.f, 0.f);
+                            if constexpr (ANG) iw4 = *reinterpret_cast<const float4 *>(sbias + j);
+                            const float iwj[4] = {iw4.x, iw4.y, iw4.z, iw4.w};
+#pragma unroll
+                            for (int u = 0; u < 4; ++u) {
+                                const bool t = j + u == (int)tj;
+                                const float p = lt_ex2(fmaf(v[j + u], LT_LOG2E, -lb));
+                                const float g = fmaf(K, fmaf(Wt, p, -wj[u]), (p - (t ? 1.0f : 0.0f)) * A);
+                                if constexpr (!ANG) {
+                                    v[j + u] = g;
+                                } else {                          // G = d loss / d dot, as below
+                                    float dcos = g * ls.s;
+                                    if (t) dcos *= tf;
+                                    v[j + u] = dcos * icv_r * iwj[u];
+                                }
+                            }
+                        }
+                    } else if constexpr (!ANG) {
 #pragma unroll
                         for (int j = 0; j < 32; ++j) v[j] = (lt_ex2(fmaf(v[j], LT_LOG2E, -lb)) - ((j == (int)tj) ? 1.0f : 0.0f)) * sc;
                     } else {
@@ -734,6 +804,88 @@ loss_finalize_kernel(const float2 *__restrict__ part2, int nsplit, int Mpad, con
     }
 }
 
+// ---- the same with the criterion options: (max, sum exp, q, W_b) partials (see LtOpt) --------------------------------
+// A merge to the larger max M adds W_b (M - m_b) to the q of the side whose max was smaller: every term stays >= 0.
+// (S, M) are merged with lt_merge's exact operations, so that lse is the same number as without options.
+__device__ __forceinline__ void lt_merge4(float4 &a, const float4 b) {
+    if (b.x > a.x) {
+        const float q = a.x > -INFINITY ? fmaf(a.w, b.x - a.x, a.z) : a.z;   // (no column merged yet: W = 0, q = 0)
+        a.y = a.y * __expf(a.x - b.x) + b.y; a.x = b.x;
+        a.z = q + b.z; a.w += b.w;
+    } else if (b.x > -INFINITY) {
+        a.y += b.y * __expf(b.x - a.x);
+        a.z += fmaf(b.w, a.x - b.x, b.z); a.w += b.w;
+    }
+}
+__global__ void __launch_bounds__(256)
+loss_partials_reduce_opts_kernel(const float4 *__restrict__ part, int P, int Mpad, float4 *__restrict__ part2)
+{
+    __shared__ float4 sh[8][32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int row = blockIdx.x * 32 + lane;
+    const int p0 = (int)((long long)P * blockIdx.y / gridDim.y), p1 = (int)((long long)P * (blockIdx.y + 1) / gridDim.y);
+    float4 acc = make_float4(-INFINITY, 0.0f, 0.0f, 0.0f);
+    for (int p = p0 + warp; p < p1; p += 8) lt_merge4(acc, part[(size_t)p * Mpad + row]);
+    sh[warp][lane] = acc;
+    __syncthreads();
+    if (warp == 0) {
+        for (int w = 1; w < 8; ++w) lt_merge4(acc, sh[w][lane]);                        // fixed order: deterministic
+        part2[(size_t)blockIdx.y * Mpad + row] = acc;
+    }
+}
+// one CTA, the reductions in loss_finalize_kernel's fixed order.  Per row i (y = label[i], w_y = weight[y] or 1; an
+// ignored row, label == ignore_index, has w_y = 0 and row term 0):
+//   lse_i = M + log S,  smooth_i = sum_j w_j (lse_i - z_ij) = q + W log S
+//   row_i = (1 - eps) w_y (lse_i - z_iy) + (eps / C) smooth_i,   den = sum_i w_y
+// loss: mean sum_i row_i / den, sum sum_i row_i, none row_i [B].  coef [2 B + 1] for the dlogits mode:
+// a_i = (1 - eps) w_y, u_i = 0 if ignored else (1 / den for mean, 1 otherwise), then W.
+// A label outside [0, C) that is not ignore_index has no target logit (tgt stays NaN): its row is NaN, as without
+// options, and it adds nothing to den.
+__global__ void __launch_bounds__(1024)
+loss_finalize_opts_kernel(const float4 *__restrict__ part2, int nsplit, int Mpad, const float *__restrict__ tgt,
+                          const long long *__restrict__ label, int B, long long C, const float *__restrict__ weight,
+                          long long ignore_index, float eps, float eps_c, int reduction, float *__restrict__ lse,
+                          float *__restrict__ loss, float *__restrict__ coef)
+{
+    __shared__ float red[32], red_den[32], s_den;
+    float acc = 0.0f, dacc = 0.0f;
+    for (int b = threadIdx.x; b < B; b += blockDim.x) {
+        float4 a = make_float4(-INFINITY, 0.0f, 0.0f, 0.0f);
+        for (int k = 0; k < nsplit; ++k) lt_merge4(a, part2[(size_t)k * Mpad + b]);
+        const float ls = logf(a.y), l = a.x + ls;
+        if (lse) lse[b] = l;
+        const long long y = label[b];
+        const bool ign = y == ignore_index, valid = y >= 0 && y < C;
+        const float wy = (ign || !valid) ? 0.0f : (weight ? weight[y] : 1.0f);
+        const float ab = (1.0f - eps) * wy;
+        const float row = ign ? 0.0f : fmaf(eps_c, fmaf(a.w, ls, a.z), ab * (l - tgt[b]));
+        if (reduction == C2V_REDUCTION_NONE && loss) loss[b] = row;
+        acc += row;
+        dacc += wy;
+        if (coef) {
+            coef[b] = ab;
+            if (b == 0) coef[2 * B] = a.w;
+        }
+    }
+    acc = warp_sum(acc);
+    dacc = warp_sum(dacc);
+    if ((threadIdx.x & 31) == 0) { red[threadIdx.x >> 5] = acc; red_den[threadIdx.x >> 5] = dacc; }
+    __syncthreads();
+    if (threadIdx.x < 32) {
+        const bool on = threadIdx.x < (blockDim.x >> 5);
+        const float v = warp_sum(on ? red[threadIdx.x] : 0.0f), den = warp_sum(on ? red_den[threadIdx.x] : 0.0f);
+        if (threadIdx.x == 0) {
+            s_den = den;
+            if (loss && reduction == C2V_REDUCTION_MEAN) *loss = v / den;       // every row ignored: 0 / 0 = NaN, as torch
+            else if (loss && reduction == C2V_REDUCTION_SUM) *loss = v;
+        }
+    }
+    if (!coef) return;
+    __syncthreads();
+    const float u = reduction == C2V_REDUCTION_MEAN ? 1.0f / s_den : 1.0f;
+    for (int b = threadIdx.x; b < B; b += blockDim.x) coef[B + b] = label[b] == ignore_index ? 0.0f : u;
+}
+
 // ---- top-k: merging the per-thread lists of label_gemm_v2_kernel<*, true> --------------------------------------------
 constexpr int LT_TOPK_MAX_CTAS = 256;               // grid cap of the top-k GEMM: bounds its workspace independently of the device
 // one warp per row b: the row's 4 per_m sorted lists (list l = 4 slice + column quarter, written by CTA slice * n_mt + mt)
@@ -805,6 +957,13 @@ static size_t lt_loss_bytes(int B, long long C)
 {
     const size_t Mpad = (size_t)(B + 127) / 128 * 128, nt = (size_t)((C + 127) / 128);
     return (nt * 4 + LT_PSPLIT) * Mpad * sizeof(float2) + Mpad * sizeof(float) + 1024;
+}
+// criterion options (c2v_*_opts): part4 [nt * 4][Mpad] float4 | part4_2 [LT_PSPLIT][Mpad] float4, in a region of its own
+// so that the label workspace keeps its layout
+size_t label_loss_opts_bytes(const c2v_dims *d, int B)
+{
+    const size_t Mpad = (size_t)(B + 127) / 128 * 128, nt = (size_t)((d->label_count + 127) / 128);
+    return (nt * 4 + LT_PSPLIT) * Mpad * sizeof(float4) + 1024;
 }
 size_t label_tcgen05_workspace_bytes(const c2v_dims *d, int B)
 {
@@ -950,8 +1109,28 @@ int launch_label_tcgen05_ex(const c2v_dims *d, const float *cv, int B, const flo
         ls.topk_k = la->topk_k;
         if (la->topk_prob) ls.part = part;                              // (max, sum exp) partials, no label / target
     }
+    const LossOptArgs *opt = la ? la->opts : nullptr;
+    LtOpt op;
+    memset(&op, 0, sizeof(op));
+    float4 *part4 = nullptr, *part4_2 = nullptr;
+    if (opt) {
+        if (topk || !opt->coef || (want_loss && !opt->part)) {
+            set_error("label loss options: top-k mode, or coefficients / partials missing");
+            return C2V_EINVAL;
+        }
+        op.weight = opt->weight; op.coef = opt->coef; op.row_grad = opt->row_grad; op.B = B;
+        op.eps_c = (float)((double)opt->eps / (double)C);
+        if (want_loss) {
+            part4 = static_cast<float4 *>(opt->part);
+            part4_2 = part4 + nt * 4 * (size_t)Mpad;
+            op.part = part4;
+            ls.part = reinterpret_cast<float2 *>(part4);          // (selects the loss mode; the OPT epilogue writes op.part)
+        }
+    }
     auto *kern = topk ? (angular ? label_gemm_v2_kernel<true, true> : label_gemm_v2_kernel<false, true>)
+               : opt  ? (angular ? label_gemm_v2_kernel<true, false, SIM_NONE, true> : label_gemm_v2_kernel<false, false, SIM_NONE, true>)
                       : (angular ? label_gemm_v2_kernel<true, false> : label_gemm_v2_kernel<false, false>);
+    const int smem_bytes = opt ? lt2::SMEM_BYTES_OPT : lt2::SMEM_BYTES;
     const bool want_arg = argmax || maxval;
     const bool fused_arg = want_arg && mt <= (size_t)lt2::MAX_MT;
     int dev = 0, sms = 0;
@@ -971,7 +1150,7 @@ int launch_label_tcgen05_ex(const c2v_dims *d, const float *cv, int B, const flo
                            reinterpret_cast<unsigned long long *>(key_region), fused_arg ? 8 + B : 0));
     C2V_COUNT_LAUNCH();
 
-    C2V_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, lt2::SMEM_BYTES));
+    C2V_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
     const long long n_tiles = (long long)mt * (long long)nt;
     int grid = (int)(n_tiles < sms ? n_tiles : sms);
     // tile order (see lt_range): lanes when that keeps >= 95 % of the CTAs busy, else groups; C2V_LABEL_ORDER=groups|lanes forces one
@@ -986,13 +1165,21 @@ int launch_label_tcgen05_ex(const c2v_dims *d, const float *cv, int B, const flo
         per_m = grid / (int)mt;
         if (per_m < 1) { set_error("label top-k: %d SMs for %zu m-tiles", sms, mt); return C2V_EUNSUPPORTED; }
     }
-    C2V_CUDA_OK(launch_pdl(kern, dim3((unsigned)grid), dim3(lt2::THREADS), (size_t)lt2::SMEM_BYTES, st,
+    C2V_CUDA_OK(launch_pdl(kern, dim3((unsigned)grid), dim3(lt2::THREADS), (size_t)smem_bytes, st,
                            (const uint8_t *)imgA, (const uint8_t *)imgB, bias, (const float *)hdr, out, B, C, nkb, (int)mt,
                            (long long)nt, n_tiles, fused_arg ? keys : (unsigned long long *)nullptr, ticket,
                            fused_arg ? argmax : (long long *)nullptr, fused_arg ? maxval : (float *)nullptr,
-                           getenv("C2V_K2_FLAGS") ? atoi(getenv("C2V_K2_FLAGS")) : 0, ls, per_m, LtSim{}));
+                           getenv("C2V_K2_FLAGS") ? atoi(getenv("C2V_K2_FLAGS")) : 0, ls, per_m, LtSim{}, op));
     C2V_LAUNCH_OK("label_gemm_v2_kernel");
-    if (want_loss) {
+    if (want_loss && opt) {
+        loss_partials_reduce_opts_kernel<<<dim3((unsigned)(Mpad / 32), LT_PSPLIT), 256, 0, st>>>(part4, (int)(nt * 4), Mpad,
+                                                                                               part4_2);
+        C2V_LAUNCH_OK("loss_partials_reduce_opts_kernel");
+        loss_finalize_opts_kernel<<<1, 1024, 0, st>>>(part4_2, LT_PSPLIT, Mpad, tgt, la->label, B, C, opt->weight,
+                                                      opt->ignore_index, opt->eps, op.eps_c, opt->reduction, la->lse_out,
+                                                      la->loss, opt->coef);
+        C2V_LAUNCH_OK("loss_finalize_opts_kernel");
+    } else if (want_loss) {
         loss_partials_reduce_kernel<<<dim3((unsigned)(Mpad / 32), LT_PSPLIT), 256, 0, st>>>(part, (int)(nt * 4), Mpad, part2);
         C2V_LAUNCH_OK("loss_partials_reduce_kernel");
         loss_finalize_kernel<<<1, 1024, 0, st>>>(part2, LT_PSPLIT, Mpad, tgt, B, la->lse_out, la->loss);
@@ -1150,7 +1337,7 @@ int launch_knn(const KnnArgs &a, cudaStream_t st)
     C2V_CUDA_OK(launch_pdl(kern, dim3((unsigned)grid), dim3(lt2::THREADS), (size_t)lt2::SMEM_BYTES, st, (const uint8_t *)imgA,
                            (const uint8_t *)imgB, (const float *)nullptr, (const float *)nullptr, (float *)nullptr, a.Q, N, nkb,
                            (int)mt, (long long)nt, n_tiles, (unsigned long long *)nullptr, (unsigned *)nullptr,
-                           (long long *)nullptr, (float *)nullptr, 0, ls, per_m, sm));
+                           (long long *)nullptr, (float *)nullptr, 0, ls, per_m, sm, LtOpt{}));
     C2V_LAUNCH_OK("label_gemm_v2_kernel");
     if (topk) {
         topk_merge_kernel<<<(unsigned)((a.Q + 7) / 8), 256, 0, st>>>(lists, a.k, a.Q, (int)mt, per_m, nullptr, 0,

@@ -456,8 +456,17 @@ class ShardedFlatAdam:
             torch.autograd.graph.increment_version(p)
 
 
-def ddp_step(model, optimizer, bucket, starts, paths, ends, label, loss_fn):
-    """One training step of main.py:171-175 on this rank's shard of the global batch."""
+def _forward_loss(model, starts, paths, ends, label, criterion):
+    # criterion None: the call without it, for any forward_loss of the (starts, paths, ends, label) form
+    if criterion is None:
+        return model.forward_loss(starts, paths, ends, label)[0]
+    return model.forward_loss(starts, paths, ends, label, criterion=criterion)[0]
+
+
+def ddp_step(model, optimizer, bucket, starts, paths, ends, label, loss_fn, criterion=None):
+    """One training step of main.py:171-175 on this rank's shard of the global batch.  loss_fn None: the fused loss of
+    Code2Vec.forward_loss with `criterion` (None, nn.NLLLoss or nn.CrossEntropyLoss; a mean is this rank's own, as with
+    DDP); else forward() and loss_fn(outputs, label)."""
     if isinstance(optimizer, (ShardedFlatAdam, FlatAdam)) and hasattr(model, "fuse_grad_accumulation"):
         model.fuse_grad_accumulation = True                  # .grad are persistent views into a flat bucket: accumulate in place
         if isinstance(optimizer, ShardedFlatAdam) and len(optimizer.regions) > 1 and optimizer.world > 1 and \
@@ -465,7 +474,7 @@ def ddp_step(model, optimizer, bucket, starts, paths, ends, label, loss_fn):
             model.on_path_grads_ready = optimizer.early_step # region 0 is reduced while the backward is still running
     if isinstance(optimizer, ShardedFlatAdam):               # reduction + optimizer + broadcast are one kernel per rank
         if loss_fn is None:                                  # fused loss: the [b, C] logits are never written
-            loss = model.forward_loss(starts, paths, ends, label)[0]
+            loss = _forward_loss(model, starts, paths, ends, label, criterion)
         else:
             outputs, code_vector, attention = model.forward(starts, paths, ends, label)
             loss = loss_fn(outputs, label)
@@ -476,7 +485,7 @@ def ddp_step(model, optimizer, bucket, starts, paths, ends, label, loss_fn):
     if not fused:
         bucket.zero()                       # (FlatAdam leaves the bucket zeroed at the end of its step)
     if loss_fn is None:                     # fused loss (Code2Vec.forward_loss)
-        loss = model.forward_loss(starts, paths, ends, label)[0]
+        loss = _forward_loss(model, starts, paths, ends, label, criterion)
     else:
         outputs, code_vector, attention = model.forward(starts, paths, ends, label)
         loss = loss_fn(outputs, label)

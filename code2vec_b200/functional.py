@@ -443,6 +443,122 @@ def angular_loss(dims, params, cv, label, margin, inverse_temp, want_logits=Fals
     return loss, lse, am, mx, inv, out
 
 
+class LossCriterion:
+    """The criterion of the fused loss, read from an nn.NLLLoss / nn.CrossEntropyLoss (c2v_loss_options):
+    F.cross_entropy(logits, label, weight, ignore_index, reduction, label_smoothing) on the head's logits."""
+
+    def __init__(self, criterion, label_count, device):
+        if type(criterion) not in (torch.nn.NLLLoss, torch.nn.CrossEntropyLoss):
+            raise TypeError("criterion must be exactly torch.nn.NLLLoss (applied, as in the reference, to log_softmax of the "
+                            "logits) or torch.nn.CrossEntropyLoss, not a subclass or another loss: got "
+                            f"{type(criterion).__name__}")
+        w = criterion.weight
+        if w is not None and (w.dtype != torch.float32 or w.device != torch.device(device) or
+                              tuple(w.shape) != (int(label_count),)):
+            raise ValueError(f"criterion weight must be float32 of shape [{int(label_count)}] on {device}, got "
+                             f"{w.dtype} {tuple(w.shape)} on {w.device}")
+        if criterion.reduction not in _lib.REDUCTIONS:
+            raise ValueError(f"{criterion.reduction} is not a valid value for reduction")
+        self.weight = w.contiguous() if w is not None else None    # (the same tensor when contiguous: in-place updates show)
+        self.ignore_index = int(criterion.ignore_index)
+        self.label_smoothing = float(getattr(criterion, "label_smoothing", 0.0))
+        self.reduction = criterion.reduction
+
+    def options(self, row_grad=None):
+        o = _lib.LossOptions(_ptr(self.weight), self.ignore_index, self.label_smoothing, _lib.REDUCTIONS[self.reduction],
+                             _ptr(row_grad))
+        o._keep = (self.weight, row_grad)
+        return o
+
+    def loss_shape(self, B):
+        return (B,) if self.reduction == "none" else ()
+
+
+def label_loss_opts(dims, params, cv, label, crit, angular=None, algo=_lib.ALGO_AUTO, cache=None, weight=None):
+    """label_loss / angular_loss (angular = (margin, inverse_temp)) with a LossCriterion
+    -> (loss 0-d or [B], lse [B], argmax [B], maxval [B], coef [2 B + 1], inv_norms [B + C] or None).  coef holds the row
+    coefficients the matching dlogits call reads on the device."""
+    lib = _lib.load()
+    _need_cuda(cv, label)
+    B = cv.shape[0]
+    dev = cv.device
+    label = _idx(label, "label", (B,))
+    with torch.cuda.device(dev):
+        loss = _empty(crit.loss_shape(B), torch.float32, dev)
+        lse = _empty((B,), torch.float32, dev)
+        am = _empty((B,), torch.int64, dev)
+        mx = _empty((B,), torch.float32, dev)
+        coef = _empty((2 * B + 1,), torch.float32, dev)
+        inv = _empty((B + dims.label_count,), torch.float32, dev) if angular is not None else None
+        sync_deterministic()                     # (the size depends on the mode)
+        nbytes = lib.c2v_label_loss_opts_workspace_bytes(ctypes.byref(dims), B)
+        ws, algo = _label_ws(dims, B, dev, algo, cache, weight, nbytes=nbytes)
+        cv = _f32c(cv, "code_vector")
+        opts = crit.options()
+        if angular is None:
+            rc = lib.c2v_label_loss_argmax_opts(ctypes.byref(dims), ctypes.byref(params), _ptr(cv), _ptr(label), B,
+                                                ctypes.byref(opts), None, _ptr(loss), _ptr(lse), _ptr(coef), _ptr(am),
+                                                _ptr(mx), _ptr(ws), ws.numel(), int(algo), _stream(dev))
+        else:
+            rc = lib.c2v_angular_loss_argmax_opts(ctypes.byref(dims), ctypes.byref(params), _ptr(cv), _ptr(label), B,
+                                                  float(angular[0]), float(angular[1]), ctypes.byref(opts), None, _ptr(loss),
+                                                  _ptr(lse), _ptr(coef), _ptr(am), _ptr(mx), _ptr(inv), _ptr(ws), ws.numel(),
+                                                  int(algo), _stream(dev))
+        _lib.check(rc, "c2v_label_loss_argmax_opts" if angular is None else "c2v_angular_loss_argmax_opts")
+    return loss, lse, am, mx, coef, inv
+
+
+def label_dlogits_opts(dims, params, cv, label, lse, coef, crit, d_loss, inv_norms=None, angular=None,
+                       algo=_lib.ALGO_AUTO, cache=None, weight=None):
+    """d loss / d logits [B, C] (angular: d loss / d (cv . W^T)) of label_loss_opts' loss for its upstream gradient d_loss
+    (0-d, or [B] for reduction none), recomputed from cv and W_out"""
+    lib = _lib.load()
+    B = cv.shape[0]
+    dev = cv.device
+    label = _idx(label, "label", (B,))
+    with torch.cuda.device(dev):
+        g = _empty((B, dims.label_count), torch.float32, dev)
+        ws, algo = _label_ws(dims, B, dev, algo, cache, weight)
+        cv = _f32c(cv, "code_vector"); lse = _f32c(lse, "lse"); d_loss = _f32c(d_loss, "d_loss")
+        none = crit.reduction == "none"
+        opts = crit.options(row_grad=d_loss if none else None)
+        sd = None if none else d_loss.reshape(1)
+        if angular is None:
+            rc = lib.c2v_label_dlogits_opts(ctypes.byref(dims), ctypes.byref(params), _ptr(cv), _ptr(label), _ptr(lse),
+                                            _ptr(coef), B, ctypes.byref(opts), 1.0, _ptr(sd), _ptr(g), _ptr(ws), ws.numel(),
+                                            int(algo), _stream(dev))
+        else:
+            inv = _f32c(inv_norms, "inv_norms")
+            rc = lib.c2v_angular_dlogits_opts(ctypes.byref(dims), ctypes.byref(params), _ptr(cv), _ptr(label), _ptr(lse),
+                                              _ptr(coef), _ptr(inv), B, float(angular[0]), float(angular[1]),
+                                              ctypes.byref(opts), 1.0, _ptr(sd), _ptr(g), _ptr(ws), ws.numel(), int(algo),
+                                              _stream(dev))
+        _lib.check(rc, "c2v_label_dlogits_opts" if angular is None else "c2v_angular_dlogits_opts")
+    return g
+
+
+def loss_argmax_opts(outputs, label, crit, want_grad=False):
+    """loss_argmax with a LossCriterion -> (loss 0-d or [B], argmax [B], maxval [B], d_outputs or None); d_outputs is the
+    gradient for a unit upstream gradient (of the scalar loss, or of every row loss for reduction none)"""
+    lib = _lib.load()
+    sync_deterministic()
+    _need_cuda(outputs, label)
+    B, C = outputs.shape
+    dev = outputs.device
+    outputs = outputs.contiguous()
+    label = _idx(label, "label", (B,))
+    with torch.cuda.device(dev):
+        am = _empty((B,), torch.int64, dev)
+        mx = _empty((B,), torch.float32, dev)
+        loss = _empty(crit.loss_shape(B), torch.float32, dev)
+        dout = torch.empty_like(outputs) if want_grad else None
+        opts = crit.options()
+        rc = lib.c2v_loss_argmax_opts(_ptr(outputs), _ptr(label), B, C, ctypes.byref(opts), _ptr(loss), _ptr(am), _ptr(mx),
+                                      _ptr(dout), _stream(dev))
+        _lib.check(rc, "c2v_loss_argmax_opts")
+    return loss, am, mx, dout
+
+
 def label_topk_supported(dims, B, k):
     return bool(_lib.load().c2v_label_topk_supported(ctypes.byref(dims), int(B), int(k)))
 

@@ -5,7 +5,8 @@ ctypes call per library entry point, the allocations around them -- can set the 
 whole step's kernels with one launch.  These helpers apply torch's capture recipe (warm-up on real batches, capture on
 static inputs, copy in and replay) to a Code2Vec step:
 
-    GraphedTrainStep(model, optimizer, batch_size, max_path_length, loss_fn=None)(starts, paths, ends, label) -> loss
+    GraphedTrainStep(model, optimizer, batch_size, max_path_length, loss_fn=None, criterion=None)(starts, paths, ends,
+                     label) -> loss
     GraphedPredict(model, batch_size, max_path_length, k=None)(starts, paths, ends) -> predict() / predict_topk(k)
 
 What a captured step needs (checked, each with a clear error): dropout keys drawn on the device
@@ -15,7 +16,7 @@ batches.  Hyper-parameters and model.training are fixed at capture.  See INTEGRA
 """
 import torch
 
-from .distributed import FlatAdam, ShardedFlatAdam, ddp_step
+from .distributed import FlatAdam, ShardedFlatAdam, _forward_loss, ddp_step
 
 __all__ = ["GraphedTrainStep", "GraphedPredict"]
 
@@ -49,7 +50,7 @@ class _Graphed:
             return self._run(*inputs)                    # e.g. the ragged last batch of an epoch: eagerly
         if self.graph is not None:
             if self._settings() != self._frozen:
-                raise RuntimeError(f"{type(self).__name__}: hyper-parameters, model.training or "
+                raise RuntimeError(f"{type(self).__name__}: hyper-parameters, the criterion, model.training or "
                                    "torch.are_deterministic_algorithms_enabled() changed since the capture "
                                    f"({self._frozen} -> {self._settings()}); build a new {type(self).__name__}")
             for s, t in zip(self.static_in, inputs):
@@ -81,12 +82,15 @@ class GraphedTrainStep(_Graphed):
       FlatAdam / ShardedFlatAdam (capturable=True): ddp_step (gradients accumulated in the flat bucket);
       any torch optimizer, e.g. torch.optim.Adam(capturable=True): zero_grad(set_to_none=False) + forward + backward +
       step().
-    loss_fn None: the fused loss of Code2Vec.forward_loss; else forward() and loss_fn(outputs, label).
+    loss_fn None: the fused loss of Code2Vec.forward_loss with `criterion` (None, nn.NLLLoss or nn.CrossEntropyLoss);
+    else forward() and loss_fn(outputs, label).  The criterion's type, ignore_index, label_smoothing, reduction and its
+    weight tensor (address and shape) are fixed at capture like the hyper-parameters; the replays read the weight's
+    values, so an in-place change to them (weight.copy_, weight.mul_) takes effect at the next replay.
     The first two [batch_size, max_path_length] calls run eagerly (warm-up on real batches: no extra optimizer step), the
     third captures and replays, later ones copy into the static inputs and replay.  Other shapes run eagerly.  After each
     replay the parameters' version counters are bumped."""
 
-    def __init__(self, model, optimizer, batch_size, max_path_length, loss_fn=None):
+    def __init__(self, model, optimizer, batch_size, max_path_length, loss_fn=None, criterion=None):
         B, L = int(batch_size), int(max_path_length)
         super().__init__(model, ((B, L), (B, L), (B, L), (B,)))
         if isinstance(optimizer, ShardedFlatAdam) and optimizer.world > 1:
@@ -98,7 +102,7 @@ class GraphedTrainStep(_Graphed):
             raise NotImplementedError("GraphedTrainStep: sparse embedding gradients cannot be captured")
         if model.training and model.input_dropout is not None and model._rng_base is None:
             raise RuntimeError("GraphedTrainStep: dropout needs device-drawn keys: call model.use_device_rng() first")
-        self.optimizer, self.loss_fn = optimizer, loss_fn
+        self.optimizer, self.loss_fn, self.criterion = optimizer, loss_fn, criterion
 
     def _settings(self):
         o = self.optimizer
@@ -107,19 +111,22 @@ class GraphedTrainStep(_Graphed):
         else:
             hyper = tuple(tuple((k, v) for k, v in sorted(g.items()) if k != "params" and not isinstance(v, torch.Tensor))
                           for g in o.param_groups)
+        c = self.criterion
+        crit = None if c is None else (type(c), c.ignore_index, getattr(c, "label_smoothing", 0.0), c.reduction,
+                                       None if c.weight is None else (c.weight.data_ptr(), tuple(c.weight.shape)))
         # the deterministic mode selects other kernels and workspace sizes than the captured ones
-        return (self.model.training, torch.are_deterministic_algorithms_enabled(), hyper)
+        return (self.model.training, torch.are_deterministic_algorithms_enabled(), hyper, crit)
 
     def _run(self, starts, paths, ends, label):
         model, opt = self.model, self.optimizer
         if isinstance(opt, FlatAdam):
-            loss = ddp_step(model, opt, opt.bucket, starts, paths, ends, label, self.loss_fn)
+            loss = ddp_step(model, opt, opt.bucket, starts, paths, ends, label, self.loss_fn, self.criterion)
         elif isinstance(opt, ShardedFlatAdam):
-            loss = ddp_step(model, opt, None, starts, paths, ends, label, self.loss_fn)
+            loss = ddp_step(model, opt, None, starts, paths, ends, label, self.loss_fn, self.criterion)
         else:
             opt.zero_grad(set_to_none=False)
             if self.loss_fn is None:
-                loss = model.forward_loss(starts, paths, ends, label)[0]
+                loss = _forward_loss(model, starts, paths, ends, label, self.criterion)
             else:
                 loss = self.loss_fn(model(starts, paths, ends, label)[0], label)
             loss.backward()

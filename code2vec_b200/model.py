@@ -217,6 +217,55 @@ class _LabelLossFn(torch.autograd.Function):
         return d_cv, d_w, d_b, None, None, None, None, None
 
 
+class _LabelLossOptsFn(torch.autograd.Function):
+    """_LabelLossFn with a criterion (functional.LossCriterion: class weights, ignore_index, label smoothing, reduction).
+    The forward leaves the row coefficients the backward needs on the device (coef), so the backward has no host
+    synchronisation; with reduction "none" the loss is [B] and its gradient d_loss [B] goes to the dlogits kernel."""
+
+    @staticmethod
+    def forward(ctx, cv, w_out, b_out, label, dims, algo, cache, angular, crit):
+        params = CF.make_params(w_out=w_out, b_out=b_out)
+        if any(ctx.needs_input_grad[:3]):
+            algo = int(algo) | CF.NO_PDL            # the calls that feed autograd use plain stream-ordered launches
+        loss, lse, am, mx, coef, inv = CF.label_loss_opts(dims, params, cv, label, crit, angular=angular, algo=algo,
+                                                          cache=cache, weight=w_out)
+        ctx.save_for_backward(cv, w_out, b_out, label, lse, coef, inv)
+        ctx.dims, ctx.cache, ctx.algo, ctx.angular, ctx.crit = dims, cache, algo, angular, crit
+        ctx.mark_non_differentiable(am, mx)
+        return loss, am, mx
+
+    @staticmethod
+    def backward(ctx, d_loss, _d_am, _d_mx):
+        cv, w_out, b_out, label, lse, coef, inv = ctx.saved_tensors
+        params = CF.make_params(w_out=w_out, b_out=b_out)
+        need = ctx.needs_input_grad
+        g = CF.label_dlogits_opts(ctx.dims, params, cv, label, lse, coef, ctx.crit, d_loss, inv_norms=inv,
+                                  angular=ctx.angular, algo=ctx.algo, cache=ctx.cache, weight=w_out)
+        bw = dict(algo=int(ctx.algo) & 0xff, cache=ctx.cache, weight=w_out, absmax_ready=True)
+        if ctx.angular is None:
+            d_cv, d_w, d_b = CF.label_backward(ctx.dims, params, cv, g, need[0], need[1], need[2], **bw)
+        else:
+            d_cv, d_w = CF.angular_backward_ws(ctx.dims, params, cv, g, inv, need[0], need[1], **bw)
+            d_b = None
+        return d_cv, d_w, d_b, None, None, None, None, None, None
+
+
+class _LossArgmaxOptsFn(torch.autograd.Function):
+    """_LossArgmaxFn with a criterion (c2v_loss_argmax_opts): the loss is summed in a fixed order"""
+
+    @staticmethod
+    def forward(ctx, outputs, label, crit):
+        loss, am, mx, d_out = CF.loss_argmax_opts(outputs.detach(), label, crit, want_grad=True)
+        ctx.save_for_backward(d_out)
+        ctx.mark_non_differentiable(am, mx)
+        return loss, am, mx
+
+    @staticmethod
+    def backward(ctx, d_loss, _d_am, _d_mx):
+        d_out, = ctx.saved_tensors
+        return d_out * (d_loss[:, None] if d_loss.dim() == 1 else d_loss), None, None
+
+
 class _LossArgmaxFn(torch.autograd.Function):
     """mean NLL of log_softmax + torch.max over materialised logits [B, C] (main.py:251-264, main.py:285) in one library
     call (c2v_loss_argmax), whose d loss / d logits comes out of the same pass.  forward_loss's fallback takes it under
@@ -423,14 +472,26 @@ class Code2Vec(nn.Module):
         return self._head_logits(code_vector, label, dims), code_vector, attention
 
     # -- additive fast path: forward + calculate_loss (main.py:251-264) + torch.max (main.py:285) -----
-    def forward_loss(self, starts, paths, ends, label):
-        """-> (loss, pred_label [b], pred_score [b], code_vector [b,H], attention [b,L]); loss is the mean NLL the
-        reference's `calculate_loss(preds, label, criterion, option)` returns (criterion weights are all
-        1) and is autograd-connected; the [b, C] logits are never written.  Both label heads: with
-        option.angular_margin_loss the loss, arg-max and max are those of the angular-margin logits (model.py:71-80).
-        Shapes the fused kernel does not take, and algo="ffma", fall back to forward()'s head + eager log_softmax / NLL +
-        torch.max; under torch.use_deterministic_algorithms(True) to forward()'s head + c2v_loss_argmax."""
+    def forward_loss(self, starts, paths, ends, label, criterion=None):
+        """-> (loss, pred_label [b], pred_score [b], code_vector [b,H], attention [b,L]); loss is what the
+        reference's `calculate_loss(preds, label, criterion, option)` returns and is autograd-connected; the [b, C] logits
+        are never written.  Both label heads: with option.angular_margin_loss the loss, arg-max and max are those of the
+        angular-margin logits (model.py:71-80).
+        criterion None: the mean NLL of log_softmax with all class weights 1.  Else exactly an nn.NLLLoss (meant, as in
+        the reference, for log_softmax of the logits) or an nn.CrossEntropyLoss, whose weight (fp32 [label_count] on the
+        model's device, else ValueError), ignore_index, reduction and label_smoothing the fused loss honours: the loss is
+        F.cross_entropy(logits, label, weight, ignore_index, reduction, label_smoothing), [b] for reduction "none".  Any
+        other criterion type, subclasses included, raises TypeError.  The weight is read at every call: in-place changes
+        to its values take effect.
+        Shapes the fused kernel does not take, and algo="ffma", fall back to forward()'s head + eager log_softmax / NLL (the
+        criterion itself when given) + torch.max; under torch.use_deterministic_algorithms(True) to forward()'s head +
+        c2v_loss_argmax (c2v_loss_argmax_opts with a criterion)."""
+        crit = None
+        if criterion is not None:
+            crit = CF.LossCriterion(criterion, self.option.label_count, self._head()[0].device)
         code_vector, attention, dims = self._encode(starts, paths, ends)
+        if crit is not None:
+            return self._forward_loss_criterion(code_vector, attention, dims, label, criterion, crit)
         if self.algo != _lib.ALGO_FFMA and CF.label_loss_supported(dims, code_vector.shape[0]):
             o = self.option
             angular = (o.angular_margin, o.inverse_temp) if o.angular_margin_loss else None
@@ -440,6 +501,21 @@ class Code2Vec(nn.Module):
             loss, am, mx = _LossArgmaxFn.apply(self._head_logits(code_vector, label, dims), label)
         else:
             loss, am, mx = self._eager_loss(self._head_logits(code_vector, label, dims), label)
+        return loss, am, mx, code_vector, attention
+
+    def _forward_loss_criterion(self, code_vector, attention, dims, label, criterion, crit):
+        """forward_loss's head with a criterion: fused, deterministic library fallback, or the criterion itself"""
+        if self.algo != _lib.ALGO_FFMA and CF.label_loss_supported(dims, code_vector.shape[0]):
+            o = self.option
+            angular = (o.angular_margin, o.inverse_temp) if o.angular_margin_loss else None
+            loss, am, mx = _LabelLossOptsFn.apply(code_vector, *self._head(), label, dims, self._label_algo, self._lab_cache,
+                                                  angular, crit)
+        elif torch.are_deterministic_algorithms_enabled():
+            loss, am, mx = _LossArgmaxOptsFn.apply(self._head_logits(code_vector, label, dims), label, crit)
+        else:
+            outputs = self._head_logits(code_vector, label, dims)
+            loss = criterion(F.log_softmax(outputs, dim=1) if type(criterion) is nn.NLLLoss else outputs, label)
+            mx, am = torch.max(outputs.detach(), dim=1)
         return loss, am, mx, code_vector, attention
 
     # -- additive convenience (the reference does torch.max(preds, dim=1) at main.py:285) ----

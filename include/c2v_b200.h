@@ -267,6 +267,51 @@ int c2v_angular_dlogits(const c2v_dims *d, const c2v_params *p, const float *cod
  *   d_code_vector[b] = (G . W)[b] - icv[b]^2 (cv[b] . (G . W)[b]) cv[b]   [B, H]
  *   d_output_weight[c] = (G^T . cv)[c] - iw[c]^2 (W[c] . (G^T . cv)[c]) W[c]   [C, H]   (either may be NULL).
  * Same workspace / algo rules (and CUDA-core fallback) as c2v_label_backward_ws. */
+/* Criterion options of the fused loss: the criterion is
+ *   F.cross_entropy(logits, label, weight, ignore_index, reduction, label_smoothing = eps)
+ * on the logits of the head (nn.NLLLoss(weight, ignore_index, reduction) on log_softmax of them is the case eps = 0).
+ * With w_y = weight[label_i] (1 without weights; 0 for an ignored row), den = sum_i w_y, lse_i = logsumexp_j z_ij:
+ *   row_i = (1 - eps) w_y (lse_i - z_i,y) + (eps / C) sum_j w_j (lse_i - z_ij)      (0 for ignored rows)
+ *   mean: sum_i row_i / den (NaN when every row is ignored)   sum: sum_i row_i   none: row_i [B]
+ *   d loss / d z_ij = u_i [ (1 - eps) w_y (p_ij - [j == y]) + (eps / C) (W p_ij - w_j) ],  W = sum_j w_j
+ * u_i: the upstream gradient (d_loss / den for mean, d_loss for sum, row_grad[i] for none), 0 for ignored rows.
+ * A label outside [0, C) that is not ignore_index gives a NaN row, as without options.
+ *   class_weight: fp32 [C] on the device (4-byte aligned) or NULL; label_smoothing in [0, 1]; reduction C2V_REDUCTION_*;
+ *   row_grad: fp32 [B] on the device, the dlogits calls with reduction none only (C2V_EINVAL there without it).
+ * The _opts entry points take the arguments of the call they extend plus the options and
+ *   coef: fp32 [2 B + 1] on the device, the row coefficients the loss call writes and the dlogits call reads (so that the
+ *   backward needs no host synchronisation);
+ *   loss: a scalar for mean / sum, [B] for none.
+ * options == NULL is exactly the call without options (coef unused).  The fused loss calls with options need
+ * c2v_label_loss_opts_workspace_bytes of workspace (the label workspace plus the options' partials); the dlogits calls
+ * take the label workspace.  Every check of the options runs before any CUDA call. */
+#define C2V_REDUCTION_MEAN 0
+#define C2V_REDUCTION_SUM 1
+#define C2V_REDUCTION_NONE 2
+typedef struct c2v_loss_options {
+    const float *class_weight;
+    int64_t ignore_index;
+    float label_smoothing;
+    int32_t reduction;
+    const float *row_grad;
+} c2v_loss_options;
+size_t c2v_label_loss_opts_workspace_bytes(const c2v_dims *d, int32_t B);
+int c2v_label_loss_argmax_opts(const c2v_dims *d, const c2v_params *p, const float *code_vector, const int64_t *label,
+                               int32_t B, const c2v_loss_options *options, float *outputs, float *loss, float *lse,
+                               float *coef, int64_t *argmax, float *maxval, void *workspace, size_t workspace_bytes,
+                               int32_t algo, void *stream);
+int c2v_label_dlogits_opts(const c2v_dims *d, const c2v_params *p, const float *code_vector, const int64_t *label,
+                           const float *lse, const float *coef, int32_t B, const c2v_loss_options *options, float scale,
+                           const float *scale_device, float *d_outputs, void *workspace, size_t workspace_bytes,
+                           int32_t algo, void *stream);
+int c2v_angular_loss_argmax_opts(const c2v_dims *d, const c2v_params *p, const float *code_vector, const int64_t *label,
+                                 int32_t B, float margin, float inverse_temp, const c2v_loss_options *options,
+                                 float *outputs, float *loss, float *lse, float *coef, int64_t *argmax, float *maxval,
+                                 float *inv_norms, void *workspace, size_t workspace_bytes, int32_t algo, void *stream);
+int c2v_angular_dlogits_opts(const c2v_dims *d, const c2v_params *p, const float *code_vector, const int64_t *label,
+                             const float *lse, const float *coef, const float *inv_norms, int32_t B, float margin,
+                             float inverse_temp, const c2v_loss_options *options, float scale, const float *scale_device,
+                             float *d_dot, void *workspace, size_t workspace_bytes, int32_t algo, void *stream);
 int c2v_angular_backward_ws(const c2v_dims *d, const c2v_params *p, const float *code_vector, const float *d_dot,
                             const float *inv_norms, int32_t B, float *d_code_vector, float *d_output_weight, void *workspace,
                             size_t workspace_bytes, int32_t algo, void *stream);
@@ -347,6 +392,12 @@ int c2v_knn_pairs(const float *bank, int64_t N, int32_t H, const float *queries,
  * dLoss/doutputs = (softmax - onehot) / B. */
 int c2v_loss_argmax(const float *outputs, const int64_t *label, int32_t B, int64_t C,
                     float *loss, int64_t *argmax, float *maxval, float *d_outputs, void *stream);
+/* The same with criterion options (c2v_loss_options; row_grad is not read): loss is a scalar for mean / sum, [B] for
+ * none; d_outputs receives d loss / d outputs for a unit upstream gradient (of the scalar loss, or of every row loss for
+ * none).  The loss is summed in a fixed order in every mode.  options == NULL is exactly c2v_loss_argmax. */
+int c2v_loss_argmax_opts(const float *outputs, const int64_t *label, int32_t B, int64_t C,
+                         const c2v_loss_options *options, float *loss, int64_t *argmax, float *maxval, float *d_outputs,
+                         void *stream);
 
 /* ---- backward ----------------------------------------------------------------------
  * Label head: d_cv = d_out . W_out ; dW_out = d_out^T . cv ; d_bias = sum_b d_out. */
