@@ -16,6 +16,10 @@ TOPK_MAX = 16                # C2V_TOPK_MAX: the largest k of the fused top-k (c
 KNN_EXCLUDE_MAX = 4          # C2V_KNN_EXCLUDE_MAX: excluded bank rows per query of c2v_knn_topk / c2v_knn_pairs
 KNN_MAX_Q = 2048             # queries per c2v_knn_* call
 DROPOUT_SEED_ON_DEVICE = 2   # C2V_DROPOUT_SEED_ON_DEVICE: c2v_dropout.seed is the device address of the key
+# c2v_eval_accumulate's counters (C2V_EVAL_*): n, skipped, k rank hits, then tp, fp, fn and the fixed-point sums
+EVAL_N, EVAL_SKIPPED, EVAL_RANK_HITS = 0, 1, 2
+EVAL_TP, EVAL_FP, EVAL_FN, EVAL_PREC_FX, EVAL_REC_FX, EVAL_F1_FX = range(6)   # offsets behind the k rank hits: 2 + k + i
+EVAL_SCALARS = 8             # C2V_EVAL_COUNTERS(k) = EVAL_SCALARS + k
 
 c_i32, c_i64, c_f32, c_vp, c_sz = ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_void_p, ctypes.c_size_t
 
@@ -191,6 +195,7 @@ SYMBOLS = {
     "c2v_vectors_get_info": (ctypes.c_int, [c_vp, _P(VectorsInfo)]),
     "c2v_vectors_export": (ctypes.c_int, [c_vp, c_vp, c_vp, c_vp]),
     "c2v_vectors_free": (None, [c_vp]),
+    "c2v_eval_accumulate": (ctypes.c_int, [c_vp, c_vp, c_i32, c_i32, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "c2v_knn_prep_workspace_bytes": (c_sz, [c_i64, c_i32]),
     "c2v_knn_prepare": (ctypes.c_int, [c_vp, c_i64, c_i32, c_vp, c_sz, c_vp]),
     "c2v_knn_topk_workspace_bytes": (c_sz, [c_i64, c_i32, c_i32, c_i32]),

@@ -399,6 +399,41 @@ int c2v_loss_argmax_opts(const float *outputs, const int64_t *label, int32_t B, 
                          const c2v_loss_options *options, float *loss, int64_t *argmax, float *maxval, float *d_outputs,
                          void *stream);
 
+/* ---- evaluation metrics (main.py:267-297: the eval pass's accuracy / precision / recall / F1) ------------------------
+ * Adds one batch's counts into counters and class_counts (never overwrites them; the caller zero-fills once).
+ *   label int64 [B], pred int64 [B, k] (best first; k = 1 is torch.max(dim=1)), all on the device.
+ *   subtoken table of the C labels: label c's subtokens are subtoken_ids[subtoken_offsets[c] .. subtoken_offsets[c+1])
+ *   (int32 ids of interned strings, duplicates kept; subtoken_offsets int64 [C + 1], non-decreasing, from 0; fewer than
+ *   2^31 entries in all).
+ * A row whose label is outside [0, C) (-1: unlabelled, an ignore_index such as -100) only adds 1 to `skipped`.  For every
+ * other row (n), with E = the label's list and P = the list of pred[.., 0] (empty when that prediction is outside
+ * [0, C)):
+ *   rank hit j: the first j < k with pred[.., j] == label (no hit when there is none);
+ *   tp = entries of P that occur in E, fp = |P| - tp, fn = entries of E that do not occur in P;
+ *   fixed-point sums (units of 2^-32, as unsigned 64-bit sums): floor(tp 2^32 / (tp + fp)),
+ *   floor(tp 2^32 / (tp + fn)), floor(2 tp 2^32 / (2 tp + fp + fn)), each 0 when its denominator is 0;
+ *   class_counts int64 [3, C]: true[label] += 1, pred[pred[.., 0]] += 1 when inside [0, C), hit[label] += 1 when
+ *   pred[.., 0] == label.
+ * counters int64 [C2V_EVAL_COUNTERS(k)]: the layout below.  Integer atomics only: the counts do not depend on the batch
+ * split, row order or launch order, and the call reads nothing on the host (capturable into a CUDA graph).
+ * C2V_EINVAL, naming the argument, before any CUDA call: a NULL pointer, B < 1, C < 1, k < 1 or k > C. */
+#define C2V_EVAL_N 0                         /* counted rows                                                   */
+#define C2V_EVAL_SKIPPED 1                   /* rows with a label outside [0, C)                               */
+#define C2V_EVAL_RANK_HITS 2                 /* k counters: rows whose label is first found at rank j          */
+#define C2V_EVAL_TP(k) (2 + (k))             /* subtoken true positives                                        */
+#define C2V_EVAL_FP(k) (3 + (k))             /* subtoken false positives                                       */
+#define C2V_EVAL_FN(k) (4 + (k))             /* subtoken false negatives                                       */
+#define C2V_EVAL_PREC_FX(k) (5 + (k))        /* sum of per-row precision, units of 2^-32                       */
+#define C2V_EVAL_REC_FX(k) (6 + (k))         /* sum of per-row recall                                          */
+#define C2V_EVAL_F1_FX(k) (7 + (k))          /* sum of per-row F1                                              */
+#define C2V_EVAL_COUNTERS(k) (8 + (k))
+#define C2V_EVAL_CLASS_TRUE 0                /* rows of class_counts                                           */
+#define C2V_EVAL_CLASS_PRED 1
+#define C2V_EVAL_CLASS_HIT 2
+int c2v_eval_accumulate(const int64_t *label, const int64_t *pred, int32_t B, int32_t k, int64_t C,
+                        const int64_t *subtoken_offsets, const int32_t *subtoken_ids, int64_t *counters,
+                        int64_t *class_counts, void *stream);
+
 /* ---- backward ----------------------------------------------------------------------
  * Label head: d_cv = d_out . W_out ; dW_out = d_out^T . cv ; d_bias = sum_b d_out. */
 int c2v_label_backward(const c2v_dims *d, const c2v_params *p, const float *code_vector,
