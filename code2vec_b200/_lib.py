@@ -16,6 +16,7 @@ TOPK_MAX = 16                # C2V_TOPK_MAX: the largest k of the fused top-k (c
 KNN_EXCLUDE_MAX = 4          # C2V_KNN_EXCLUDE_MAX: excluded bank rows per query of c2v_knn_topk / c2v_knn_pairs
 KNN_MAX_Q = 2048             # queries per c2v_knn_* call
 DROPOUT_SEED_ON_DEVICE = 2   # C2V_DROPOUT_SEED_ON_DEVICE: c2v_dropout.seed is the device address of the key
+MATMUL_IEEE, MATMUL_TF32 = 0, 1   # C2V_MATMUL_*: modes of c2v_set_matmul_precision
 # c2v_eval_accumulate's counters (C2V_EVAL_*): n, skipped, k rank hits, then tp, fp, fn and the fixed-point sums
 EVAL_N, EVAL_SKIPPED, EVAL_RANK_HITS = 0, 1, 2
 EVAL_TP, EVAL_FP, EVAL_FN, EVAL_PREC_FX, EVAL_REC_FX, EVAL_F1_FX = range(6)   # offsets behind the k rank hits: 2 + k + i
@@ -179,6 +180,8 @@ SYMBOLS = {
     "c2v_launch_count": (c_i64, []),
     "c2v_set_deterministic": (ctypes.c_int, [c_i32]),
     "c2v_get_deterministic": (ctypes.c_int, []),
+    "c2v_set_matmul_precision": (ctypes.c_int, [c_i32]),
+    "c2v_get_matmul_precision": (ctypes.c_int, []),
     "c2v_profile_enable": (ctypes.c_int, [c_i32]),
     "c2v_profile_read": (ctypes.c_int, [_P(ctypes.c_double), _P(c_i64)]),
     "c2v_corpus_parse_buffer": (ctypes.c_int, [ctypes.c_char_p, c_sz, c_i32, _P(c_vp)]),

@@ -18,6 +18,8 @@ bool pdl_enabled()
 }
 static thread_local char g_err[512] = "";
 thread_local bool g_pdl_this_call = true;
+static thread_local int g_matmul = C2V_MATMUL_IEEE;
+bool matmul_tf32() { return g_matmul == C2V_MATMUL_TF32; }
 
 void set_error(const char *fmt, ...)
 {
@@ -194,6 +196,18 @@ int c2v_set_deterministic(int32_t on)
 }
 
 int c2v_get_deterministic(void) { return deterministic() ? 1 : 0; }
+
+int c2v_set_matmul_precision(int32_t mode)
+{
+    if (mode != C2V_MATMUL_IEEE && mode != C2V_MATMUL_TF32) {
+        set_error("c2v_set_matmul_precision: mode %d is neither C2V_MATMUL_IEEE (0) nor C2V_MATMUL_TF32 (1)", (int)mode);
+        return C2V_EINVAL;
+    }
+    g_matmul = mode;
+    return C2V_OK;
+}
+
+int c2v_get_matmul_precision(void) { return g_matmul; }
 const char *c2v_last_error(void) { return g_err; }
 int64_t c2v_launch_count(void) { return __atomic_load_n(&g_launches, __ATOMIC_RELAXED); }
 

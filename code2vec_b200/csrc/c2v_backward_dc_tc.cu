@@ -8,8 +8,9 @@
 // A = dX, K-major: the same [128 rows x 64 h] fp16 128-byte-swizzled hi/lo panels the dW kernel builds
 // (c2v_backward_dw_tc.cu), read here with K-major descriptors.  B = W^T as a K-major image [128 d x 64 h] per
 // (sub-vector, k-block), built once per call by split_wt_kernel and streamed from L2 with 32 KB cp.async.bulk copies.
-// 3-pass fp16 hi/lo split, fp32 accumulation in registers; dX is pre-scaled by the power of two from max |dx|, W by the
-// one from max |W|.
+// 3-pass fp16 hi/lo split in both matmul precisions (C2V_MATMUL_TF32 gains nothing here: the kernel is bound by its
+// scatter into the embedding gradients, not by the tensor pipe), fp32 accumulation in registers; dX is pre-scaled by
+// the power of two from max |dx|, W by the one from max |W|.
 //
 // Warps: 0-7 two consumer warpgroups (warpgroup g: rows 64g .. 64g+63 of the tile; m64n128 wgmma into registers, then
 // the scatter straight from the accumulator fragments with vector atomics into the embedding rows) | 8-15 dX producers |

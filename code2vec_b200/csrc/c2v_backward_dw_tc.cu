@@ -9,7 +9,7 @@
 // kernels build (one 128-byte line per row); only the descriptors change: transposed operands, LBO = stride between
 // 64-column panels, SBO = 1024 B between 8-row groups, and a K step of 16 rows advances the start address by 2 KB.  Same
 // 3-pass fp16 hi/lo split as everywhere else (dX and C are fp32; fp32 accumulation), so the result matches the fp32 GEMM
-// to ~1e-6 relative.
+// to ~1e-6 relative (one pass under C2V_MATMUL_TF32).
 //
 // One persistent CTA per SM and window walks 128-row tiles and keeps its partial dW [128 h x 128 d] in the registers of
 // two consumer warpgroups (warpgroup g: h panel g, two m64n64 accumulators) for the whole launch; at the end they add it
@@ -40,8 +40,9 @@ constexpr int SMEM_A_OFF = 0, SMEM_B_OFF = 2 * A_STAGE, SMEM_BAR_OFF = SMEM_B_OF
 constexpr int SMEM_BYTES = SMEM_BAR_OFF + 128 + 1024;
 }  // namespace dwt
 
-// DET (deterministic mode): dW is the slab array [gridDim.x][H][3E]; CTA x stores its window of the partial to slab x
-template <bool DET = false>
+// DET (deterministic mode): dW is the slab array [gridDim.x][H][3E]; CTA x stores its window of the partial to slab x.
+// PASS = OnePass (C2V_MATMUL_TF32): hi.hi only, and the producers store no lo panels.
+template <bool DET = false, class PASS = ThreePass>
 __global__ void __launch_bounds__(dwt::THREADS, 1)
 backward_dw_tc_kernel(const EncodeArgs a, const float *__restrict__ dx, const unsigned *__restrict__ dx_absmax,
                       float *__restrict__ dW, const int n_db)
@@ -103,7 +104,7 @@ backward_dw_tc_kernel(const EncodeArgs a, const float *__restrict__ dx, const un
                 const __half2 l01 = __floats2half2_rn(v.x - f01.x, v.y - f01.y);
                 const __half2 l23 = __floats2half2_rn(v.z - f23.x, v.w - f23.y);
                 sts_v2(hi + st_off[j], pack_h2(h01), pack_h2(h23));
-                sts_v2(lo + st_off[j], pack_h2(l01), pack_h2(l23));
+                if constexpr (!one_pass<PASS>) sts_v2(lo + st_off[j], pack_h2(l01), pack_h2(l23));
             }
         };
         const int E4 = a.Et / 4, H4 = a.H / 4;        // row lengths in 16-byte pieces (columns beyond them are zero padding)
@@ -193,6 +194,7 @@ backward_dw_tc_kernel(const EncodeArgs a, const float *__restrict__ dx, const un
                     const uint64_t b_hi = wgmma_desc_mn(sb + k * 2048, dwt::PANEL);
                     const uint64_t b_lo = wgmma_desc_mn(sb + dwt::PANEL + k * 2048, dwt::PANEL);
                     wgmma_m64n64<1, 1>(acc[kb], a_hi, b_hi, (tl | k) != 0);
+                    if constexpr (one_pass<PASS>) continue;
                     wgmma_m64n64<1, 1>(acc[kb], a_lo, b_hi, 1);
                     wgmma_m64n64<1, 1>(acc[kb], a_hi, b_lo, 1);
                 }
@@ -242,7 +244,8 @@ int launch_backward_dw_tc(const EncodeArgs &a_in, const float *dx, const unsigne
     int dev = 0, sms = 0;
     C2V_CUDA_OK(cudaGetDevice(&dev));
     C2V_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    auto kern = dw_slabs ? backward_dw_tc_kernel<true> : backward_dw_tc_kernel<false>;
+    auto kern = matmul_tf32() ? (dw_slabs ? backward_dw_tc_kernel<true, OnePass> : backward_dw_tc_kernel<false, OnePass>)
+                              : (dw_slabs ? backward_dw_tc_kernel<true> : backward_dw_tc_kernel<false>);
     C2V_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, dwt::SMEM_BYTES));
     const int n_hb = (a.H + dwt::H - 1) / dwt::H, n_db = (a.Et + dwt::E - 1) / dwt::E;
     int grid = sms / (3 * n_hb * n_db);                    // one CTA per SM over all windows

@@ -153,6 +153,9 @@ int launch_row_bag(const long long *bag_off, int B, long long N, int *row_bag, c
 // order instead of through atomics (c2v_deterministic.cu)
 // ---------------------------------------------------------------------------------
 bool deterministic();
+// matmul precision (c2v_set_matmul_precision, per host thread): true under C2V_MATMUL_TF32, where the tensor-core GEMMs of
+// the encode, its backward and the label head launch their OnePass instantiations (c2v_tc_ptx.cuh)
+bool matmul_tf32();
 constexpr int kDetSlabs = 64;          // per-CTA partial slabs of dW (tensor-core CTAs per window / CUDA-core row splits)
 constexpr int kDetRowSlabs = 512;      // per-CTA partials of d attention / d gamma / d beta (caps the row kernels' grids)
 constexpr int kDetLabelSplits = 32;    // label splits of d code_vector on the tensor cores

@@ -5,8 +5,9 @@
 // Numerics.  The reference contraction x = c . W^T is fp32; plain TF32/BF16 miss the 1e-4 parity bar.
 // Both operands are split into fp16 hi + fp16 lo (a = a_hi + a_lo exactly to ~2^-22) and three f16 MMAs with fp32
 // accumulation are issued per k-step:  a_hi.w_hi + a_lo.w_hi + a_hi.w_lo  (the dropped a_lo.w_lo term is 2^-22
-// relative).  W is pre-multiplied by a power of two so its lo part stays out of the fp16 subnormals; the epilogue folds
-// the exact inverse into the LayerNorm scale.
+// relative).  Under C2V_MATMUL_TF32 the OnePass instantiations issue a_hi.w_hi alone (TF32-class).  W is pre-multiplied
+// by a power of two so its lo part stays out of the fp16 subnormals; the epilogue folds the exact inverse into the
+// LayerNorm scale.
 //
 // Shapes: terminal_embed == path_embed = E, E % 4 == 0; (E <= 128 and encode_size in {100, 128}) or (E <= 256 and
 // encode_size == 256).  Every sub-vector is padded to EP = 128 (256) k and the encode size to HP = 128 (256) n.
@@ -133,7 +134,9 @@ int launch_split_w_tcgen05(const c2v_dims *d, const float *W, EncodeWorkspace &w
 // ------------------------------------------------------------------------------------
 // the kernel
 // ------------------------------------------------------------------------------------
-template <bool DROPOUT, int HV, bool PACKED = false, bool SEED_DEV = false>
+// PASS: ThreePass (fp32-accurate) or OnePass (C2V_MATMUL_TF32: a_hi.w_hi only; the A producers store no lo tile and the
+// W producer copies only the hi tile of each k-block of the image)
+template <bool DROPOUT, int HV, bool PACKED = false, bool SEED_DEV = false, class PASS = ThreePass>
 __global__ void __launch_bounds__(WgCfg<(HV > 128)>::THREADS, 1)
 encode_wgmma_kernel(const EncodeArgs a)
 {
@@ -193,6 +196,7 @@ encode_wgmma_kernel(const EncodeArgs a)
                     const int first = (kb | k) == 0;
                     wgmma_m64n128<0>(acc, a_hi, w_hi, !first);
                     if (WIDE) wgmma_m64n128<64 % C::NACC>(acc, a_hi, w_hi + (16384 >> 4), !first);
+                    if constexpr (one_pass<PASS>) continue;
                     wgmma_m64n128<0>(acc, a_lo, w_hi, 1);
                     if (WIDE) wgmma_m64n128<64 % C::NACC>(acc, a_lo, w_hi + (16384 >> 4), 1);
                     wgmma_m64n128<0>(acc, a_hi, w_lo, 1);
@@ -362,6 +366,7 @@ encode_wgmma_kernel(const EncodeArgs a)
                     const __half2 h01 = __floats2half2_rn(v.x, v.y), h23 = __floats2half2_rn(v.z, v.w);
                     const float2 f01 = __half22float2(h01), f23 = __half22float2(h23);
                     sts_v2(a_hi + so, pack_h2(h01), pack_h2(h23));
+                    if constexpr (one_pass<PASS>) continue;
                     sts_v2(a_lo + so, pack_h2(__floats2half2_rn(v.x - f01.x, v.y - f01.y)),
                            pack_h2(__floats2half2_rn(v.z - f23.x, v.w - f23.y)));
                 }
@@ -379,9 +384,10 @@ encode_wgmma_kernel(const EncodeArgs a)
             for (int it = 0; it < n_items; ++it) {
                 const int stage = it % C::STAGES;
                 mbar_wait(bar_empty + 8 * stage, ((uint32_t)(it / C::STAGES) & 1u) ^ 1u, status);
-                mbar_arrive_expect_tx(bar_full + 8 * stage, C::W_KB_BYTES);
-                bulk_copy_g2s(base + stage * C::STAGE_BYTES + 2 * C::A_TILE, img + (size_t)kb * C::W_KB_BYTES,
-                              C::W_KB_BYTES, bar_full + 8 * stage);
+                constexpr uint32_t bytes = one_pass<PASS> ? C::W_TILE : C::W_KB_BYTES;     // hi tile first in the image
+                mbar_arrive_expect_tx(bar_full + 8 * stage, bytes);
+                bulk_copy_g2s(base + stage * C::STAGE_BYTES + 2 * C::A_TILE, img + (size_t)kb * C::W_KB_BYTES, bytes,
+                              bar_full + 8 * stage);
                 if (++kb == C::NKB) kb = 0;
             }
         }
@@ -404,26 +410,32 @@ static int launch_wg(void (*kern)(const EncodeArgs), const EncodeArgs &a, cudaSt
     return C2V_OK;
 }
 
-template <bool PACKED>
+template <bool PACKED, class PASS>
 static int launch_encode_wg(const EncodeArgs &a, cudaStream_t st)
 {
     const bool drop = a.drop_p > 0.0f, dev_key = drop && a.seed_dev;
     if (a.H == 256)
-        return launch_wg<true>(dev_key ? encode_wgmma_kernel<true, 256, PACKED, true>
-                               : drop ? encode_wgmma_kernel<true, 256, PACKED> : encode_wgmma_kernel<false, 256, PACKED>, a, st);
+        return launch_wg<true>(dev_key ? encode_wgmma_kernel<true, 256, PACKED, true, PASS>
+                               : drop ? encode_wgmma_kernel<true, 256, PACKED, false, PASS>
+                                      : encode_wgmma_kernel<false, 256, PACKED, false, PASS>, a, st);
     if (a.H == 128)
-        return launch_wg<false>(dev_key ? encode_wgmma_kernel<true, 128, PACKED, true>
-                                : drop ? encode_wgmma_kernel<true, 128, PACKED> : encode_wgmma_kernel<false, 128, PACKED>, a, st);
+        return launch_wg<false>(dev_key ? encode_wgmma_kernel<true, 128, PACKED, true, PASS>
+                                : drop ? encode_wgmma_kernel<true, 128, PACKED, false, PASS>
+                                       : encode_wgmma_kernel<false, 128, PACKED, false, PASS>, a, st);
     if (a.H == 100)
-        return launch_wg<false>(dev_key ? encode_wgmma_kernel<true, 100, PACKED, true>
-                                : drop ? encode_wgmma_kernel<true, 100, PACKED> : encode_wgmma_kernel<false, 100, PACKED>, a, st);
+        return launch_wg<false>(dev_key ? encode_wgmma_kernel<true, 100, PACKED, true, PASS>
+                                : drop ? encode_wgmma_kernel<true, 100, PACKED, false, PASS>
+                                       : encode_wgmma_kernel<false, 100, PACKED, false, PASS>, a, st);
     set_error("encode_wgmma_kernel: encode_size %d not supported (100, 128 or 256)", a.H);
     return C2V_EUNSUPPORTED;
 }
 
+// the matmul precision of the calling host thread picks the instantiations (c2v_set_matmul_precision)
 int launch_encode_tcgen05(const EncodeArgs &a, cudaStream_t st)
 {
-    return a.bag_off ? launch_encode_wg<true>(a, st) : launch_encode_wg<false>(a, st);
+    if (matmul_tf32())
+        return a.bag_off ? launch_encode_wg<true, OnePass>(a, st) : launch_encode_wg<false, OnePass>(a, st);
+    return a.bag_off ? launch_encode_wg<true, ThreePass>(a, st) : launch_encode_wg<false, ThreePass>(a, st);
 }
 
 }  // namespace c2v

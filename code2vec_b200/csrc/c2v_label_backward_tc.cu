@@ -5,7 +5,7 @@
 //   LB2  d_cv[b, h]   = sum_c G[b, c] W_out[c, h]   M = b, N = h, K = c : A K-major (G rows), B MN-major = the forward's
 //        cached W_out image ([128 c x 64 h] fp16 hi/lo tiles) streamed as it is with cp.async.bulk
 // Same fp32-accurate scheme as everywhere: operands split into fp16 hi + lo, three f16 MMAs per k-step
-// (hi.hi + lo.hi + hi.lo), fp32 accumulation in registers; G is multiplied by the power of two that lifts max |G| just
+// (hi.hi + lo.hi + hi.lo; hi.hi alone under C2V_MATMUL_TF32), fp32 accumulation in registers; G is multiplied by the power of two that lifts max |G| just
 // below 2^14 before the split (mean-NLL gradients are ~1e-6) and the result by its exact inverse.
 // The shared-memory image of a G tile is identical for both kernels ([128 rows(b) x 64 cols(c)] 128-byte-swizzled
 // panels); only the descriptors differ (MN-major in LB1, K-major in LB2).
@@ -51,12 +51,13 @@ __device__ __forceinline__ float4 lbt_load4(const float *p, long long remaining,
     if (remaining > 3) v.w = __ldg(p + 3);
     return v;
 }
+template <class PASS>
 __device__ __forceinline__ void lbt_split_store(uint32_t hi, uint32_t lo, uint32_t off, float4 v) {
     const __half2 h01 = __floats2half2_rn(v.x, v.y), h23 = __floats2half2_rn(v.z, v.w);
     const float2 f01 = __half22float2(h01), f23 = __half22float2(h23);
     const __half2 l01 = __floats2half2_rn(v.x - f01.x, v.y - f01.y), l23 = __floats2half2_rn(v.z - f23.x, v.w - f23.y);
     sts_v2(hi + off, pack_h2(h01), pack_h2(h23));
-    sts_v2(lo + off, pack_h2(l01), pack_h2(l23));
+    if constexpr (!one_pass<PASS>) sts_v2(lo + off, pack_h2(l01), pack_h2(l23));     // OnePass: no lo half
 }
 
 __global__ void lbt_absmax_kernel(const float *__restrict__ x, long long n, unsigned *__restrict__ out_bits)
@@ -85,7 +86,8 @@ constexpr int SMEM_BYTES = SMEM_BAR_OFF + 128 + 1024;
 // same step left in the label workspace ([128 bags x 64 h] K-major 128-byte-swizzled tiles = the very bytes an MN-major B
 // tile of this GEMM needs), streamed by warp 16 with one 32 KB cp.async.bulk per (batch tile, k-block); the producers then
 // only handle G.
-template <bool CV_IMG, int NKB>
+// PASS = OnePass (C2V_MATMUL_TF32): hi.hi only; no lo panels are stored or copied.
+template <bool CV_IMG, int NKB, class PASS = ThreePass>
 __global__ void __launch_bounds__(lbt::THREADS, 1)
 label_dw_tc_kernel(const float *__restrict__ G, const float *__restrict__ cv, int B, long long C, int H,
                    const unsigned *__restrict__ g_absmax, float *__restrict__ dW, float *__restrict__ d_bias,
@@ -149,7 +151,7 @@ label_dw_tc_kernel(const float *__restrict__ G, const float *__restrict__ cv, in
                         float4 v = g[j];
                         cs[p].x += v.x; cs[p].y += v.y; cs[p].z += v.z; cs[p].w += v.w;
                         v.x *= g_scale; v.y *= g_scale; v.z *= g_scale; v.w *= g_scale;
-                        lbt_split_store(hi, lo, lbt_st_off(pw * lbt::ROWS_PER_PW + 2 * j + sub_row, q), v);
+                        lbt_split_store<PASS>(hi, lo, lbt_st_off(pw * lbt::ROWS_PER_PW + 2 * j + sub_row, q), v);
                     }
                     fence_proxy_async_smem();
                     __syncwarp();
@@ -170,7 +172,7 @@ label_dw_tc_kernel(const float *__restrict__ G, const float *__restrict__ cv, in
                     const uint32_t hi = base + lb1::SMEM_B_OFF + bs * lb1::B_SLOT;
 #pragma unroll
                     for (int j = 0; j < lbt::LD; ++j)
-                        lbt_split_store(hi, hi + lbt::PANEL, lbt_st_off(pw * lbt::ROWS_PER_PW + 2 * j + sub_row, q), buf[j]);
+                        lbt_split_store<PASS>(hi, hi + lbt::PANEL, lbt_st_off(pw * lbt::ROWS_PER_PW + 2 * j + sub_row, q), buf[j]);
                     fence_proxy_async_smem();
                     __syncwarp();
                     if (lane == 0) mbar_arrive(bar_bfull + 8 * bs);
@@ -205,9 +207,10 @@ label_dw_tc_kernel(const float *__restrict__ G, const float *__restrict__ cv, in
                     for (int kb = 0; kb < NKB; ++kb, ++itb) {
                         const int bs = itb & 1;
                         mbar_wait(bar_bempty + 8 * bs, (((uint32_t)(itb >> 1)) & 1u) ^ 1u, status);
-                        mbar_arrive_expect_tx(bar_bfull + 8 * bs, lb1::B_SLOT);
+                        constexpr uint32_t bytes = one_pass<PASS> ? lbt::PANEL : lb1::B_SLOT;     // hi first in the image
+                        mbar_arrive_expect_tx(bar_bfull + 8 * bs, bytes);
                         bulk_copy_g2s(base + lb1::SMEM_B_OFF + bs * lb1::B_SLOT, cv_img + ((size_t)bt * NKB + kb) * lb1::B_SLOT,
-                                      lb1::B_SLOT, bar_bfull + 8 * bs);
+                                      bytes, bar_bfull + 8 * bs);
                     }
         }
         __syncwarp();
@@ -236,6 +239,7 @@ label_dw_tc_kernel(const float *__restrict__ G, const float *__restrict__ cv, in
                         const uint64_t b_hi = wgmma_desc_mn(sb + k * 2048, lbt::PANEL);
                         const uint64_t b_lo = wgmma_desc_mn(sb + lbt::PANEL + k * 2048, lbt::PANEL);
                         wgmma_m64n64<1, 1>(acc[kb], a_hi, b_hi, (bt | k) != 0);
+                        if constexpr (one_pass<PASS>) continue;
                         wgmma_m64n64<1, 1>(acc[kb], a_lo, b_hi, 1);
                         wgmma_m64n64<1, 1>(acc[kb], a_hi, b_lo, 1);
                     }
@@ -284,8 +288,9 @@ constexpr int SMEM_A_OFF = 0;
 static inline int lb2_stages(int nkb) { return nkb <= 2 ? 3 : 2; }
 static inline int lb2_smem_bytes(int nkb) { return lb2_stages(nkb) * (lb2::A_STAGE + nkb * 2 * lb2::B_HALF) + 128 + 1024; }
 
-// DET (deterministic mode): d_cv is the slab array [n_split][B][H]; label split sp stores its partial to slab sp
-template <int NKB, bool DET = false>
+// DET (deterministic mode): d_cv is the slab array [n_split][B][H]; label split sp stores its partial to slab sp.
+// PASS = OnePass (C2V_MATMUL_TF32): hi.hi only; the G producers store no lo panel and only the hi halves of W_out are copied.
+template <int NKB, bool DET = false, class PASS = ThreePass>
 __global__ void __launch_bounds__(lbt::THREADS, 1)
 label_dcv_tc_kernel(const float *__restrict__ G, int B, long long C, int H, const uint8_t *__restrict__ w_img,
                     const float *__restrict__ w_hdr, const unsigned *__restrict__ g_absmax, int n_split,
@@ -355,7 +360,7 @@ label_dcv_tc_kernel(const float *__restrict__ G, int B, long long C, int H, cons
                 const uint32_t hi = base + lb2::SMEM_A_OFF + st * lb2::A_STAGE;
 #pragma unroll
                 for (int j = 0; j < lbt::LD; ++j)
-                    lbt_split_store(hi, hi + lbt::PANEL, lbt_st_off(pw * lbt::ROWS_PER_PW + 2 * j + sub_row, q), buf[j]);
+                    lbt_split_store<PASS>(hi, hi + lbt::PANEL, lbt_st_off(pw * lbt::ROWS_PER_PW + 2 * j + sub_row, q), buf[j]);
                 fence_proxy_async_smem();
                 __syncwarp();
                 if (lane == 0) mbar_arrive(bar_afull + 8 * st);
@@ -375,12 +380,13 @@ label_dcv_tc_kernel(const float *__restrict__ G, int B, long long C, int H, cons
                     const int half = (int)(kblk & 1);
                     const int st = it % S;
                     mbar_wait(bar_bempty + 8 * st, (((uint32_t)(it / S)) & 1u) ^ 1u, status);
-                    mbar_arrive_expect_tx(bar_bfull + 8 * st, (uint32_t)b_stage);
+                    mbar_arrive_expect_tx(bar_bfull + 8 * st, (uint32_t)(one_pass<PASS> ? b_stage / 2 : b_stage));
                     for (int kb = 0; kb < NKB; ++kb) {
                         const uint8_t *src = w_img + ((size_t)nt * NKB + kb) * (size_t)(2 * lbt::PANEL) + half * lb2::B_HALF;
                         const uint32_t dst = smem_b + st * b_stage + kb * 2 * lb2::B_HALF;
                         bulk_copy_g2s(dst, src, lb2::B_HALF, bar_bfull + 8 * st);                                // hi
-                        bulk_copy_g2s(dst + lb2::B_HALF, src + lbt::PANEL, lb2::B_HALF, bar_bfull + 8 * st);     // lo
+                        if constexpr (!one_pass<PASS>)
+                            bulk_copy_g2s(dst + lb2::B_HALF, src + lbt::PANEL, lb2::B_HALF, bar_bfull + 8 * st); // lo
                     }
                 }
             }
@@ -413,6 +419,7 @@ label_dcv_tc_kernel(const float *__restrict__ G, int B, long long C, int H, cons
                         const uint64_t b_hi = wgmma_desc_mn(sb + kb * 2 * lb2::B_HALF + k * 2048, 2 * lb2::B_HALF);
                         const uint64_t b_lo = wgmma_desc_mn(sb + kb * 2 * lb2::B_HALF + lb2::B_HALF + k * 2048, 2 * lb2::B_HALF);
                         wgmma_m64n64<0, 1>(acc[kb], a_hi, b_hi, (kk | k) != 0);
+                        if constexpr (one_pass<PASS>) continue;
                         wgmma_m64n64<0, 1>(acc[kb], a_lo, b_hi, 1);
                         wgmma_m64n64<0, 1>(acc[kb], a_hi, b_lo, 1);
                     }
@@ -460,6 +467,7 @@ int launch_label_backward_tc(const c2v_dims *d, const float *cv, const float *G,
 {
     const int H = d->encode, nkb = (H + 63) / 64;
     const long long C = d->label_count;
+    const bool tf32 = matmul_tf32();           // the calling host thread's matmul precision (c2v_set_matmul_precision)
     int dev = 0, sms = 0;
     C2V_CUDA_OK(cudaGetDevice(&dev));
     C2V_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
@@ -471,10 +479,14 @@ int launch_label_backward_tc(const c2v_dims *d, const float *cv, const float *G,
     if (d_w || d_b) {
         if (!d_w) { set_error("label backward (tensor cores): d_output_bias needs d_output_weight"); return C2V_EINVAL; }
         void (*kern)(const float *, const float *, int, long long, int, const unsigned *, float *, float *, const uint8_t *) =
-            nkb == 1 ? (cv_img ? label_dw_tc_kernel<true, 1> : label_dw_tc_kernel<false, 1>)
-          : nkb == 2 ? (cv_img ? label_dw_tc_kernel<true, 2> : label_dw_tc_kernel<false, 2>)
-          : nkb == 3 ? (cv_img ? label_dw_tc_kernel<true, 3> : label_dw_tc_kernel<false, 3>)
-                     : (cv_img ? label_dw_tc_kernel<true, 4> : label_dw_tc_kernel<false, 4>);
+            tf32 ? (nkb == 1 ? (cv_img ? label_dw_tc_kernel<true, 1, OnePass> : label_dw_tc_kernel<false, 1, OnePass>)
+                  : nkb == 2 ? (cv_img ? label_dw_tc_kernel<true, 2, OnePass> : label_dw_tc_kernel<false, 2, OnePass>)
+                  : nkb == 3 ? (cv_img ? label_dw_tc_kernel<true, 3, OnePass> : label_dw_tc_kernel<false, 3, OnePass>)
+                             : (cv_img ? label_dw_tc_kernel<true, 4, OnePass> : label_dw_tc_kernel<false, 4, OnePass>))
+                 : (nkb == 1 ? (cv_img ? label_dw_tc_kernel<true, 1> : label_dw_tc_kernel<false, 1>)
+                  : nkb == 2 ? (cv_img ? label_dw_tc_kernel<true, 2> : label_dw_tc_kernel<false, 2>)
+                  : nkb == 3 ? (cv_img ? label_dw_tc_kernel<true, 3> : label_dw_tc_kernel<false, 3>)
+                             : (cv_img ? label_dw_tc_kernel<true, 4> : label_dw_tc_kernel<false, 4>));
         C2V_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, lb1::SMEM_BYTES));
         const long long n_ct = (C + 127) / 128;
         const int grid = (int)(n_ct < sms ? n_ct : sms);
@@ -485,10 +497,15 @@ int launch_label_backward_tc(const c2v_dims *d, const float *cv, const float *G,
         if (!dcv_slabs) C2V_CUDA_OK(cudaMemsetAsync(d_cv, 0, (size_t)B * H * sizeof(float), st));
         const int smem = lb2_smem_bytes(nkb);
         void (*kern)(const float *, int, long long, int, const uint8_t *, const float *, const unsigned *, int, long long, float *,
-                     int) = dcv_slabs ? (nkb == 1 ? label_dcv_tc_kernel<1, true> : nkb == 2 ? label_dcv_tc_kernel<2, true>
-                                         : nkb == 3 ? label_dcv_tc_kernel<3, true> : label_dcv_tc_kernel<4, true>)
-                                      : (nkb == 1 ? label_dcv_tc_kernel<1> : nkb == 2 ? label_dcv_tc_kernel<2>
-                                         : nkb == 3 ? label_dcv_tc_kernel<3> : label_dcv_tc_kernel<4>);
+                     int) =
+            tf32 ? (dcv_slabs ? (nkb == 1 ? label_dcv_tc_kernel<1, true, OnePass> : nkb == 2 ? label_dcv_tc_kernel<2, true, OnePass>
+                                 : nkb == 3 ? label_dcv_tc_kernel<3, true, OnePass> : label_dcv_tc_kernel<4, true, OnePass>)
+                              : (nkb == 1 ? label_dcv_tc_kernel<1, false, OnePass> : nkb == 2 ? label_dcv_tc_kernel<2, false, OnePass>
+                                 : nkb == 3 ? label_dcv_tc_kernel<3, false, OnePass> : label_dcv_tc_kernel<4, false, OnePass>))
+                 : (dcv_slabs ? (nkb == 1 ? label_dcv_tc_kernel<1, true> : nkb == 2 ? label_dcv_tc_kernel<2, true>
+                                 : nkb == 3 ? label_dcv_tc_kernel<3, true> : label_dcv_tc_kernel<4, true>)
+                              : (nkb == 1 ? label_dcv_tc_kernel<1> : nkb == 2 ? label_dcv_tc_kernel<2>
+                                 : nkb == 3 ? label_dcv_tc_kernel<3> : label_dcv_tc_kernel<4>));
         C2V_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
         const int n_bt = (B + 127) / 128;
         const long long n_kblocks = (C + 63) / 64;

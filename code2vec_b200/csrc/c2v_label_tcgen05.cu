@@ -1,7 +1,7 @@
 // c2v_label_tcgen05.cu -- K2: label logits  outputs = cv . W_out^T + b  (model.py:83) on the tensor cores (wgmma).
 //
 // Same fp32-accurate scheme as the encode kernel: both operands are split into fp16 hi + lo and
-// three f16 MMAs (hi.hi + lo.hi + hi.lo) accumulate in fp32 registers.  W_out is scaled by a
+// three f16 MMAs (hi.hi + lo.hi + hi.lo) accumulate in fp32 registers (hi.hi alone under C2V_MATMUL_TF32).  W_out is scaled by a
 // power of two (from its absmax) before the split; the epilogue multiplies by the exact inverse
 // and adds the bias.  Plain TF32 fails the 1e-4 bar on trained weights.
 //
@@ -247,8 +247,11 @@ constexpr int SMEM_BYTES_OPT = SMEM_W_OFF + N_EPI_WARPS * 32 * 4 + 1024;
 // itself (see LtSim).  SIM_KNN is the top-k mode with the columns of sm.excl left out; SIM_PAIRS writes every
 // (row, column, cos) with cos >= sm.thr instead.
 // OPT (loss / dlogits modes only, lt2::SMEM_BYTES_OPT of shared memory): the criterion options of LtOpt.
+// PASS = OnePass (the logits / loss / dlogits modes under C2V_MATMUL_TF32): hi.hi only, and the load warp copies only the
+// hi tile of each k-block of both images.  The top-k and similarity modes always run ThreePass (top-k is bound by its
+// epilogue and is not faster in one pass; the similarity queries keep their fp32 contract).
 constexpr int SIM_NONE = 0, SIM_KNN = 1, SIM_PAIRS = 2;
-template <bool ANG, bool TOPK, int SIM = SIM_NONE, bool OPT = false>
+template <bool ANG, bool TOPK, int SIM = SIM_NONE, bool OPT = false, class PASS = ThreePass>
 __global__ void __launch_bounds__(lt2::THREADS, 1)
 label_gemm_v2_kernel(const uint8_t *__restrict__ imgA, const uint8_t *__restrict__ imgB,
                      const float *__restrict__ bias, const float *__restrict__ hdr, float *__restrict__ out,
@@ -258,6 +261,7 @@ label_gemm_v2_kernel(const uint8_t *__restrict__ imgA, const uint8_t *__restrict
                      const LtSim sm, const LtOpt op)
 {
     static_assert(!OPT || (!TOPK && SIM == SIM_NONE), "criterion options belong to the loss / dlogits modes");
+    static_assert(!one_pass<PASS> || (!TOPK && SIM == SIM_NONE), "top-k and the similarity queries run three passes");
     extern __shared__ unsigned char smem_raw[];
     const uint32_t raw = lt_smem_u32(smem_raw);
     const uint32_t base = (raw + 1023u) & ~1023u;
@@ -300,11 +304,12 @@ label_gemm_v2_kernel(const uint8_t *__restrict__ imgA, const uint8_t *__restrict
                     const int st = it & 1;
                     const uint32_t dst = base + st * lt2::STAGE_BYTES;
                     lt_mbar_wait(bar_oempty + 8 * st, ((uint32_t)(it >> 1) & 1u) ^ 1u);
-                    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar_ofull + 8 * st), "r"((uint32_t)(2 * kb_bytes)) : "memory");
+                    constexpr int cp_bytes = one_pass<PASS> ? lt::TILE_BYTES : 2 * lt::TILE_BYTES;   // hi tile first
+                    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar_ofull + 8 * st), "r"((uint32_t)(2 * cp_bytes)) : "memory");
                     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                                 ::"r"(dst), "l"(imgA + ((size_t)mt * nkb + kb) * kb_bytes), "r"((uint32_t)kb_bytes), "r"(bar_ofull + 8 * st) : "memory");
+                                 ::"r"(dst), "l"(imgA + ((size_t)mt * nkb + kb) * kb_bytes), "r"((uint32_t)cp_bytes), "r"(bar_ofull + 8 * st) : "memory");
                     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                                 ::"r"(dst + kb_bytes), "l"(imgB + ((size_t)nt * nkb + kb) * kb_bytes), "r"((uint32_t)kb_bytes), "r"(bar_ofull + 8 * st) : "memory");
+                                 ::"r"(dst + kb_bytes), "l"(imgB + ((size_t)nt * nkb + kb) * kb_bytes), "r"((uint32_t)cp_bytes), "r"(bar_ofull + 8 * st) : "memory");
                 }
             }
         }
@@ -408,6 +413,7 @@ label_gemm_v2_kernel(const uint8_t *__restrict__ imgA, const uint8_t *__restrict
                     for (int hh = 0; hh < 2; ++hh) {
                         const uint64_t a_hi = wgmma_desc(sa + hh * 8192 + k * 32), a_lo = wgmma_desc(sa + lt::TILE_BYTES + hh * 8192 + k * 32);
                         lt_wgmma_m64n32(d[hh], a_hi, b_hi, (kb | k) != 0);
+                        if constexpr (one_pass<PASS>) continue;
                         lt_wgmma_m64n32(d[hh], a_lo, b_hi, 1);
                         lt_wgmma_m64n32(d[hh], a_hi, b_lo, 1);
                     }
@@ -1127,9 +1133,14 @@ int launch_label_tcgen05_ex(const c2v_dims *d, const float *cv, int B, const flo
             ls.part = reinterpret_cast<float2 *>(part4);          // (selects the loss mode; the OPT epilogue writes op.part)
         }
     }
+    // the matmul precision of the calling host thread picks the instantiation (c2v_set_matmul_precision); top-k always
+    // runs three passes
     auto *kern = topk ? (angular ? label_gemm_v2_kernel<true, true> : label_gemm_v2_kernel<false, true>)
-               : opt  ? (angular ? label_gemm_v2_kernel<true, false, SIM_NONE, true> : label_gemm_v2_kernel<false, false, SIM_NONE, true>)
-                      : (angular ? label_gemm_v2_kernel<true, false> : label_gemm_v2_kernel<false, false>);
+               : matmul_tf32()
+        ? (opt ? (angular ? label_gemm_v2_kernel<true, false, SIM_NONE, true, OnePass> : label_gemm_v2_kernel<false, false, SIM_NONE, true, OnePass>)
+               : (angular ? label_gemm_v2_kernel<true, false, SIM_NONE, false, OnePass> : label_gemm_v2_kernel<false, false, SIM_NONE, false, OnePass>))
+        : (opt ? (angular ? label_gemm_v2_kernel<true, false, SIM_NONE, true> : label_gemm_v2_kernel<false, false, SIM_NONE, true>)
+               : (angular ? label_gemm_v2_kernel<true, false> : label_gemm_v2_kernel<false, false>));
     const int smem_bytes = opt ? lt2::SMEM_BYTES_OPT : lt2::SMEM_BYTES;
     const bool want_arg = argmax || maxval;
     const bool fused_arg = want_arg && mt <= (size_t)lt2::MAX_MT;

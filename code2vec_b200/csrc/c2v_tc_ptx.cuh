@@ -3,6 +3,8 @@
 #pragma once
 #include <cuda_fp16.h>
 
+#include <type_traits>
+
 #include "c2v_common.cuh"
 
 #ifndef C2V_SPIN_NS
@@ -10,6 +12,14 @@
 #endif
 
 namespace c2v {
+
+// Passes of the fp16 tensor-core GEMMs, the last template argument of every kernel that has both (named types, so that
+// profiles tell the instantiations apart).  ThreePass (the default): both operands split into fp16 hi + lo, three MMAs
+// per k-step, hi.hi + lo.hi + hi.lo, fp32-accurate.  OnePass (C2V_MATMUL_TF32): hi.hi only -- 10 explicit mantissa bits
+// per operand, TF32-class -- with the lo halves neither converted, loaded nor multiplied.
+struct ThreePass {};
+struct OnePass {};
+template <class P> constexpr bool one_pass = std::is_same<P, OnePass>::value;
 
 // ------------------------------------------------------------------------------------
 // PTX wrappers

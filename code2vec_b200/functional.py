@@ -39,6 +39,27 @@ def sync_deterministic():
     return on
 
 
+def torch_matmul_tf32():
+    """True while torch lets its fp32 CUDA matmuls use TF32: torch.backends.cuda.matmul.fp32_precision == "tf32", what
+    torch.set_float32_matmul_precision("high" / "medium"), allow_tf32 = True and the fp32_precision setters (this one and
+    torch.backends.fp32_precision) select.  The legacy getters (allow_tf32, get_float32_matmul_precision()) are not read:
+    they raise once a setter of the new API has been used."""
+    return torch.backends.cuda.matmul.fp32_precision == "tf32"
+
+
+def sync_matmul_precision():
+    """Set the library's matmul precision (c2v_set_matmul_precision) of the calling thread from torch's switch:
+    C2V_MATMUL_TF32 while torch_matmul_tf32(), C2V_MATMUL_IEEE otherwise.  Like sync_deterministic the mode is per host
+    thread and the library is called only when the value changed; every wrapper that can reach a tensor-core GEMM calls
+    this.  Returns True in TF32 mode."""
+    on = torch_matmul_tf32()
+    if getattr(_det, "tf32", False) != on:
+        _lib.check(_lib.load().c2v_set_matmul_precision(_lib.MATMUL_TF32 if on else _lib.MATMUL_IEEE),
+                   "c2v_set_matmul_precision")
+        _det.tf32 = on
+    return on
+
+
 def _ptr(t):
     return ctypes.c_void_p(t.data_ptr()) if t is not None else None
 
@@ -174,6 +195,7 @@ def encode_forward(dims, params, starts, paths, ends, drop_p=0.0, training=False
     stash=True (training): also returns x = c . W^T [B*L, H] for encode_backward(x_stash=...), which then skips the
     re-gather and the recompute GEMM."""
     lib = _lib.load()
+    sync_matmul_precision()
     _need_cuda(starts, paths, ends)
     B, L = starts.shape
     starts = _idx(starts, "starts"); paths = _idx(paths, "paths", (B, L)); ends = _idx(ends, "ends", (B, L))
@@ -293,6 +315,7 @@ def encode_forward_packed(dims, params, bags, drop_p=0.0, training=False, seed=0
         raise RuntimeError("PackedBags batches cannot be captured into a CUDA graph: their context count N changes from "
                            "batch to batch; capture padded [B, L] batches")
     lib = _lib.load()
+    sync_matmul_precision()
     _need_cuda(bags.starts, bags.paths, bags.ends, bags.offsets)
     B, N, L = bags.B, bags.N, bags.L
     dev = bags.device
@@ -328,6 +351,7 @@ def _label_ws(dims, B, dev, algo, cache, weight, nbytes=None, absmax_ready=False
     workspace, plus REUSE_PREP while its W_out image is current and GRAD_ABSMAX_READY if absmax_ready.  Without one a fresh
     workspace, or None if not fresh (the backward calls then run on the CUDA cores)."""
     sync_deterministic()
+    sync_matmul_precision()
     if nbytes is None:
         nbytes = _lib.load().c2v_label_workspace_bytes(ctypes.byref(dims), B)
     algo = capture_flags(algo)
@@ -748,6 +772,7 @@ def encode_backward(dims, params, starts, paths, ends, cv, att, d_cv, d_att, sha
     with a slot map (c2v_encode_backward_sparse)."""
     lib = _lib.load()
     sync_deterministic()
+    sync_matmul_precision()
     B, L = starts.shape
     dev = starts.device
     with torch.cuda.device(dev):
@@ -782,6 +807,7 @@ def encode_backward_packed(dims, params, bags, cv, att, d_cv, d_att, shapes, dro
     """encode_backward for a PackedBags batch: att / d_att [N], x_stash [N, H] from encode_forward_packed(stash=True)."""
     lib = _lib.load()
     sync_deterministic()
+    sync_matmul_precision()
     B, N, L = bags.B, bags.N, bags.L
     dev = bags.device
     with torch.cuda.device(dev):

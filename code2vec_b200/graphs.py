@@ -12,11 +12,12 @@ static inputs, copy in and replay) to a Code2Vec step:
 What a captured step needs (checked, each with a clear error): dropout keys drawn on the device
 (Code2Vec.use_device_rng), an optimizer whose step count lives on the device (FlatAdam / ShardedFlatAdam with
 capturable=True at world size 1, or torch.optim.Adam(capturable=True)), dense embedding gradients and padded [B, L]
-batches.  Hyper-parameters and model.training are fixed at capture.  See INTEGRATION.md, "CUDA graphs".
+batches.  Hyper-parameters, model.training and torch's TF32 matmul switch are fixed at capture.  See INTEGRATION.md, "CUDA graphs".
 """
 import torch
 
 from .distributed import FlatAdam, ShardedFlatAdam, _forward_loss, ddp_step
+from .functional import torch_matmul_tf32
 
 __all__ = ["GraphedTrainStep", "GraphedPredict"]
 
@@ -39,7 +40,8 @@ class _Graphed:
         self._frozen = None
 
     def _settings(self):
-        return (self.model.training,)
+        # the matmul precision selects other kernels than the captured ones
+        return (self.model.training, torch_matmul_tf32())
 
     def _call(self, *inputs):
         self.model._enc_cache.raise_deferred()           # an out-of-range index in an earlier replay
@@ -50,8 +52,9 @@ class _Graphed:
             return self._run(*inputs)                    # e.g. the ragged last batch of an epoch: eagerly
         if self.graph is not None:
             if self._settings() != self._frozen:
-                raise RuntimeError(f"{type(self).__name__}: hyper-parameters, the criterion, model.training or "
-                                   "torch.are_deterministic_algorithms_enabled() changed since the capture "
+                raise RuntimeError(f"{type(self).__name__}: hyper-parameters, the criterion, model.training, "
+                                   "torch.are_deterministic_algorithms_enabled() or the TF32 matmul switch "
+                                   "(torch.backends.cuda.matmul.fp32_precision) changed since the capture "
                                    f"({self._frozen} -> {self._settings()}); build a new {type(self).__name__}")
             for s, t in zip(self.static_in, inputs):
                 s.copy_(t, non_blocking=True)
@@ -114,8 +117,9 @@ class GraphedTrainStep(_Graphed):
         c = self.criterion
         crit = None if c is None else (type(c), c.ignore_index, getattr(c, "label_smoothing", 0.0), c.reduction,
                                        None if c.weight is None else (c.weight.data_ptr(), tuple(c.weight.shape)))
-        # the deterministic mode selects other kernels and workspace sizes than the captured ones
-        return (self.model.training, torch.are_deterministic_algorithms_enabled(), hyper, crit)
+        # the deterministic mode selects other kernels and workspace sizes than the captured ones, the matmul precision
+        # other kernels
+        return (self.model.training, torch.are_deterministic_algorithms_enabled(), torch_matmul_tf32(), hyper, crit)
 
     def _run(self, starts, paths, ends, label):
         model, opt = self.model, self.optimizer

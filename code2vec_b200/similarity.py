@@ -24,12 +24,29 @@ FALLBACK_BLOCK_ELEMS = 1 << 26         # torch fallback: at most this many [q, N
 
 @contextlib.contextmanager
 def _fp32_matmul():
-    prev = torch.backends.cuda.matmul.allow_tf32
-    torch.backends.cuda.matmul.allow_tf32 = False
+    # Through fp32_precision whichever API set the switch: the legacy getter raises once the new API has been used, and
+    # restoring through the legacy setter would pin a setting that followed torch.backends.fp32_precision before.
+    m = torch.backends.cuda.matmul
+    prev = "none" if _matmul_inherits() else m.fp32_precision
+    m.fp32_precision = "ieee"
     try:
         yield
     finally:
-        torch.backends.cuda.matmul.allow_tf32 = prev
+        m.fp32_precision = prev
+
+
+def _matmul_inherits():
+    """True while torch.backends.cuda.matmul.fp32_precision is "none", i.e. follows torch.backends.fp32_precision.  Its
+    getter returns the resolved value, so the global setting (whose getter returns what was set) is flipped and
+    restored: an inheriting matmul setting follows the flip."""
+    b, m = torch.backends, torch.backends.cuda.matmul
+    saved = b.fp32_precision
+    probe = "ieee" if m.fp32_precision == "tf32" else "tf32"
+    b.fp32_precision = probe
+    try:
+        return m.fp32_precision == probe
+    finally:
+        b.fp32_precision = saved
 
 
 def analogy_query(vectors, positive, negative=()):

@@ -53,7 +53,8 @@ enum {
 enum {
     C2V_ALGO_AUTO = 0,
     C2V_ALGO_FFMA = 1,    /* fp32 CUDA-core path, any shape                         */
-    C2V_ALGO_TCGEN05 = 2  /* tensor cores (wgmma f16), 3-pass hi/lo split, fp32-accurate */
+    C2V_ALGO_TCGEN05 = 2  /* tensor cores (wgmma f16): fp16 hi/lo split, three passes (fp32-accurate) under
+                           * C2V_MATMUL_IEEE, one pass (hi.hi, TF32-class) under C2V_MATMUL_TF32 */
 };
 
 /* OR-ed into `algo`: the caller guarantees that the parameters behind this workspace have not
@@ -153,6 +154,27 @@ const char *c2v_last_error(void);
  * stays capturable into a CUDA graph. */
 int c2v_set_deterministic(int32_t on);
 int c2v_get_deterministic(void);
+
+/* Matmul precision, per host thread like the deterministic mode (C2V_MATMUL_IEEE by default); what
+ * torch.set_float32_matmul_precision("high") selects for torch's own fp32 GEMMs.
+ *   C2V_MATMUL_IEEE: every tensor-core GEMM splits both fp32 operands into fp16 hi + lo and issues three MMAs per k-step
+ *     (hi.hi + lo.hi + hi.lo): fp32-accurate.
+ *   C2V_MATMUL_TF32: the same kernels issue hi.hi only (10 explicit mantissa bits per operand, as TF32), and the operands
+ *     split per tile in registers (embedding rows, dX, d logits) lose their lo half.  This covers the encode forward (all
+ *     layouts and sizes, the session calls included), c2v_encode_backward*'s dW on the tensor cores, and the label GEMM
+ *     and its backward (logits, arg-max, fused loss, dlogits, both heads, c2v_label_backward_ws,
+ *     c2v_angular_backward_ws).  Two tensor-core kernels keep three passes because one pass is not faster there: dC of
+ *     c2v_encode_backward* (bound by its scatter) and the top-k label GEMM (c2v_label_topk / c2v_angular_topk, bound by
+ *     its epilogue).  Unscaled operands (embedding rows, code vectors) keep fp16's range: below 2^-14 they are
+ *     subnormal with an absolute error of ~2^-25, and |v| >= 65520 overflows in both modes.
+ * Unchanged in both modes: c2v_knn_topk / c2v_knn_pairs (fp32 contract), every CUDA-core path (C2V_ALGO_FFMA,
+ * c2v_angular_* on the CUDA cores, c2v_loss_argmax), workspace sizes and the cached weight images (the OnePass kernels
+ * read their hi halves), so switching modes between calls needs no new workspace and leaves no stale image.
+ * Combines with the deterministic mode.  Any other mode: C2V_EINVAL. */
+#define C2V_MATMUL_IEEE 0
+#define C2V_MATMUL_TF32 1
+int c2v_set_matmul_precision(int32_t mode);
+int c2v_get_matmul_precision(void);
 
 /* Device facts the host side sizes grids with. */
 typedef struct c2v_device_info {
