@@ -140,6 +140,10 @@ SYMBOLS = {
     "c2v_adam_step": (ctypes.c_int, [c_vp, c_vp, c_vp, c_vp, c_i64, c_f32, c_f32, c_f32, c_f32, c_f32, c_i64, c_f32, c_i32, c_vp]),
     "c2v_adam_step_capturable": (ctypes.c_int, [c_vp, c_vp, c_vp, c_vp, c_i64, c_f32, c_f32, c_f32, c_f32, c_f32, c_vp, c_f32,
                                                 c_i32, c_vp]),
+    "c2v_grad_norm_workspace_bytes": (c_sz, [c_i64]),
+    "c2v_grad_clip_coef": (ctypes.c_int, [c_vp, c_i64, c_f32, c_f32, c_vp, c_vp, c_sz, c_vp]),
+    "c2v_adam_step_ex": (ctypes.c_int, [c_vp, c_vp, c_vp, c_vp, c_i64, c_f32, c_f32, c_f32, c_f32, c_f32, c_i64, c_vp, c_f32,
+                                        c_i32, c_vp, c_vp, c_vp]),
     "c2v_next_dropout_key": (ctypes.c_int, [c_vp, c_vp, c_vp]),
     "c2v_adam_step_sharded": (ctypes.c_int, [c_vp, c_vp, c_vp, _P(c_vp), _P(c_vp), c_i32, c_vp, c_vp, c_i64, c_i64, c_vp, c_i64,
                                              c_f32, c_f32, c_f32, c_f32, c_f32, c_i64, c_f32, c_vp]),

@@ -17,7 +17,9 @@ namespace c2v {
 // The gradient Adam sees: g * gscale (the 1/world of the data-parallel mean) + wd * p (weight decay), rounded once
 // relative to the result.  fmaf(wd, p, g * gscale) alone would round g * gscale first, and where the two terms nearly
 // cancel that rounding is large next to the result (then m is off by tens of ulp); the second fmaf recovers the product's
-// rounding error exactly.  With wd == 0, or an exact gscale (world 1), both forms give the same value.
+// rounding error exactly.  With wd == 0, or an exact gscale (1, or a power of two), both forms give the same value;
+// 1/world for other world sizes and every active clip coefficient (gscale = grad_scale * coef, c2v_grad_clip_coef) are
+// inexact.
 __device__ __forceinline__ float adam_grad(float g, float gscale, float wd, float p) {
     const float gs = g * gscale;
     if (wd == 0.0f) return gs;
@@ -26,14 +28,18 @@ __device__ __forceinline__ float adam_grad(float g, float gscale, float wd, floa
 
 // DEV_SCALARS (c2v_adam_step_capturable): step_size and inv_sqrt_bc2 are read from dev_scalars[0..1], where
 // adam_step_count_kernel left them, instead of the launch parameters.
-template <bool DEV_SCALARS = false>
+// DEV_COEF (c2v_adam_step_ex with coef_dev): the gradient is read as g * (gscale * *coef_dev), the clip coefficient that
+// grad_norm_finalize_kernel left on the device, formed once per thread: no host read between the norm and the update.
+template <bool DEV_SCALARS = false, bool DEV_COEF = false>
 __global__ void __launch_bounds__(256)
 adam_step_kernel(float4 *__restrict__ p, float4 *__restrict__ g, float4 *__restrict__ m, float4 *__restrict__ v,
                  long long n4, float *__restrict__ pt, float *__restrict__ gt, float *__restrict__ mt, float *__restrict__ vt,
                  int tail, float step_size, float one_minus_b1, float b2, float one_minus_b2, float inv_sqrt_bc2, float eps,
-                 float wd, float gscale, int zero_grad, const float *__restrict__ dev_scalars)
+                 float wd, float gscale, int zero_grad, const float *__restrict__ dev_scalars,
+                 const float *__restrict__ coef_dev)
 {
     if (DEV_SCALARS) { step_size = dev_scalars[0]; inv_sqrt_bc2 = dev_scalars[1]; }
+    if (DEV_COEF) gscale *= *coef_dev;
     auto upd = [&](float &pp, float &gg, float &mm, float &vv) {
         const float gr = adam_grad(gg, gscale, wd, pp);
         mm = mm + (gr - mm) * one_minus_b1;                 // exp_avg.lerp_(grad, 1 - beta1)
@@ -61,15 +67,71 @@ adam_step_kernel(float4 *__restrict__ p, float4 *__restrict__ g, float4 *__restr
 }
 
 // The step count of c2v_adam_step_capturable: state = {int64 step; float step_size; float inv_sqrt_bc2}.  The bias
-// corrections use c2v_adam_step's host expressions, in double.
-__global__ void adam_step_count_kernel(long long *state, float lr, float beta1, float beta2)
+// corrections use c2v_adam_step's host expressions, in double.  lr_dev != NULL: the learning rate is read from there
+// (a tensor lr that a scheduler fills between the replays of a captured step) instead of the launch parameter.
+__global__ void adam_step_count_kernel(long long *state, float lr, float beta1, float beta2, const float *lr_dev)
 {
+    if (lr_dev) lr = *lr_dev;
     const long long t = state[0] + 1;
     state[0] = t;
     const double bc1 = 1.0 - pow((double)beta1, (double)t), bc2 = 1.0 - pow((double)beta2, (double)t);
     float *f = reinterpret_cast<float *>(state + 1);
     f[0] = (float)((double)lr / bc1);
     f[1] = (float)(1.0 / sqrt(bc2));
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// Gradient clipping by global L2 norm (torch.nn.utils.clip_grad_norm_, norm_type 2) in front of the flat step: one pass
+// over the flat gradient leaves one partial sum of squares per CTA, a one-warp finalize adds the partials in a fixed order
+// in double and writes {norm, coef} = {|grad_scale| * sqrt(sum),  min(1, max_norm / (norm + 1e-6))}.  The grid depends
+// on n alone and no float atomic is involved, so the norm is bit-reproducible.  A NaN norm gives a NaN coef (torch's
+// clamp keeps a NaN), an inf norm gives 0: the update then multiplies the inf by 0, and a diverged step stays visible.
+// ------------------------------------------------------------------------------------------------------------------
+constexpr int GN_THREADS = 256, GN_MAX_CTAS = 1024;
+
+static long long grad_norm_ctas(long long n)
+{
+    const long long ctas = (n / 4 + GN_THREADS - 1) / GN_THREADS;
+    return ctas < 1 ? 1 : (ctas > GN_MAX_CTAS ? GN_MAX_CTAS : ctas);
+}
+
+__global__ void __launch_bounds__(GN_THREADS)
+grad_sumsq_kernel(const float4 *__restrict__ g, long long n4, const float *__restrict__ gt, int tail,
+                  float *__restrict__ partial)
+{
+    __shared__ float warp_part[GN_THREADS / 32];
+    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
+        const float4 G = g[i];
+        acc.x = fmaf(G.x, G.x, acc.x); acc.y = fmaf(G.y, G.y, acc.y);
+        acc.z = fmaf(G.z, G.z, acc.z); acc.w = fmaf(G.w, G.w, acc.w);
+    }
+    if (blockIdx.x == 0 && (int)threadIdx.x < tail) acc.x = fmaf(gt[threadIdx.x], gt[threadIdx.x], acc.x);
+    const float s = warp_sum((acc.x + acc.y) + (acc.z + acc.w));
+    if ((threadIdx.x & 31) == 0) warp_part[threadIdx.x >> 5] = s;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float t = 0.0f;
+        for (int w = 0; w < GN_THREADS / 32; ++w) t += warp_part[w];
+        partial[blockIdx.x] = t;
+    }
+}
+
+// one warp: lane l adds partials l, l + 32, ... in that order, then the lanes are added pairwise (xor 16, 8, 4, 2, 1)
+__global__ void __launch_bounds__(32)
+grad_norm_finalize_kernel(const float *__restrict__ partial, int n_partial, float grad_scale, float max_norm,
+                          float *__restrict__ norm_coef)
+{
+    double s = 0.0;
+    for (int i = threadIdx.x; i < n_partial; i += 32) s += (double)partial[i];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (threadIdx.x == 0) {
+        const float norm = (float)(sqrt(s) * fabs((double)grad_scale));
+        const float c = max_norm / (norm + 1e-6f);
+        norm_coef[0] = norm;
+        norm_coef[1] = c > 1.0f ? 1.0f : c;                 // not fminf: a NaN norm must give a NaN coefficient
+    }
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -322,10 +384,10 @@ static bool adam_buffers_ok(const char *fn, const float *param, const float *gra
     return true;
 }
 
-// the flat update kernel; dev_scalars != NULL: its DEV_SCALARS instantiation
+// the flat update kernel; dev_scalars != NULL: its DEV_SCALARS instantiation, coef_dev != NULL: its DEV_COEF one
 static int launch_adam_flat(float *param, float *grad, float *exp_avg, float *exp_avg_sq, int64_t n, float step_size,
                             float beta1, float beta2, float inv_sqrt_bc2, float eps, float weight_decay, float grad_scale,
-                            int32_t zero_grad, const float *dev_scalars, cudaStream_t st)
+                            int32_t zero_grad, const float *dev_scalars, const float *coef_dev, cudaStream_t st)
 {
     const long long n4 = n / 4;
     const int tail = (int)(n % 4);
@@ -335,45 +397,116 @@ static int launch_adam_flat(float *param, float *grad, float *exp_avg, float *ex
     long long blocks = (n4 + 255) / 256;
     if (blocks > (long long)sms * 16) blocks = (long long)sms * 16;
     if (blocks < 1) blocks = 1;
-    (dev_scalars ? adam_step_kernel<true> : adam_step_kernel<false>)<<<(unsigned)blocks, 256, 0, st>>>(
+    auto kernel = dev_scalars ? (coef_dev ? adam_step_kernel<true, true> : adam_step_kernel<true>)
+                              : (coef_dev ? adam_step_kernel<false, true> : adam_step_kernel<false>);
+    kernel<<<(unsigned)blocks, 256, 0, st>>>(
         reinterpret_cast<float4 *>(param), reinterpret_cast<float4 *>(grad), reinterpret_cast<float4 *>(exp_avg),
         reinterpret_cast<float4 *>(exp_avg_sq), n4, param + n4 * 4, grad + n4 * 4, exp_avg + n4 * 4, exp_avg_sq + n4 * 4, tail,
-        step_size, 1.0f - beta1, beta2, 1.0f - beta2, inv_sqrt_bc2, eps, weight_decay, grad_scale, zero_grad, dev_scalars);
+        step_size, 1.0f - beta1, beta2, 1.0f - beta2, inv_sqrt_bc2, eps, weight_decay, grad_scale, zero_grad, dev_scalars,
+        coef_dev);
     C2V_LAUNCH_OK("adam_step_kernel");
     return C2V_OK;
+}
+
+// c2v_adam_step (step_state NULL: bias corrections on the host from `step`) and c2v_adam_step_capturable (step count on
+// the device) with the optional device scalars of c2v_adam_step_ex
+static int adam_step_flat(const char *fn, float *param, float *grad, float *exp_avg, float *exp_avg_sq, int64_t n, float lr,
+                          float beta1, float beta2, float eps, float weight_decay, int64_t step, void *step_state,
+                          float grad_scale, int32_t zero_grad, const float *lr_dev, const float *coef_dev, void *stream)
+{
+    if (!adam_buffers_ok(fn, param, grad, exp_avg, exp_avg_sq, n)) return C2V_EINVAL;
+    if (misaligned(lr_dev, 4) || misaligned(coef_dev, 4)) {
+        set_error("%s: lr_dev and coef_dev must be 4-byte aligned", fn);
+        return C2V_EINVAL;
+    }
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (!step_state) {
+        if (lr_dev) {
+            set_error("%s: lr_dev needs the step count on the device (step_state)", fn);
+            return C2V_EINVAL;
+        }
+        if (step < 1) {
+            set_error("%s: bad argument", fn);
+            return C2V_EINVAL;
+        }
+        const double bc1 = 1.0 - pow((double)beta1, (double)step), bc2 = 1.0 - pow((double)beta2, (double)step);
+        const float step_size = (float)((double)lr / bc1);
+        const float inv_sqrt_bc2 = (float)(1.0 / sqrt(bc2));
+        return launch_adam_flat(param, grad, exp_avg, exp_avg_sq, n, step_size, beta1, beta2, inv_sqrt_bc2, eps,
+                                weight_decay, grad_scale, zero_grad, nullptr, coef_dev, st);
+    }
+    if (reinterpret_cast<uintptr_t>(step_state) & 7) {
+        set_error("%s: step_state must be an 8-byte aligned device buffer of 16 bytes", fn);
+        return C2V_EINVAL;
+    }
+    long long *state = static_cast<long long *>(step_state);
+    adam_step_count_kernel<<<1, 1, 0, st>>>(state, lr, beta1, beta2, lr_dev);
+    C2V_LAUNCH_OK("adam_step_count_kernel");
+    return launch_adam_flat(param, grad, exp_avg, exp_avg_sq, n, 0.0f, beta1, beta2, 0.0f, eps, weight_decay, grad_scale,
+                            zero_grad, reinterpret_cast<const float *>(state + 1), coef_dev, st);
 }
 
 extern "C" int c2v_adam_step(float *param, float *grad, float *exp_avg, float *exp_avg_sq, int64_t n, float lr,
                              float beta1, float beta2, float eps, float weight_decay, int64_t step, float grad_scale,
                              int32_t zero_grad, void *stream)
 {
-    if (!adam_buffers_ok("c2v_adam_step", param, grad, exp_avg, exp_avg_sq, n)) return C2V_EINVAL;
-    if (step < 1) {
-        set_error("c2v_adam_step: bad argument");
-        return C2V_EINVAL;
-    }
-    const double bc1 = 1.0 - pow((double)beta1, (double)step), bc2 = 1.0 - pow((double)beta2, (double)step);
-    const float step_size = (float)((double)lr / bc1);
-    const float inv_sqrt_bc2 = (float)(1.0 / sqrt(bc2));
-    return launch_adam_flat(param, grad, exp_avg, exp_avg_sq, n, step_size, beta1, beta2, inv_sqrt_bc2, eps, weight_decay,
-                            grad_scale, zero_grad, nullptr, static_cast<cudaStream_t>(stream));
+    return adam_step_flat("c2v_adam_step", param, grad, exp_avg, exp_avg_sq, n, lr, beta1, beta2, eps, weight_decay, step,
+                          nullptr, grad_scale, zero_grad, nullptr, nullptr, stream);
 }
 
 extern "C" int c2v_adam_step_capturable(float *param, float *grad, float *exp_avg, float *exp_avg_sq, int64_t n, float lr,
                                         float beta1, float beta2, float eps, float weight_decay, void *step_state,
                                         float grad_scale, int32_t zero_grad, void *stream)
 {
-    if (!adam_buffers_ok("c2v_adam_step_capturable", param, grad, exp_avg, exp_avg_sq, n)) return C2V_EINVAL;
-    if (!step_state || (reinterpret_cast<uintptr_t>(step_state) & 7)) {
+    if (!step_state) {
         set_error("c2v_adam_step_capturable: step_state must be an 8-byte aligned device buffer of 16 bytes");
         return C2V_EINVAL;
     }
+    return adam_step_flat("c2v_adam_step_capturable", param, grad, exp_avg, exp_avg_sq, n, lr, beta1, beta2, eps,
+                          weight_decay, 0, step_state, grad_scale, zero_grad, nullptr, nullptr, stream);
+}
+
+extern "C" int c2v_adam_step_ex(float *param, float *grad, float *exp_avg, float *exp_avg_sq, int64_t n, float lr,
+                                float beta1, float beta2, float eps, float weight_decay, int64_t step, void *step_state,
+                                float grad_scale, int32_t zero_grad, const float *lr_dev, const float *coef_dev,
+                                void *stream)
+{
+    return adam_step_flat("c2v_adam_step_ex", param, grad, exp_avg, exp_avg_sq, n, lr, beta1, beta2, eps, weight_decay, step,
+                          step_state, grad_scale, zero_grad, lr_dev, coef_dev, stream);
+}
+
+extern "C" size_t c2v_grad_norm_workspace_bytes(int64_t n) { return n < 1 ? 0 : (size_t)grad_norm_ctas(n) * sizeof(float); }
+
+extern "C" int c2v_grad_clip_coef(const float *grad, int64_t n, float grad_scale, float max_norm, float *out_norm_coef,
+                                  void *workspace, size_t workspace_bytes, void *stream)
+{
+    if (!grad || !out_norm_coef || !workspace || n < 1) {
+        set_error("c2v_grad_clip_coef: bad argument (NULL pointer or n = %lld)", (long long)n);
+        return C2V_EINVAL;
+    }
+    if (!(max_norm > 0.0f)) {
+        set_error("c2v_grad_clip_coef: max_norm must be > 0");
+        return C2V_EINVAL;
+    }
+    if (misaligned(grad, 16) || misaligned(out_norm_coef, 4) || misaligned(workspace, 4)) {
+        set_error("c2v_grad_clip_coef: misaligned pointer (grad: 16 bytes, out_norm_coef and workspace: 4)");
+        return C2V_EINVAL;
+    }
+    const long long ctas = grad_norm_ctas(n);
+    if (workspace_bytes < (size_t)ctas * sizeof(float)) {
+        set_error("c2v_grad_clip_coef: workspace of %zu bytes, c2v_grad_norm_workspace_bytes(%lld) = %zu", workspace_bytes,
+                  (long long)n, (size_t)ctas * sizeof(float));
+        return C2V_EINVAL;
+    }
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    long long *state = static_cast<long long *>(step_state);
-    adam_step_count_kernel<<<1, 1, 0, st>>>(state, lr, beta1, beta2);
-    C2V_LAUNCH_OK("adam_step_count_kernel");
-    return launch_adam_flat(param, grad, exp_avg, exp_avg_sq, n, 0.0f, beta1, beta2, 0.0f, eps, weight_decay, grad_scale,
-                            zero_grad, reinterpret_cast<const float *>(state + 1), st);
+    float *partial = static_cast<float *>(workspace);
+    const long long n4 = n / 4;
+    grad_sumsq_kernel<<<(unsigned)ctas, GN_THREADS, 0, st>>>(reinterpret_cast<const float4 *>(grad), n4, grad + n4 * 4,
+                                                             (int)(n % 4), partial);
+    C2V_LAUNCH_OK("grad_sumsq_kernel");
+    grad_norm_finalize_kernel<<<1, 32, 0, st>>>(partial, (int)ctas, grad_scale, max_norm, out_norm_coef);
+    C2V_LAUNCH_OK("grad_norm_finalize_kernel");
+    return C2V_OK;
 }
 
 extern "C" int c2v_adam_step_sharded(const float *param_local, float *param_multicast, const float *grad_multicast,

@@ -74,64 +74,233 @@ class FlatGradBucket:
                 self.flat.mul_(1.0 / dist.get_world_size())
 
 
-class FlatAdam:
-    """torch.optim.Adam(model.parameters(), lr, betas, weight_decay) (main.py:138) as ONE kernel launch per step
-    (`c2v_adam_step`): parameters, like the gradients of `bucket`, become views into one flat buffer; the step reads
-    p, g, m, v once, writes p, m, v and leaves the gradient zeroed for the next backward (main.py:171), folding the
-    1/world of the data-parallel mean into the read.  Dense, same update rule and operation order as torch's Adam.
+class _FlatAdamBase(torch.optim.Optimizer):
+    """What FlatAdam and ShardedFlatAdam share as torch.optim.Optimizers: ONE parameter group (a flat launch has one set of
+    hyper-parameters) that is the source of truth for lr, betas, eps, weight_decay and max_grad_norm, so that the
+    torch.optim.lr_scheduler classes drive them (the group's `capturable` records the `capturable` attribute, which is
+    fixed at construction); state_dict() / load_state_dict() in torch.optim.Adam's format; and the flat launch itself.  Subclasses provide `_flat_offsets` (caller-order parameter -> offset in the flat buffers),
+    `_gather_state()` and `_scatter_state()`."""
 
-    capturable=True (torch.optim.Adam's flag): the step count lives on the device (`step_state`, see
-    c2v_adam_step_capturable) and every step, eager or inside a CUDA graph, runs the capturable kernels; `t` is then not
-    kept (read `step_count()`).  With capturable=False a step cannot be captured."""
+    def _init_optimizer(self, params, dev, lr, betas, eps, weight_decay, max_grad_norm, capturable):
+        if isinstance(lr, torch.Tensor):
+            if not capturable:
+                raise ValueError("a tensor lr is read by the captured step-count kernel: it needs capturable=True")
+            if lr.device != dev or lr.dtype != torch.float32 or lr.numel() != 1:
+                raise ValueError(f"a tensor lr must be a one-element fp32 tensor on {dev}, got {lr.dtype} "
+                                 f"{tuple(lr.shape)} on {lr.device}")
+        else:
+            lr = float(lr)
+        if max_grad_norm is not None and not float(max_grad_norm) > 0.0:
+            raise ValueError(f"max_grad_norm must be None or > 0, got {max_grad_norm}")
+        super().__init__(params, dict(lr=lr, betas=(float(betas[0]), float(betas[1])), eps=float(eps),
+                                      weight_decay=float(weight_decay),
+                                      max_grad_norm=None if max_grad_norm is None else float(max_grad_norm),
+                                      capturable=bool(capturable)))
+        self.capturable = bool(capturable)               # fixed at construction: it decides where the step count lives
+        # {norm, coef} of the last clipped step (c2v_grad_clip_coef) and the per-CTA partials of its norm pass
+        self._norm_coef = torch.zeros(2, dtype=torch.float32, device=dev)
+        self._norm_ws = torch.empty(1024, dtype=torch.float32, device=dev)
 
-    def __init__(self, bucket, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, capturable=False):
-        self.bucket = bucket
-        self.lr, self.betas, self.eps, self.weight_decay = float(lr), (float(betas[0]), float(betas[1])), float(eps), float(weight_decay)
-        flat = torch.empty_like(bucket.flat)
-        o = 0
-        for p in bucket.params:                                  # same order as the gradient bucket
-            n = p.numel()
-            flat[o:o + n].copy_(p.data.reshape(-1))
-            p.data = flat[o:o + n].view_as(p)
-            o += n
-        self.flat_param = flat
-        self.exp_avg = torch.zeros_like(flat)
-        self.exp_avg_sq = torch.zeros_like(flat)
-        self.t = 0
-        self.capturable = bool(capturable)
-        self.step_state = _step_state(flat.device) if self.capturable else None
+    def _patch_step_function(self):
+        # torch wraps the class's step() with the step hooks when the first instance is built; wrap this instance's
+        # instead, so that the class keeps the plain function whether or not an instance exists
+        self._zero_grad_profile_name = f"Optimizer.zero_grad#{type(self).__name__}.zero_grad"
+        self.step = torch.optim.Optimizer.profile_hook_step(type(self).step).__get__(self)
+
+    def add_param_group(self, param_group):
+        if self.param_groups:
+            raise ValueError(f"{type(self).__name__} has one parameter group: one flat launch has one set of "
+                             "hyper-parameters")
+        super().add_param_group(param_group)
+
+    def _group_value(name):
+        def get(self):
+            return self.param_groups[0][name]
+
+        def put(self, value):
+            g = self.param_groups[0]
+            if name == "lr" and isinstance(g["lr"], torch.Tensor):
+                g["lr"].fill_(float(value))              # a captured graph reads this address
+            else:
+                g[name] = value
+        return property(get, put)
+
+    lr, betas, eps, weight_decay = _group_value("lr"), _group_value("betas"), _group_value("eps"), _group_value("weight_decay")
+    max_grad_norm = _group_value("max_grad_norm")
+    del _group_value
 
     def step_count(self):
         """the number of steps taken (synchronises in capturable mode)"""
         return int(self.step_state[0]) if self.capturable else self.t
 
-    def step(self, grad_scale=1.0, zero_grad=True):
+    @property
+    def grad_norm(self):
+        """one-element fp32 device tensor: the global L2 norm of the last step's gradient (after grad_scale, before
+        the clip: what clip_grad_norm_ returns); written only by steps with max_grad_norm set.  No synchronise."""
+        return self._norm_coef[:1]
+
+    def _launch(self, p, g, m, v, step, grad_scale, zero_grad):
+        """c2v_adam_step_ex on flat fp32 buffers with the group's hyper-parameters, behind c2v_grad_clip_coef on the same
+        gradient when max_grad_norm is set.  With max_grad_norm None and a float lr it is c2v_adam_step /
+        c2v_adam_step_capturable: same kernels, same launch parameters."""
         import ctypes
         from . import _lib
         lib = _lib.load()
-        _check_capturable(self.capturable, "FlatAdam")
         P = lambda t: ctypes.c_void_p(t.data_ptr())
-        dev = self.flat_param.device
+        group = self.param_groups[0]
+        lr, (beta1, beta2), max_norm = group["lr"], group["betas"], group["max_grad_norm"]
+        lr_dev = P(lr) if isinstance(lr, torch.Tensor) else None
+        dev = p.device
         with torch.cuda.device(dev):
             stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-            if self.capturable:
-                rc = lib.c2v_adam_step_capturable(P(self.flat_param), P(self.bucket.flat), P(self.exp_avg), P(self.exp_avg_sq),
-                                                  self.flat_param.numel(), self.lr, self.betas[0], self.betas[1], self.eps,
-                                                  self.weight_decay, P(self.step_state), float(grad_scale),
-                                                  1 if zero_grad else 0, stream)
+            coef_dev = None
+            if max_norm is not None:
+                rc = lib.c2v_grad_clip_coef(P(g), g.numel(), float(grad_scale), float(max_norm), P(self._norm_coef),
+                                            P(self._norm_ws), 4 * self._norm_ws.numel(), stream)
+                _lib.check(rc, "c2v_grad_clip_coef")
+                coef_dev = ctypes.c_void_p(self._norm_coef.data_ptr() + 4)
+            rc = lib.c2v_adam_step_ex(P(p), P(g), P(m), P(v), p.numel(), 0.0 if lr_dev else float(lr), beta1, beta2,
+                                      group["eps"], group["weight_decay"], step,
+                                      P(self.step_state) if self.capturable else None, float(grad_scale),
+                                      1 if zero_grad else 0, lr_dev, coef_dev, stream)
+        _lib.check(rc, "c2v_adam_step_ex")
+
+    # ---- checkpoints ---------------------------------------------------------------------------------------------------
+    def state_dict(self):
+        """torch.optim.Adam's state_dict for the same parameters in the order the caller passed them:
+        state[i] = {"step", "exp_avg", "exp_avg_sq"} (copies shaped like parameter i; step a tensor as in torch: on the
+        device and without a host read when capturable, a CPU fp32 scalar otherwise) and one group with integer
+        `params`, plus the key max_grad_norm.  torch.optim.Adam loads it and continues.  ShardedFlatAdam at world
+        size > 1: a collective, every rank returns the full dict."""
+        exp_avg, exp_avg_sq = self._gather_state()
+        if self.capturable:
+            step = self.step_state[0].to(torch.float32)
+        else:
+            step = torch.tensor(float(self.t), dtype=torch.float32)
+        params = self.param_groups[0]["params"]
+        state = {}
+        for i, (p, o) in enumerate(zip(params, self._flat_offsets)):
+            n = p.numel()
+            state[i] = {"step": step.clone(), "exp_avg": exp_avg[o:o + n].view_as(p).clone(),
+                        "exp_avg_sq": exp_avg_sq[o:o + n].view_as(p).clone()}
+        group = {k: (v.clone() if isinstance(v, torch.Tensor) else v) for k, v in self.param_groups[0].items()
+                 if k != "params"}
+        group["params"] = list(range(len(params)))
+        return {"state": state, "param_groups": [group]}
+
+    def load_state_dict(self, state_dict):
+        """Loads state_dict()'s output or torch.optim.Adam's for the same parameters.  The group's hyper-parameters are
+        taken over (a tensor lr is filled in place, capturable stays as constructed, max_grad_norm defaults to None),
+        the moments are copied into the flat buffers (at world size > 1: this rank's slices of them) and the step count
+        is set.  Parameters without state load as zeros and step 0; per-parameter steps that differ raise ValueError:
+        the flat kernel has one step count."""
+        groups = state_dict["param_groups"]
+        params = self.param_groups[0]["params"]
+        if len(groups) != 1 or len(groups[0]["params"]) != len(params):
+            raise ValueError(f"{type(self).__name__}.load_state_dict: expected one parameter group of {len(params)} "
+                             f"parameters, got {[len(g['params']) for g in groups]}")
+        saved = groups[0]
+        for k in ("amsgrad", "maximize", "decoupled_weight_decay"):
+            if saved.get(k):
+                raise ValueError(f"{type(self).__name__}.load_state_dict: {k}=True is not this optimizer's update rule")
+        state, steps = state_dict["state"], set()
+        exp_avg, exp_avg_sq = (torch.zeros(self._flat_numel, dtype=torch.float32, device=self._norm_coef.device)
+                               for _ in range(2))
+        for i, (p, o, key) in enumerate(zip(params, self._flat_offsets, saved["params"])):
+            st = state.get(key)
+            if not st:
+                steps.add(0)
+                continue
+            if tuple(st["exp_avg"].shape) != tuple(p.shape) or tuple(st["exp_avg_sq"].shape) != tuple(p.shape):
+                raise ValueError(f"{type(self).__name__}.load_state_dict: state {i} has shape "
+                                 f"{tuple(st['exp_avg'].shape)}, the parameter {tuple(p.shape)}")
+            n = p.numel()
+            exp_avg[o:o + n].copy_(st["exp_avg"].reshape(-1))
+            exp_avg_sq[o:o + n].copy_(st["exp_avg_sq"].reshape(-1))
+            steps.add(int(st["step"]))
+        if len(steps) != 1:
+            raise ValueError(f"{type(self).__name__}.load_state_dict: the parameters have different step counts "
+                             f"{sorted(steps)}; the flat kernel has one")
+        group = self.param_groups[0]
+        for k, v in saved.items():
+            if k in ("params", "capturable", "amsgrad", "maximize", "foreach", "differentiable", "fused",
+                     "decoupled_weight_decay"):             # ours, or torch.optim.Adam's switches
+                continue
+            if k == "lr":
+                self.lr = float(v)
+            elif k == "betas":
+                group[k] = (float(v[0]), float(v[1]))
             else:
-                self.t += 1
-                rc = lib.c2v_adam_step(P(self.flat_param), P(self.bucket.flat), P(self.exp_avg), P(self.exp_avg_sq),
-                                       self.flat_param.numel(), self.lr, self.betas[0], self.betas[1], self.eps,
-                                       self.weight_decay, self.t, float(grad_scale), 1 if zero_grad else 0, stream)
-        _lib.check(rc, "c2v_adam_step_capturable" if self.capturable else "c2v_adam_step")
+                group[k] = v.clone() if isinstance(v, torch.Tensor) else v
+        group["max_grad_norm"] = saved.get("max_grad_norm")
+        self._scatter_state(exp_avg, exp_avg_sq)
+        if self.capturable:
+            self.step_state[0] = steps.pop()
+        else:
+            self.t = steps.pop()
+
+
+class FlatAdam(_FlatAdamBase):
+    """torch.optim.Adam(model.parameters(), lr, betas, weight_decay) (main.py:138) as ONE kernel launch per step
+    (`c2v_adam_step`): parameters, like the gradients of `bucket`, become views into one flat buffer; the step reads
+    p, g, m, v once, writes p, m, v and leaves the gradient zeroed for the next backward (main.py:171), folding the
+    1/world of the data-parallel mean into the read.  Dense, same update rule and operation order as torch's Adam.
+
+    A torch.optim.Optimizer with one parameter group: the torch.optim.lr_scheduler classes drive `lr` (and OneCycleLR
+    `betas[0]`), and state_dict() / load_state_dict() interchange with torch.optim.Adam's.
+
+    capturable=True (torch.optim.Adam's flag): the step count lives on the device (`step_state`, see
+    c2v_adam_step_capturable) and every step, eager or inside a CUDA graph, runs the capturable kernels; `t` is then not
+    kept (read `step_count()`).  With capturable=False a step cannot be captured.  With capturable=True `lr` may be a
+    one-element fp32 device tensor, torch's convention: the step reads it on the device, so the replays of a captured
+    step follow a scheduler (which fills the tensor in place).  betas stay launch parameters, fixed at capture.
+
+    max_grad_norm: clip the gradient by its global L2 norm inside the step, as
+    torch.nn.utils.clip_grad_norm_(params, max_grad_norm) between the backward and the step would: the norm of
+    g * grad_scale over the whole bucket (after `bucket.allreduce` at world size > 1 every rank computes the same one),
+    coef = min(1, max_grad_norm / (norm + 1e-6)), Adam reads g * (grad_scale * coef), weight decay is added after the
+    clip.  One extra read of the bucket; no host read, so it is capturable.  A NaN or inf gradient gives NaN parameters,
+    as in torch.  `grad_norm` holds the last norm."""
+
+    def __init__(self, bucket, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, capturable=False,
+                 max_grad_norm=None):
+        self.bucket = bucket
+        self._init_optimizer(bucket.params, bucket.flat.device, lr, betas, eps, weight_decay, max_grad_norm, capturable)
+        flat = torch.empty_like(bucket.flat)
+        o, self._flat_offsets = 0, []
+        for p in bucket.params:                                  # same order as the gradient bucket
+            n = p.numel()
+            flat[o:o + n].copy_(p.data.reshape(-1))
+            p.data = flat[o:o + n].view_as(p)
+            self._flat_offsets.append(o)
+            o += n
+        self._flat_numel = o
+        self.flat_param = flat
+        self.exp_avg = torch.zeros_like(flat)
+        self.exp_avg_sq = torch.zeros_like(flat)
+        self.t = 0
+        self.step_state = _step_state(flat.device) if self.capturable else None
+
+    def step(self, grad_scale=1.0, zero_grad=True):
+        _check_capturable(self.capturable, "FlatAdam")
+        if not self.capturable:
+            self.t += 1
+        self._launch(self.flat_param, self.bucket.flat, self.exp_avg, self.exp_avg_sq, self.t, grad_scale, zero_grad)
         # the kernel wrote through raw pointers: tell autograd (and the weight-image caches of the model, which key on
         # Tensor._version) that every parameter changed, as an in-place torch op would
         for p in self.bucket.params:
             torch.autograd.graph.increment_version(p)
 
-    def zero_grad(self):
+    def zero_grad(self, set_to_none=False):
+        """zeroes the bucket; `.grad` stays a view of it whatever set_to_none says"""
         self.bucket.zero()
+
+    def _gather_state(self):
+        return self.exp_avg, self.exp_avg_sq
+
+    def _scatter_state(self, exp_avg, exp_avg_sq):
+        self.exp_avg.copy_(exp_avg)
+        self.exp_avg_sq.copy_(exp_avg_sq)
 
 
 def _step_state(device):
@@ -180,7 +349,7 @@ def nvls_allowed(transport, world):
     return False
 
 
-class ShardedFlatAdam:
+class ShardedFlatAdam(_FlatAdamBase):
     """Data-parallel Adam with the optimizer state sharded over the ranks and the gradient reduction fused into the
     optimizer kernel.  Same update rule, dense, as
     torch.optim.Adam (main.py:138) -- every rank ends a step with bit-identical parameters.
@@ -202,10 +371,18 @@ class ShardedFlatAdam:
       "nccl"  reduce_scatter -> `c2v_adam_step` on the slice -> all_gather (two NCCL collectives; the fallback when
               symmetric memory is unavailable, and what the gloo CPU tests drive with a stand-in kernel).
       "auto"  nvls or p2p, whichever is faster on this group (timed at construction), else nccl.
+
+    A torch.optim.Optimizer with one parameter group, like FlatAdam: lr schedulers, and state_dict() /
+    load_state_dict() in torch.optim.Adam's format.  At world size > 1 state_dict() is a collective (it all-gathers the
+    owned slices) that returns the full dict on every rank, and load_state_dict() keeps this rank's slices of the full
+    dict: a checkpoint saved at one world size loads at another.  At world size 1 a tensor `lr` (capturable=True) and
+    `max_grad_norm` work as in FlatAdam.  max_grad_norm at world size > 1 raises NotImplementedError: the fused kernel
+    reduces the gradient and applies Adam in one pass, so the norm of the reduced gradient does not exist before the
+    update; clipping there would be a two-phase kernel.
     """
 
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, group=None, transport="auto",
-                 early=(), capturable=False):
+                 early=(), capturable=False, max_grad_norm=None):
         params = [p for p in params if p.requires_grad]
         if not params:
             raise ValueError("no trainable parameters")
@@ -218,11 +395,14 @@ class ShardedFlatAdam:
         if capturable and self.world > 1:
             raise NotImplementedError("ShardedFlatAdam(capturable=True) supports one process only: the data-parallel step "
                                       f"uses cross-GPU barriers and a side stream (world size {self.world})")
-        self.capturable = bool(capturable)
-        self.lr, self.betas, self.eps, self.weight_decay = float(lr), (float(betas[0]), float(betas[1])), float(eps), float(weight_decay)
+        if max_grad_norm is not None and self.world > 1:
+            raise NotImplementedError("ShardedFlatAdam(max_grad_norm=...) supports one process only: the data-parallel "
+                                      "step reduces the gradient and applies Adam in one pass, so the norm of the reduced "
+                                      f"gradient does not exist before the update (world size {self.world})")
         dev, dt = self.params[0].device, self.params[0].dtype
         if dt != torch.float32:
             raise TypeError("parameters must be fp32")
+        self._init_optimizer(params, dev, lr, betas, eps, weight_decay, max_grad_norm, capturable)
         self.numel = sum(p.numel() for p in self.params)
         n_early = sum(p.numel() for p in first)
         # regions: (begin, length) in the flat buffers; region 0 = the early parameters (absent when there are none);
@@ -243,6 +423,9 @@ class ShardedFlatAdam:
                 o = self.regions[1][0]                           # region 1 starts after region 0's padding
             pos[i] = o
             o += p.numel()
+        flat_pos = {id(p): pos[i] for i, p in enumerate(self.params)}
+        self._flat_offsets = [flat_pos[id(p)] for p in params]      # in the caller's order, which state_dict() keeps
+        self._flat_numel = self.padded
         for i, p in enumerate(self.params):
             n, o = p.numel(), pos[i]
             self.flat_param[o:o + n].copy_(p.data.reshape(-1))
@@ -330,30 +513,32 @@ class ShardedFlatAdam:
     def state_bytes(self):
         return 4 * (2 * self.state_numel)
 
-    def zero_grad(self):
+    def zero_grad(self, set_to_none=False):
+        """zeroes the current bucket; `.grad` stays a view of it whatever set_to_none says"""
         self.buckets[self.cur].zero_()
+
+    def _gather_state(self):
+        """the full flat exp_avg / exp_avg_sq [padded]: at world size > 1 every region's slices, all-gathered"""
+        if self.world == 1:
+            return self.exp_avg, self.exp_avg_sq
+        full = []
+        for own in (self.exp_avg, self.exp_avg_sq):
+            out = torch.empty(self.padded, dtype=own.dtype, device=own.device)
+            for (rb, rn), (lo, n, so) in zip(self.regions, self.slices):
+                dist.all_gather_into_tensor(out[rb:rb + rn], own[so:so + n].clone(), group=self.group)
+            full.append(out)
+        return full
+
+    def _scatter_state(self, exp_avg, exp_avg_sq):
+        for lo, n, so in self.slices:
+            self.exp_avg[so:so + n].copy_(exp_avg[lo:lo + n])
+            self.exp_avg_sq[so:so + n].copy_(exp_avg_sq[lo:lo + n])
 
     # ---- the step -----------------------------------------------------------------------------------------------------
     def _adam_slice(self, p_slice, g_slice, zero_grad=False, state=None):
-        """c2v_adam_step on an owned slice (the gloo CPU tests replace this method with a torch stand-in)"""
-        import ctypes
-        from . import _lib
-        lib = _lib.load()
-        P = lambda t: ctypes.c_void_p(t.data_ptr())
+        """the flat step on an owned slice (the gloo CPU tests replace this method with a torch stand-in)"""
         m, v = state if state is not None else (self.exp_avg, self.exp_avg_sq)
-        dev = p_slice.device
-        with torch.cuda.device(dev):
-            if self.capturable:                               # (world 1 only)
-                rc = lib.c2v_adam_step_capturable(P(p_slice), P(g_slice), P(m), P(v), p_slice.numel(), self.lr, self.betas[0],
-                                                  self.betas[1], self.eps, self.weight_decay, P(self.step_state), 1.0,
-                                                  1 if zero_grad else 0,
-                                                  ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
-                _lib.check(rc, "c2v_adam_step_capturable")
-                return
-            rc = lib.c2v_adam_step(P(p_slice), P(g_slice), P(m), P(v), p_slice.numel(), self.lr,
-                                   self.betas[0], self.betas[1], self.eps, self.weight_decay, self.t, 1.0 / self.world,
-                                   1 if zero_grad else 0, ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
-        _lib.check(rc, "c2v_adam_step")
+        self._launch(p_slice, g_slice, m, v, self.t, 1.0 / self.world, zero_grad)
 
     def _reduce_scatter(self, out, full):
         try:
@@ -427,6 +612,8 @@ class ShardedFlatAdam:
         _check_capturable(self.capturable, "ShardedFlatAdam")
         if self.transport == "nvls":             # the switch may have been turned on after the construction chose "nvls"
             nvls_allowed("nvls", self.world)
+        if self.world > 1 and self.max_grad_norm is not None:
+            raise NotImplementedError("ShardedFlatAdam: max_grad_norm supports one process only")
         cur, nxt = self.cur, 1 - self.cur
         if not self._early_done and not self.capturable:
             self.t += 1

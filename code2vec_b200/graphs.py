@@ -12,7 +12,9 @@ static inputs, copy in and replay) to a Code2Vec step:
 What a captured step needs (checked, each with a clear error): dropout keys drawn on the device
 (Code2Vec.use_device_rng), an optimizer whose step count lives on the device (FlatAdam / ShardedFlatAdam with
 capturable=True at world size 1, or torch.optim.Adam(capturable=True)), dense embedding gradients and padded [B, L]
-batches.  Hyper-parameters, model.training and torch's TF32 matmul switch are fixed at capture.  See INTEGRATION.md, "CUDA graphs".
+batches.  Hyper-parameters, model.training and torch's TF32 matmul switch are fixed at capture, except a tensor `lr`
+(FlatAdam / ShardedFlatAdam, as for torch's capturable optimizers), which the step reads on the device so that a
+learning-rate scheduler can drive the replays.  See INTEGRATION.md, "CUDA graphs".
 """
 import torch
 
@@ -110,7 +112,8 @@ class GraphedTrainStep(_Graphed):
     def _settings(self):
         o = self.optimizer
         if isinstance(o, (FlatAdam, ShardedFlatAdam)):
-            hyper = (o.lr, o.betas, o.eps, o.weight_decay)
+            # a tensor lr is read on the device at every replay (a scheduler fills it); the rest are launch parameters
+            hyper = (None if isinstance(o.lr, torch.Tensor) else o.lr, o.betas, o.eps, o.weight_decay, o.max_grad_norm)
         else:
             hyper = tuple(tuple((k, v) for k, v in sorted(g.items()) if k != "params" and not isinstance(v, torch.Tensor))
                           for g in o.param_groups)

@@ -665,6 +665,27 @@ int c2v_adam_step_capturable(float *param, float *grad, float *exp_avg, float *e
                              float beta1, float beta2, float eps, float weight_decay, void *step_state, float grad_scale,
                              int32_t zero_grad, void *stream);
 
+/* Gradient clipping by global L2 norm for the flat step: torch.nn.utils.clip_grad_norm_(params, max_norm, norm_type=2.0,
+ * error_if_nonfinite=False) on the gradient Adam sees.  One pass over grad [n] (fp32, 16-byte aligned) and a one-warp
+ * finalize write out_norm_coef (device, 2 floats) = {norm, coef}: norm = |grad_scale| * ||grad||_2 and
+ * coef = min(1, max_norm / (norm + 1e-6)); a NaN norm gives a NaN coef, an inf norm gives 0.  Per-CTA partial sums of
+ * squares (fp32) are added in a fixed order in double, the grid depends on n alone: the same gradient gives the same
+ * bits.  grad is not modified; pass out_norm_coef + 1 as coef_dev of c2v_adam_step_ex.  workspace: device,
+ * c2v_grad_norm_workspace_bytes(n) bytes (0 for n < 1), needs no initialisation.  max_norm > 0.  Two launches, no host
+ * read: capturable. */
+size_t c2v_grad_norm_workspace_bytes(int64_t n);
+int c2v_grad_clip_coef(const float *grad, int64_t n, float grad_scale, float max_norm, float *out_norm_coef,
+                       void *workspace, size_t workspace_bytes, void *stream);
+/* c2v_adam_step (step_state NULL: `step` is the 1-based step count) or c2v_adam_step_capturable (step_state not NULL:
+ * `step` is ignored) with two optional device scalars (fp32, 4-byte aligned, NULL: absent):
+ *   coef_dev  the gradient is read as grad * (grad_scale * *coef_dev): the clip coefficient of c2v_grad_clip_coef;
+ *   lr_dev    the step-count kernel reads the learning rate from *lr_dev instead of `lr` (needs step_state), so that the
+ *             replays of a captured step follow a learning-rate schedule written there between them.
+ * With both NULL the call is c2v_adam_step / c2v_adam_step_capturable: same kernels, same launch parameters. */
+int c2v_adam_step_ex(float *param, float *grad, float *exp_avg, float *exp_avg_sq, int64_t n, float lr, float beta1,
+                     float beta2, float eps, float weight_decay, int64_t step, void *step_state, float grad_scale,
+                     int32_t zero_grad, const float *lr_dev, const float *coef_dev, void *stream);
+
 /* The same optimizer for data-parallel training, fused with its collective (the reference's
  * one all_reduce per step becomes one kernel per rank): for the rank's slice [slice_begin, slice_begin + slice_n) of the flat buffers the kernel
  * (1) sums the gradients of all ranks -- `multimem.ld_reduce` on grad_multicast (NVSwitch in-switch reduction) or, when
