@@ -170,6 +170,11 @@ SYMBOLS = {
                                                          c_vp, c_sz, c_i32, c_vp]),
     "c2v_sparse_adam_step": (ctypes.c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_i32, ctypes.c_double,
                                             ctypes.c_double, ctypes.c_double, ctypes.c_double, c_i64, c_vp]),
+    "c2v_sparse_union_rows_workspace_bytes": (c_sz, [c_i64]),
+    "c2v_sparse_union_rows": (ctypes.c_int, [c_vp, c_vp, c_i32, c_i64, c_i64, c_vp, c_vp, c_vp, c_sz, c_vp]),
+    "c2v_sparse_adam_step_merged": (ctypes.c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_i64, c_vp, c_vp, c_i64, c_i32,
+                                                   c_f32, ctypes.c_double, ctypes.c_double, ctypes.c_double,
+                                                   ctypes.c_double, c_i64, c_vp]),
     "c2v_session_create": (ctypes.c_int, [ctypes.c_int, _P(Dims), c_i32, c_i32, _P(c_vp)]),
     "c2v_session_destroy": (None, [c_vp]),
     "c2v_forward_host": (ctypes.c_int, [c_vp, _P(Params), c_vp, c_vp, c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp,

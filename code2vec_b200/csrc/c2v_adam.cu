@@ -338,6 +338,20 @@ adam_step_bulk_kernel(const float *__restrict__ p_local, const AdamPeers peers, 
 // torch.optim._functional.sparse_adam on the rows of a coalesced gradient, every operation rounded as torch rounds it
 // (the _rn intrinsics keep nvcc from contracting a multiply and an add into one fma).  One warp per gradient row.
 // ------------------------------------------------------------------------------------------------------------------
+// element c of a row: gg is its gradient
+__device__ __forceinline__ void sparse_adam_update(float gg, float *pr, float *mr, float *vr, int c, float neg_step_size,
+                                                   float one_minus_b1, float one_minus_b2, float eps)
+{
+    const float m0 = mr[c], v0 = vr[c];
+    const float u1 = __fmul_rn(__fsub_rn(gg, m0), one_minus_b1);              // (g - m) * (1 - b1)
+    const float u2 = __fmul_rn(__fsub_rn(__fmul_rn(gg, gg), v0), one_minus_b2); // (g^2 - v) * (1 - b2)
+    mr[c] = __fadd_rn(m0, u1);
+    vr[c] = __fadd_rn(v0, u2);
+    const float numer = __fadd_rn(u1, m0);
+    const float denom = __fadd_rn(__fsqrt_rn(__fadd_rn(u2, v0)), eps);
+    pr[c] = __fadd_rn(pr[c], __fmul_rn(neg_step_size, __fdiv_rn(numer, denom)));
+}
+
 __global__ void __launch_bounds__(256)
 sparse_adam_step_kernel(float *__restrict__ p, float *__restrict__ m, float *__restrict__ v, const float *__restrict__ g,
                         const long long *__restrict__ rows, long long U, long long n_rows, int E, float neg_step_size,
@@ -350,16 +364,65 @@ sparse_adam_step_kernel(float *__restrict__ p, float *__restrict__ m, float *__r
         if (r < 0 || r >= n_rows) continue;
         const float *gi = g + (size_t)i * E;
         float *pr = p + (size_t)r * E, *mr = m + (size_t)r * E, *vr = v + (size_t)r * E;
-        for (int c = lane; c < E; c += 32) {
-            const float gg = gi[c], m0 = mr[c], v0 = vr[c];
-            const float u1 = __fmul_rn(__fsub_rn(gg, m0), one_minus_b1);              // (g - m) * (1 - b1)
-            const float u2 = __fmul_rn(__fsub_rn(__fmul_rn(gg, gg), v0), one_minus_b2); // (g^2 - v) * (1 - b2)
-            mr[c] = __fadd_rn(m0, u1);
-            vr[c] = __fadd_rn(v0, u2);
-            const float numer = __fadd_rn(u1, m0);
-            const float denom = __fadd_rn(__fsqrt_rn(__fadd_rn(u2, v0)), eps);
-            pr[c] = __fadd_rn(pr[c], __fmul_rn(neg_step_size, __fdiv_rn(numer, denom)));
+        for (int c = lane; c < E; c += 32)
+            sparse_adam_update(gi[c], pr, mr, vr, c, neg_step_size, one_minus_b1, one_minus_b2, eps);
+    }
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// The data-parallel SparseAdam step: the W ranks' row lists rows [W, u_max] (list r ascending, valid up to counts[r])
+// and values [W, u_max, E], all-gathered, are merged into one gradient row by row and applied with
+// sparse_adam_update, without writing the merged gradient.  One warp per row of the union (c2v_sparse_union_rows; its
+// size U is read here, the grid covers the host-known capacity): the lanes binary-search the W lists for the row (lane
+// l searches ranks l, l + 32, ...) and leave the positions in shared memory; then every lane adds its columns' rank rows
+// in rank order, starting from the first rank that has the row, and multiplies the sum by `scale` (+-1/W, negative
+// under maximize).  No atomics: every replica computes the same bits.
+// ------------------------------------------------------------------------------------------------------------------
+constexpr int SPM_THREADS = 256;
+
+__global__ void __launch_bounds__(SPM_THREADS)
+sparse_adam_merged_kernel(float *__restrict__ p, float *__restrict__ m, float *__restrict__ v,
+                          const float *__restrict__ values, const long long *__restrict__ rows,
+                          const long long *__restrict__ counts, int world, long long u_max,
+                          const long long *__restrict__ union_rows, const long long *__restrict__ union_count,
+                          long long capacity, long long n_rows, int E, float scale, float neg_step_size,
+                          float one_minus_b1, float one_minus_b2, float eps)
+{
+    extern __shared__ int spm_pos[];                        // [warps per CTA][world]: position of the row in list r, or -1
+    const int lane = threadIdx.x & 31;
+    int *pos = spm_pos + (threadIdx.x >> 5) * world;
+    long long U = *union_count;
+    if (U > capacity) U = capacity;
+    const long long n_warps = (long long)gridDim.x * (blockDim.x >> 5);
+    for (long long i = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); i < U; i += n_warps) {
+        const long long r = union_rows[i];
+        if (r < 0 || r >= n_rows) continue;
+        for (int k = lane; k < world; k += 32) {             // lower bound of r in list k
+            const long long *lst = rows + (size_t)k * u_max;
+            long long lo = 0, hi = counts[k];
+            if (hi > u_max) hi = u_max;
+            if (hi < 0) hi = 0;
+            while (lo < hi) {
+                const long long mid = (lo + hi) >> 1;
+                if (lst[mid] < r) lo = mid + 1; else hi = mid;
+            }
+            pos[k] = (lo < (counts[k] < u_max ? counts[k] : u_max) && lst[lo] == r) ? (int)lo : -1;
         }
+        __syncwarp();
+        float *pr = p + (size_t)r * E, *mr = m + (size_t)r * E, *vr = v + (size_t)r * E;
+        for (int c = lane; c < E; c += 32) {
+            float acc = 0.0f;
+            bool any = false;
+            for (int k = 0; k < world; ++k) {
+                const int j = pos[k];
+                if (j < 0) continue;
+                const float x = values[((size_t)k * u_max + j) * E + c];
+                acc = any ? __fadd_rn(acc, x) : x;
+                any = true;
+            }
+            sparse_adam_update(__fmul_rn(acc, scale), pr, mr, vr, c, neg_step_size, one_minus_b1, one_minus_b2, eps);
+        }
+        __syncwarp();                                        // pos is rewritten for the warp's next row
     }
 }
 
@@ -638,5 +701,49 @@ extern "C" int c2v_sparse_adam_step(float *param, float *exp_avg, float *exp_avg
         param, exp_avg, exp_avg_sq, values, reinterpret_cast<const long long *>(rows), U, n_rows, E, (float)(-step_size),
         (float)(1.0 - beta1), (float)(1.0 - beta2), (float)eps);
     C2V_LAUNCH_OK("sparse_adam_step_kernel");
+    return C2V_OK;
+}
+
+static const int32_t MERGED_WORLD_MAX = 1024;               // as c2v_sparse_union_rows: 32 KB of positions per CTA
+
+extern "C" int c2v_sparse_adam_step_merged(float *param, float *exp_avg, float *exp_avg_sq, const float *values,
+                                           const int64_t *rows, const int64_t *counts, int32_t world, int64_t u_max,
+                                           const int64_t *union_rows, const int64_t *union_count, int64_t n_rows,
+                                           int32_t E, float scale, double lr, double beta1, double beta2, double eps,
+                                           int64_t step, void *stream)
+{
+    if (world < 1 || world > MERGED_WORLD_MAX || u_max < 0 || u_max > n_rows || n_rows < 1 || n_rows >= (1LL << 31) ||
+        E < 1 || E > 65536 || step < 1) {
+        set_error("c2v_sparse_adam_step_merged: bad argument (world = %d, u_max = %lld, n_rows = %lld, E = %d, "
+                  "step = %lld)", world, (long long)u_max, (long long)n_rows, E, (long long)step);
+        return C2V_EINVAL;
+    }
+    if (!param || !exp_avg || !exp_avg_sq || !counts || !union_count || (u_max > 0 && (!values || !rows || !union_rows))) {
+        set_error("c2v_sparse_adam_step_merged: NULL pointer argument");
+        return C2V_EINVAL;
+    }
+    if (misaligned(param, 4) || misaligned(exp_avg, 4) || misaligned(exp_avg_sq, 4) || misaligned(values, 4) ||
+        misaligned(rows, 8) || misaligned(counts, 8) || misaligned(union_rows, 8) || misaligned(union_count, 8)) {
+        set_error("c2v_sparse_adam_step_merged: misaligned pointer (float buffers: 4 bytes, rows, counts, union_rows, "
+                  "union_count: 8)");
+        return C2V_EINVAL;
+    }
+    // the union has at most min(n_rows, world * u_max) rows: the grid covers that many, the kernel reads U
+    const long long capacity = (long long)world * u_max < n_rows ? (long long)world * u_max : n_rows;
+    if (capacity == 0) return C2V_OK;
+    const double bc1 = 1.0 - pow(beta1, (double)step), bc2 = 1.0 - pow(beta2, (double)step);
+    const double step_size = lr * sqrt(bc2) / bc1;          // as c2v_sparse_adam_step
+    int dev = 0, sms = 0;
+    C2V_CUDA_OK(cudaGetDevice(&dev));
+    C2V_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    long long blocks = (capacity + SPM_THREADS / 32 - 1) / (SPM_THREADS / 32);
+    if (blocks > (long long)sms * 8) blocks = (long long)sms * 8;
+    const size_t smem = (size_t)(SPM_THREADS / 32) * world * sizeof(int);
+    sparse_adam_merged_kernel<<<(unsigned)blocks, SPM_THREADS, smem, static_cast<cudaStream_t>(stream)>>>(
+        param, exp_avg, exp_avg_sq, values, reinterpret_cast<const long long *>(rows),
+        reinterpret_cast<const long long *>(counts), world, u_max, reinterpret_cast<const long long *>(union_rows),
+        reinterpret_cast<const long long *>(union_count), capacity, n_rows, E, scale, (float)(-step_size),
+        (float)(1.0 - beta1), (float)(1.0 - beta2), (float)eps);
+    C2V_LAUNCH_OK("sparse_adam_merged_kernel");
     return C2V_OK;
 }

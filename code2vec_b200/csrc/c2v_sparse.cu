@@ -9,6 +9,8 @@
 //            writes slot[row] (-1 for unmarked rows) and rows[slot] = row
 // Out-of-range indices count as row 0: the encode reads them as row 0 (and reports them), so row 0 receives their
 // gradient.
+// c2v_sparse_union_rows runs the same count / scan / compact passes behind a mark pass of its own over the W row lists
+// that the ranks of a data-parallel step all-gathered: their union, ascending, and its size on the device.
 #include "c2v_common.cuh"
 
 namespace c2v {
@@ -25,6 +27,21 @@ sparse_mark_kernel(const long long *__restrict__ ia, long long na, const long lo
         long long v = i < na ? ia[i] : ib[i - na];
         if (v < 0 || v >= vocab) v = 0;
         flag[v] = 1;
+    }
+}
+
+// The mark pass of c2v_sparse_union_rows: the W padded row lists [W, u_max] of a data-parallel exchange, list r valid up
+// to counts[r] (clamped to [0, u_max]); padding is never read.  Rows outside [0, vocab) are not marked: no rank's step
+// can apply them (c2v_sparse_adam_step skips them too).
+__global__ void __launch_bounds__(256)
+sparse_union_mark_kernel(const long long *__restrict__ rows, const long long *__restrict__ counts, int world,
+                         long long u_max, long long vocab, uint8_t *__restrict__ flag)
+{
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < world * u_max; i += (long long)gridDim.x * blockDim.x) {
+        const long long r = i / u_max, j = i - r * u_max;
+        if (j >= counts[r]) continue;                        // (a negative count marks nothing)
+        const long long v = rows[i];
+        if (v >= 0 && v < vocab) flag[v] = 1;
     }
 }
 
@@ -126,6 +143,19 @@ using namespace c2v;
 
 static bool sr_misaligned(const void *ptr, uintptr_t a) { return (reinterpret_cast<uintptr_t>(ptr) & (a - 1)) != 0; }
 
+// the passes behind the mark: count, scan and compact of the marked flags into rows / *count (and slot)
+static int sr_count_scan_compact(const uint8_t *flag, long long *chunk, long long n_chunks, long long vocab, int *slot,
+                                 long long *rows, long long *count, cudaStream_t st)
+{
+    sparse_count_kernel<<<(unsigned)n_chunks, srows::THREADS, 0, st>>>(flag, chunk);
+    C2V_LAUNCH_OK("sparse_count_kernel");
+    sparse_scan_kernel<<<1, srows::THREADS, 0, st>>>(chunk, (int)n_chunks, count);
+    C2V_LAUNCH_OK("sparse_scan_kernel");
+    sparse_compact_kernel<<<(unsigned)n_chunks, srows::THREADS, 0, st>>>(flag, chunk, vocab, slot, rows);
+    C2V_LAUNCH_OK("sparse_compact_kernel");
+    return C2V_OK;
+}
+
 extern "C" size_t c2v_sparse_rows_workspace_bytes(int64_t vocab)
 {
     if (vocab < 1 || vocab >= (1LL << 31)) return 0;
@@ -170,12 +200,63 @@ extern "C" int c2v_sparse_rows(const int64_t *idx_a, int64_t n_a, const int64_t 
                                                             reinterpret_cast<const long long *>(idx_b), n_b, vocab, flag);
         C2V_LAUNCH_OK("sparse_mark_kernel");
     }
-    sparse_count_kernel<<<(unsigned)n_chunks, srows::THREADS, 0, st>>>(flag, chunk);
-    C2V_LAUNCH_OK("sparse_count_kernel");
-    sparse_scan_kernel<<<1, srows::THREADS, 0, st>>>(chunk, (int)n_chunks, reinterpret_cast<long long *>(count));
-    C2V_LAUNCH_OK("sparse_scan_kernel");
-    sparse_compact_kernel<<<(unsigned)n_chunks, srows::THREADS, 0, st>>>(flag, chunk, vocab, slot,
-                                                                        reinterpret_cast<long long *>(rows));
-    C2V_LAUNCH_OK("sparse_compact_kernel");
-    return C2V_OK;
+    return sr_count_scan_compact(flag, chunk, n_chunks, vocab, slot, reinterpret_cast<long long *>(rows),
+                                 reinterpret_cast<long long *>(count), st);
+}
+
+static const int64_t UNION_WORLD_MAX = 1024;
+
+// [0, sparse_rows_ws) the workspace of c2v_sparse_rows | slot map int32 [vocab] (written by the compact pass, not used)
+static size_t union_rows_ws(long long vocab) { return sparse_rows_ws(vocab) + align_up((size_t)vocab * 4, 256); }
+
+extern "C" size_t c2v_sparse_union_rows_workspace_bytes(int64_t vocab)
+{
+    if (vocab < 1 || vocab >= (1LL << 31)) return 0;
+    return union_rows_ws(vocab);
+}
+
+extern "C" int c2v_sparse_union_rows(const int64_t *rows, const int64_t *counts, int32_t world, int64_t u_max,
+                                     int64_t vocab, int64_t *union_rows, int64_t *union_count, void *workspace,
+                                     size_t workspace_bytes, void *stream)
+{
+    if (vocab < 1 || vocab >= (1LL << 31)) {
+        set_error("c2v_sparse_union_rows: vocab = %lld outside [1, 2^31)", (long long)vocab);
+        return C2V_EINVAL;
+    }
+    if (world < 1 || world > UNION_WORLD_MAX || u_max < 0 || u_max > vocab) {
+        set_error("c2v_sparse_union_rows: world = %d outside [1, %lld] or u_max = %lld outside [0, vocab = %lld]", world,
+                  (long long)UNION_WORLD_MAX, (long long)u_max, (long long)vocab);
+        return C2V_EINVAL;
+    }
+    if ((u_max > 0 && (!rows || !union_rows)) || !counts || !union_count || !workspace) {
+        set_error("c2v_sparse_union_rows: NULL pointer argument");
+        return C2V_EINVAL;
+    }
+    if (sr_misaligned(rows, 8) || sr_misaligned(counts, 8) || sr_misaligned(union_rows, 8) ||
+        sr_misaligned(union_count, 8) || sr_misaligned(workspace, 16)) {
+        set_error("c2v_sparse_union_rows: misaligned pointer (rows, counts, union_rows, union_count: 8 bytes, "
+                  "workspace: 16)");
+        return C2V_EINVAL;
+    }
+    const size_t need = union_rows_ws(vocab);
+    if (workspace_bytes < need) {
+        set_error("c2v_sparse_union_rows: workspace too small: %zu < %zu", workspace_bytes, need);
+        return C2V_EWORKSPACE;
+    }
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const long long n_chunks = sr_chunks(vocab);
+    uint8_t *flag = static_cast<uint8_t *>(workspace);
+    long long *chunk = reinterpret_cast<long long *>(flag + align_up((size_t)n_chunks * srows::CHUNK, 256));
+    int *slot = reinterpret_cast<int *>(static_cast<uint8_t *>(workspace) + sparse_rows_ws(vocab));
+    C2V_CUDA_OK(cudaMemsetAsync(flag, 0, (size_t)n_chunks * srows::CHUNK, st));
+    if (u_max > 0) {
+        long long blocks = (world * u_max + 255) / 256;
+        if (blocks > 4096) blocks = 4096;
+        sparse_union_mark_kernel<<<(unsigned)blocks, 256, 0, st>>>(reinterpret_cast<const long long *>(rows),
+                                                                   reinterpret_cast<const long long *>(counts), world,
+                                                                   u_max, vocab, flag);
+        C2V_LAUNCH_OK("sparse_union_mark_kernel");
+    }
+    return sr_count_scan_compact(flag, chunk, n_chunks, vocab, slot, reinterpret_cast<long long *>(union_rows),
+                                 reinterpret_cast<long long *>(union_count), st);
 }

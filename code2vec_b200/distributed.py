@@ -704,8 +704,88 @@ class FusedSparseAdam(torch.optim.SparseAdam):
     overridden: parameter groups, hyper-parameter checks and state_dict are torch's and interchange with
     torch.optim.SparseAdam in both directions.  For the embedding tables of a Code2Vec whose `.sparse` is set (see
     INTEGRATION.md, "Sparse embedding gradients").  Lazy Adam: rows a batch does not touch keep their moments and do not
-    move, unlike the dense torch.optim.Adam of the reference.  Single process only: a data-parallel reduction of sparse
-    gradients is not implemented, and without one the replicas would drift apart."""
+    move, unlike the dense torch.optim.Adam of the reference.
+
+    Data-parallel training (`group`: the process group, default the world; an attribute, not a group default, so
+    state_dict() is unchanged): at world size > 1 step() first reduces each parameter's sparse gradient over the group
+    and then takes one SparseAdam step on the result, the same on every rank, so parameters and state stay replicated
+    bit for bit.  The reduced gradient holds the union of the ranks' rows, ascending, each the fp32 sum of the ranks that
+    touched it, in rank order, times the fp32 1/W (the mean, as for the dense parameters).  A parameter whose gradient is
+    None on every rank is skipped; one with a gradient on some ranks is stepped on all, a None gradient counting as an
+    empty one.  One all-gather of every parameter's row count (read on the host, to size the buffers), then per
+    parameter an all-gather of its rows and of its values, each padded to the largest count, and
+    `c2v_sparse_union_rows` + `c2v_sparse_adam_step_merged`, which merge the lists inside the update."""
+
+    def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, maximize=False, group=None):
+        super().__init__(params, lr=lr, betas=betas, eps=eps, maximize=maximize)
+        self.group = group
+
+    def _world_size(self):
+        return dist.get_world_size(self.group) if dist.is_available() and dist.is_initialized() else 1
+
+    def _all_gather(self, t):
+        """[W, *t.shape]: every rank's `t` in rank order (the collective of the data-parallel step; the one-GPU tests
+        replace this method)"""
+        world = self._world_size()
+        out = t.new_empty(world * t.numel())
+        dist.all_gather_into_tensor(out, t.contiguous().reshape(-1), group=self.group)
+        return out.view((world,) + tuple(t.shape))
+
+    def _merged_step(self, p, state, rows, values, counts, lr, beta1, beta2, eps, scale):
+        """the union of the gathered row lists and the merged SparseAdam step on it, on the device (the gloo CPU tests
+        replace this method with a torch restatement)"""
+        from . import functional as CF
+        union, count = CF.sparse_union_rows(rows, counts, p.shape[0])
+        CF.sparse_adam_step_merged(p, state["exp_avg"], state["exp_avg_sq"], values, rows, counts, union, count, lr,
+                                   beta1, beta2, eps, state["step"], scale)
+
+    def _step_data_parallel(self, world):
+        entries, local = [], []
+        for group in self.param_groups:
+            for p in group["params"]:
+                grad = p.grad
+                if grad is not None:
+                    if not grad.is_sparse:
+                        raise RuntimeError("SparseAdam does not support dense gradients, please consider Adam instead")
+                    if not grad.is_coalesced():
+                        grad = grad.coalesce()
+                    if grad.sparse_dim() != 1:
+                        raise NotImplementedError("FusedSparseAdam: gradients must be sparse in the first dimension "
+                                                  "only (row-sparse, as nn.Embedding(sparse=True) produces)")
+                entries.append((group, p, grad))
+                local.append(-1 if grad is None else grad._nnz())
+        if not entries:
+            return
+        counts = self._all_gather(torch.tensor(local, dtype=torch.int64, device=entries[0][1].device))
+        host = counts.cpu()                                  # the step's one host wait: it sizes the exchange buffers
+        inv_world = float(torch.tensor(1.0 / world, dtype=torch.float32))
+        for i, (group, p, grad) in enumerate(entries):
+            col = host[:, i]
+            if bool((col < 0).all()):                        # None on every rank: skipped, as torch skips it
+                continue
+            state = self.state[p]
+            if len(state) == 0:
+                state["step"] = 0
+                state["exp_avg"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+                state["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+            state["step"] += 1
+            u_max = int(col.max())
+            if u_max == 0:                                   # an empty union: the step still counts
+                continue
+            E = p[0].numel()
+            rows = torch.zeros(u_max, dtype=torch.int64, device=p.device)
+            values = torch.zeros((u_max, E), dtype=p.dtype, device=p.device)
+            n = int(local[i]) if grad is not None else 0
+            if n:
+                rows[:n] = grad._indices()[0]
+                values[:n] = grad._values().reshape(n, E)
+            lr = group["lr"]
+            lr = float(lr.item()) if isinstance(lr, torch.Tensor) else float(lr)
+            beta1, beta2 = group["betas"]
+            scale = -inv_world if group.get("maximize", False) else inv_world
+            self._merged_step(p, state, self._all_gather(rows), self._all_gather(values), counts[:, i].contiguous(), lr,
+                              beta1, beta2, group["eps"], scale)
+            torch.autograd.graph.increment_version(p)        # raw-pointer writes: bump the version counter
 
     @torch.no_grad()
     def step(self, closure=None):
@@ -714,9 +794,10 @@ class FusedSparseAdam(torch.optim.SparseAdam):
         if closure is not None:
             with torch.enable_grad():
                 loss = closure()
-        if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
-            raise NotImplementedError("FusedSparseAdam: sparse gradients are not reduced across processes "
-                                      f"(world size {dist.get_world_size()}); use one process or dense gradients")
+        world = self._world_size()
+        if world > 1:
+            self._step_data_parallel(world)
+            return loss
         for group in self.param_groups:
             beta1, beta2 = group["betas"]
             maximize = group.get("maximize", False)

@@ -883,3 +883,63 @@ def sparse_adam_step(param, exp_avg, exp_avg_sq, values, rows, lr, beta1, beta2,
         rc = lib.c2v_sparse_adam_step(_ptr(param), _ptr(exp_avg), _ptr(exp_avg_sq), _ptr(values), _ptr(rows), rows.numel(),
                                       n, E, float(lr), float(beta1), float(beta2), float(eps), int(step), _stream(dev))
         _lib.check(rc, "c2v_sparse_adam_step")
+
+
+def _gathered_lists(rows, counts):
+    rows = _idx(rows, "rows")
+    counts = _idx(counts, "counts")
+    if rows.dim() != 2 or tuple(counts.shape) != (rows.shape[0],):
+        raise ValueError(f"rows must be [world, u_max] and counts [world], got {tuple(rows.shape)} and "
+                         f"{tuple(counts.shape)}")
+    return rows, counts
+
+
+def sparse_union_rows(rows, counts, vocab):
+    """The union of W ascending row lists (c2v_sparse_union_rows): rows int64 [W, u_max], list r valid up to counts[r]
+    (int64 [W], on the device; negative = empty), as the ranks of a data-parallel step all-gathered them ->
+    (union_rows int64 [min(vocab, W * u_max)] whose first U entries are the union, ascending, count int64 [1] = U), on
+    the device and enqueued on the current stream; U is not read on the host."""
+    lib = _lib.load()
+    rows, counts = _gathered_lists(rows, counts)
+    _need_cuda(rows, counts)
+    world, u_max, vocab = rows.shape[0], rows.shape[1], int(vocab)
+    nbytes = lib.c2v_sparse_union_rows_workspace_bytes(vocab)
+    if nbytes == 0:
+        raise ValueError(f"sparse_union_rows: vocab = {vocab} outside [1, 2^31)")
+    dev = rows.device
+    with torch.cuda.device(dev):
+        union = _empty((min(vocab, world * u_max),), torch.int64, dev)
+        count = _empty((1,), torch.int64, dev)
+        ws = _empty((nbytes,), torch.uint8, dev)
+        rc = lib.c2v_sparse_union_rows(_ptr(rows) if u_max else None, _ptr(counts), world, u_max, vocab,
+                                       _ptr(union) if union.numel() else None, _ptr(count), _ptr(ws), nbytes, _stream(dev))
+        _lib.check(rc, "c2v_sparse_union_rows")
+    return union, count
+
+
+def sparse_adam_step_merged(param, exp_avg, exp_avg_sq, values, rows, counts, union_rows, union_count, lr, beta1,
+                            beta2, eps, step, scale):
+    """sparse_adam_step on the merged gradient of W ranks (c2v_sparse_adam_step_merged): values fp32 [W, u_max, E] and
+    rows / counts as in sparse_union_rows, union_rows / union_count what it returned for them.  Each union row's gradient
+    is the sum of the ranks' rows, in fp32 in rank order, times `scale` (the fp32 1/W of the mean, negated for
+    maximize); it is applied without being written.  No host read."""
+    lib = _lib.load()
+    _need_cuda(param, exp_avg, exp_avg_sq, values, rows, counts, union_rows, union_count)
+    for t, name in ((param, "param"), (exp_avg, "exp_avg"), (exp_avg_sq, "exp_avg_sq")):
+        if t.dtype != torch.float32 or not t.is_contiguous() or t.shape != param.shape:
+            raise TypeError(f"{name} must be contiguous fp32 of the parameter's shape")
+    rows, counts = _gathered_lists(rows, counts)
+    n, E = param.shape[0], param[0].numel()
+    world, u_max = rows.shape
+    values = _f32c(values, "values")
+    if values.numel() != world * u_max * E:
+        raise ValueError(f"sparse_adam_step_merged: values has {values.numel()} elements, rows {tuple(rows.shape)} with "
+                         f"E = {E} need {world * u_max * E}")
+    union_rows, union_count = _idx(union_rows, "union_rows"), _idx(union_count, "union_count")
+    dev = param.device
+    with torch.cuda.device(dev):
+        rc = lib.c2v_sparse_adam_step_merged(
+            _ptr(param), _ptr(exp_avg), _ptr(exp_avg_sq), _ptr(values) if u_max else None, _ptr(rows) if u_max else None,
+            _ptr(counts), world, u_max, _ptr(union_rows) if union_rows.numel() else None, _ptr(union_count), n, E,
+            float(scale), float(lr), float(beta1), float(beta2), float(eps), int(step), _stream(dev))
+        _lib.check(rc, "c2v_sparse_adam_step_merged")

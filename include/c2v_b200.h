@@ -553,6 +553,33 @@ int c2v_sparse_adam_step(float *param, float *exp_avg, float *exp_avg_sq, const 
                          int64_t U, int64_t n_rows, int32_t E, double lr, double beta1, double beta2, double eps,
                          int64_t step, void *stream);
 
+/* ---- sparse gradients in data-parallel training ---------------------------------------------------------------------
+ * After the ranks all-gathered their coalesced gradients, each holds W padded lists in device memory:
+ *   rows   int64 [world, u_max]     list r ascending and distinct, valid up to counts[r] (the padding is never read)
+ *   values fp32  [world, u_max, E]  row j of list r is the gradient of row rows[r, j] on rank r
+ *   counts int64 [world]            a negative count is an empty list
+ * 1 <= world <= 1024, 0 <= u_max <= vocab (n_rows).
+ *
+ * c2v_sparse_union_rows: the union of the W lists, ascending, into union_rows [min(vocab, world * u_max)] and its size U
+ * into *union_count (device).  Rows outside [0, vocab) are left out.  The count / scan / compact passes of
+ * c2v_sparse_rows behind a mark pass over the lists: O(vocab + world * u_max), no sort, no host read. */
+size_t c2v_sparse_union_rows_workspace_bytes(int64_t vocab);
+int c2v_sparse_union_rows(const int64_t *rows, const int64_t *counts, int32_t world, int64_t u_max, int64_t vocab,
+                          int64_t *union_rows, int64_t *union_count, void *workspace, size_t workspace_bytes,
+                          void *stream);
+
+/* c2v_sparse_adam_step_merged: c2v_sparse_adam_step on the merged gradient of the union rows, without writing it.  For
+ * each of the U union rows (U read from *union_count on the device) the gradient is
+ *   (g_0 + g_1 + ... + g_{W-1}) * scale
+ * over the ranks whose list holds the row, added in fp32 in rank order; scale is the fp32 1/world of the mean, negated
+ * for maximize.  The update's operations and rounding are c2v_sparse_adam_step's.  No atomics: the result does not
+ * depend on scheduling, so every rank computes the same bits. */
+int c2v_sparse_adam_step_merged(float *param, float *exp_avg, float *exp_avg_sq, const float *values,
+                                const int64_t *rows, const int64_t *counts, int32_t world, int64_t u_max,
+                                const int64_t *union_rows, const int64_t *union_count, int64_t n_rows, int32_t E,
+                                float scale, double lr, double beta1, double beta2, double eps, int64_t step,
+                                void *stream);
+
 /* ---- host-buffer call: what a reference-side caller with CPU tensors uses ----------
  * One whole Code2Vec.forward + torch.max for a batch held in HOST memory (pinned
  * for full speed): copies the int64 indices in, runs encode + label head +
