@@ -182,7 +182,9 @@ backward_rows_kernel(const EncodeArgs a, const BackwardArgs b, const int Hs, con
             dal = warp_sum(dal); gvv = warp_sum(gvv);
             float extra = 0.0f, sbag = 0.0f;
             if (b.d_att) { extra = b.d_att[row]; sbag = b.sb[bag]; }
-            const float dz = alpha * (dal + extra - gvv - sbag);
+            // att = 1 (a one-context bag): the softmax derivative is exactly 0, while dal (recomputed h) - gvv (the
+            // forward's cv) would leave a rounding residue
+            const float dz = alpha == 1.0f ? 0.0f : alpha * (dal + extra - gvv - sbag);
             const float du = sidx[r] > 0 ? dz : 0.0f;            // mask = starts > 0 (model.py:64)
             float dxh[MAXC];
             float m1 = 0.0f, m2 = 0.0f;
@@ -427,7 +429,9 @@ backward_rows_lite_kernel(const EncodeArgs a, const BackwardArgs b)
         dal = warp_sum(dal); gvv = warp_sum(gvv);
         float extra = 0.0f, sbag = 0.0f;
         if (b.d_att) { extra = b.d_att[row]; sbag = b.sb[bag]; }
-        const float dz = alpha * (dal + extra - gvv - sbag);
+        // att = 1 (a one-context bag): the softmax derivative is exactly 0, while dal (recomputed h) - gvv (the
+        // forward's cv) would leave a rounding residue
+        const float dz = alpha == 1.0f ? 0.0f : alpha * (dal + extra - gvv - sbag);
         const float du = start_idx > 0 ? dz : 0.0f;              // mask = starts > 0 (model.py:64)
         float dxh[MAXC];
         float m1 = 0.0f, m2 = 0.0f;
