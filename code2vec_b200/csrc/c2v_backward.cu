@@ -28,7 +28,7 @@ namespace c2v {
 int launch_transpose_w(const float *W, float *Wt, int H, int D, int Hs, cudaStream_t st);
 bool backward_dw_tc_ok(const EncodeArgs &a);
 bool backward_dc_tc_ok(const EncodeArgs &a);
-size_t backward_dc_tc_workspace_bytes();
+size_t backward_dc_tc_workspace_bytes(int H, int Et, int Ep);
 // dc_rows / dw_slabs (deterministic mode, else NULL): dC rows stored to dc_rows [N, D] instead of scattered; dW from per-CTA
 // slabs added in CTA order
 int launch_backward_dc_tc(const EncodeArgs &a, const float *W, const float *dx, const unsigned *dx_absmax, void *ws,
@@ -50,7 +50,8 @@ struct BackwardArgs {
     float *dc_rows, *ln_part;
 };
 
-constexpr int MAXC = 8;   // columns per lane: encode_size <= 256
+constexpr int MAXC = 8;         // columns per lane: encode_size <= 256
+constexpr int MAXC_WIDE = 16;   // 256 < encode_size <= 512 (the encode backward's limit)
 // lane owns 4 consecutive columns per 128-column group (k = 0..3, 4..7): one Philox4x32 block gives the dropout masks of
 // all four (it is keyed by column / 4), and rows of X are read as one 16-byte piece per lane and group
 __device__ __forceinline__ int bk_col(int lane, int k) { return (k >> 2) * 128 + lane * 4 + (k & 3); }
@@ -103,7 +104,8 @@ __device__ __forceinline__ void load_wrow_chunk(const float *__restrict__ W, int
 
 // SPARSE: compact embedding gradients as in backward_dc_tc_kernel (slot maps in sl, a parameter behind the others)
 // DET: deterministic mode (b.dc_rows / b.ln_part instead of atomics)
-template <bool VEC, bool PACKED = false, bool SPARSE = false, bool SEED_DEV = false, bool DET = false>
+// NC: columns per lane, MAXC (encode_size <= 256) or MAXC_WIDE (<= 512)
+template <bool VEC, bool PACKED = false, bool SPARSE = false, bool SEED_DEV = false, bool DET = false, int NC = MAXC>
 __global__ void __launch_bounds__(THREADS)
 backward_rows_kernel(const EncodeArgs a, const BackwardArgs b, const int Hs, const c2v_row_slots sl)
 {
@@ -123,10 +125,10 @@ backward_rows_kernel(const EncodeArgs a, const BackwardArgs b, const int Hs, con
     const int H = a.H, D = a.D, L = a.L, Et = a.Et, Ep = a.Ep;
     const float invH = 1.0f / (float)H;
 
-    float acc_a[MAXC], acc_g[MAXC], acc_b[MAXC];              // per-lane partial da / dgamma / dbeta
+    float acc_a[NC], acc_g[NC], acc_b[NC];              // per-lane partial da / dgamma / dbeta
     float dx_max = 0.0f;
 #pragma unroll
-    for (int k = 0; k < MAXC; ++k) acc_a[k] = acc_g[k] = acc_b[k] = 0.0f;
+    for (int k = 0; k < NC; ++k) acc_a[k] = acc_g[k] = acc_b[k] = 0.0f;
 
     for (int tile = blockIdx.x; tile < a.n_tiles; tile += gridDim.x) {
         const long long row0 = (long long)tile * TM;
@@ -160,11 +162,11 @@ backward_rows_kernel(const EncodeArgs a, const BackwardArgs b, const int Hs, con
             float v = 0.0f;
             for (int c = lane; c < H; c += 32) { const float d = xr[c] - mean; v = fmaf(d, d, v); }
             const float rstd = 1.0f / sqrtf(warp_sum(v) * invH + C2V_LN_EPS);
-            float xh[MAXC], tt[MAXC], dm[MAXC];
+            float xh[NC], tt[NC], dm[NC];
             float dal = 0.0f, gvv = 0.0f;
             uint4 dbits = make_uint4(0u, 0u, 0u, 0u);
 #pragma unroll
-            for (int k = 0; k < MAXC; ++k) {
+            for (int k = 0; k < NC; ++k) {
                 const int c = bk_col(lane, k);
                 xh[k] = tt[k] = 0.0f; dm[k] = 1.0f;
                 if (c < H) {
@@ -186,10 +188,10 @@ backward_rows_kernel(const EncodeArgs a, const BackwardArgs b, const int Hs, con
             // forward's cv) would leave a rounding residue
             const float dz = alpha == 1.0f ? 0.0f : alpha * (dal + extra - gvv - sbag);
             const float du = sidx[r] > 0 ? dz : 0.0f;            // mask = starts > 0 (model.py:64)
-            float dxh[MAXC];
+            float dxh[NC];
             float m1 = 0.0f, m2 = 0.0f;
 #pragma unroll
-            for (int k = 0; k < MAXC; ++k) {
+            for (int k = 0; k < NC; ++k) {
                 const int c = bk_col(lane, k);
                 dxh[k] = 0.0f;
                 if (c < H) {
@@ -206,7 +208,7 @@ backward_rows_kernel(const EncodeArgs a, const BackwardArgs b, const int Hs, con
             }
             m1 = warp_sum(m1) * invH; m2 = warp_sum(m2) * invH;
 #pragma unroll
-            for (int k = 0; k < MAXC; ++k) {
+            for (int k = 0; k < NC; ++k) {
                 const int c = bk_col(lane, k);
                 if (c < H) {
                     const float dxv = rstd * (dxh[k] - m1 - xh[k] * m2);
@@ -315,7 +317,7 @@ backward_rows_kernel(const EncodeArgs a, const BackwardArgs b, const int Hs, con
     // ---- da / dgamma / dbeta: 8 warps -> smem -> one atomic per column per CTA
     __syncthreads();
 #pragma unroll
-    for (int k = 0; k < MAXC; ++k) {
+    for (int k = 0; k < NC; ++k) {
         const int c = bk_col(lane, k);
         if (c < H) {
             red[(0 * 8 + warp) * H + c] = acc_a[k];
@@ -339,14 +341,16 @@ backward_rows_kernel(const EncodeArgs a, const BackwardArgs b, const int Hs, con
 // cores (K3b, K3c), i.e. no GEMM in this kernel at all.  One warp per context row, rows strided over all warps; lane l
 // owns columns 4l..4l+3 of every 128-column group, so x, d_cv, cv and dx move as 16-byte pieces, gamma / beta / attn sit
 // in registers for the whole launch, one Philox block serves four columns, and padded contexts (attention weight
-// exactly 0) cost one zero store.  encode_size % 4 == 0, <= 256.
+// exactly 0) cost one zero store.  encode_size % 4 == 0, <= 512.
 // ------------------------------------------------------------------------------------
-template <int NG, bool PACKED = false, bool SEED_DEV = false, bool DET = false> // 128-column groups: 1 (encode_size <= 128) or 2
-__global__ void __launch_bounds__(256, NG == 1 ? 4 : 2)
+template <int NG, bool PACKED = false, bool SEED_DEV = false, bool DET = false> // 128-column groups: ceil(encode_size / 128)
+__global__ void __launch_bounds__(256, NG == 1 ? 4 : NG == 2 ? 2 : 1)
 backward_rows_lite_kernel(const EncodeArgs a, const BackwardArgs b)
 {
     constexpr int MAXC = 4 * NG;
-    __shared__ float red[3 * 8 * 32 * MAXC];
+    // NG <= 2 reduces d attention / d gamma / d beta at once; NG 3 / 4 one gradient after the other, which keeps red at
+    // 16 KB (three at once would be 48 KB at NG = 4, past the static shared-memory limit)
+    __shared__ float red[(NG <= 2 ? 3 : 1) * 8 * 32 * MAXC];
     // warp index through a lane-0 broadcast, so that the compiler sees the row loop and its branches as warp-uniform
     // (otherwise every shuffle of the six warp sums per row is wrapped in WARPSYNC.COLLECTIVE / ENDCOLLECTIVE)
     const int tid = threadIdx.x, lane = tid & 31, warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
@@ -471,22 +475,43 @@ backward_rows_lite_kernel(const EncodeArgs a, const BackwardArgs b)
     dx_max = warp_max(dx_max);
     if (lane == 0 && dx_max > 0.0f) atomicMax(b.dx_absmax, __float_as_uint(dx_max));
     // da / dgamma / dbeta: 8 warps -> smem -> one atomic per column per CTA
+    if constexpr (NG <= 2) {
 #pragma unroll
-    for (int k = 0; k < MAXC; ++k) {
-        red[((0 * 8 + warp) * MAXC + k) * 32 + lane] = acc_a[k];
-        red[((1 * 8 + warp) * MAXC + k) * 32 + lane] = acc_g[k];
-        red[((2 * 8 + warp) * MAXC + k) * 32 + lane] = acc_b[k];
-    }
-    __syncthreads();
-    for (int i = tid; i < 3 * MAXC * 32; i += 256) {
-        const int which = i / (MAXC * 32), k = (i / 32) % MAXC, l = i % 32;
-        const int c = bk_col(l, k);
-        if (c >= H) continue;
-        float sum = 0.0f;
-        for (int w = 0; w < 8; ++w) sum += red[((which * 8 + w) * MAXC + k) * 32 + l];
-        if (DET) { b.ln_part[((size_t)blockIdx.x * 3 + which) * H + c] = sum; continue; }
-        float *dst = which == 0 ? b.g_attn : which == 1 ? b.g_ln_g : b.g_ln_b;
-        if (sum != 0.0f) atomicAdd(dst + c, sum);
+        for (int k = 0; k < MAXC; ++k) {
+            red[((0 * 8 + warp) * MAXC + k) * 32 + lane] = acc_a[k];
+            red[((1 * 8 + warp) * MAXC + k) * 32 + lane] = acc_g[k];
+            red[((2 * 8 + warp) * MAXC + k) * 32 + lane] = acc_b[k];
+        }
+        __syncthreads();
+        for (int i = tid; i < 3 * MAXC * 32; i += 256) {
+            const int which = i / (MAXC * 32), k = (i / 32) % MAXC, l = i % 32;
+            const int c = bk_col(l, k);
+            if (c >= H) continue;
+            float sum = 0.0f;
+            for (int w = 0; w < 8; ++w) sum += red[((which * 8 + w) * MAXC + k) * 32 + l];
+            if (DET) { b.ln_part[((size_t)blockIdx.x * 3 + which) * H + c] = sum; continue; }
+            float *dst = which == 0 ? b.g_attn : which == 1 ? b.g_ln_g : b.g_ln_b;
+            if (sum != 0.0f) atomicAdd(dst + c, sum);
+        }
+    } else {
+#pragma unroll
+        for (int which = 0; which < 3; ++which) {
+            if (which > 0) __syncthreads();                 // the previous gradient's sums have read red
+#pragma unroll
+            for (int k = 0; k < MAXC; ++k)
+                red[(warp * MAXC + k) * 32 + lane] = which == 0 ? acc_a[k] : which == 1 ? acc_g[k] : acc_b[k];
+            __syncthreads();
+            float *dst = which == 0 ? b.g_attn : which == 1 ? b.g_ln_g : b.g_ln_b;
+            for (int i = tid; i < MAXC * 32; i += 256) {
+                const int k = i / 32, l = i % 32;
+                const int c = bk_col(l, k);
+                if (c >= H) continue;
+                float sum = 0.0f;
+                for (int w = 0; w < 8; ++w) sum += red[(w * MAXC + k) * 32 + l];
+                if (DET) b.ln_part[((size_t)blockIdx.x * 3 + which) * H + c] = sum;
+                else if (sum != 0.0f) atomicAdd(dst + c, sum);
+            }
+        }
     }
 }
 
@@ -566,7 +591,8 @@ static size_t backward_base_bytes(const c2v_dims *d, int B, long long N, bool pa
     const size_t H = d->encode, D = 2 * (size_t)d->terminal_embed + d->path_embed;
     const size_t Hs = (H + 3) / 4 * 4;
     return align_up((size_t)N * H * 4, 1024) + align_up((size_t)B * 4, 1024) + align_up(D * Hs * 4, 1024) + 1024 +   // 1 KB: dx absmax word
-           align_up(backward_dc_tc_workspace_bytes(), 1024) + (packed ? align_up((size_t)N * 4, 1024) : 0);
+           align_up(backward_dc_tc_workspace_bytes(d->encode, d->terminal_embed, d->path_embed), 1024) +
+           (packed ? align_up((size_t)N * 4, 1024) : 0);
 }
 
 // deterministic mode, behind the base layout: dC rows [N, D] | dW slabs [kDetSlabs][H][D] | d attention / gamma / beta
@@ -622,6 +648,36 @@ static int det_ln_grads(const float *ln_part, int n_slabs, int H, const c2v_grad
     return launch_det_slab_sum3(ln_part, n_slabs, (size_t)3 * H, (size_t)H, 3, out, false, st);
 }
 
+// the instantiation of backward_rows_kernel with NC columns per lane for the launch's modes
+template <int NC>
+static auto rows_kernel(bool det, bool dev_key, bool sparse, bool packed, bool vec)
+{
+    return det
+        ? (dev_key ? (packed ? (vec ? backward_rows_kernel<true, true, false, true, true, NC> : backward_rows_kernel<false, true, false, true, true, NC>)
+                             : (vec ? backward_rows_kernel<true, false, false, true, true, NC> : backward_rows_kernel<false, false, false, true, true, NC>))
+                   : (packed ? (vec ? backward_rows_kernel<true, true, false, false, true, NC> : backward_rows_kernel<false, true, false, false, true, NC>)
+                             : (vec ? backward_rows_kernel<true, false, false, false, true, NC> : backward_rows_kernel<false, false, false, false, true, NC>)))
+        : dev_key
+        ? (sparse ? (packed ? (vec ? backward_rows_kernel<true, true, true, true, false, NC> : backward_rows_kernel<false, true, true, true, false, NC>)
+                            : (vec ? backward_rows_kernel<true, false, true, true, false, NC> : backward_rows_kernel<false, false, true, true, false, NC>))
+                  : (packed ? (vec ? backward_rows_kernel<true, true, false, true, false, NC> : backward_rows_kernel<false, true, false, true, false, NC>)
+                            : (vec ? backward_rows_kernel<true, false, false, true, false, NC> : backward_rows_kernel<false, false, false, true, false, NC>)))
+        : (sparse ? (packed ? (vec ? backward_rows_kernel<true, true, true, false, false, NC> : backward_rows_kernel<false, true, true, false, false, NC>)
+                            : (vec ? backward_rows_kernel<true, false, true, false, false, NC> : backward_rows_kernel<false, false, true, false, false, NC>))
+                  : (packed ? (vec ? backward_rows_kernel<true, true, false, false, false, NC> : backward_rows_kernel<false, true, false, false, false, NC>)
+                            : (vec ? backward_rows_kernel<true, false, false, false, false, NC> : backward_rows_kernel<false, false, false, false, false, NC>)));
+}
+
+// the instantiation of backward_rows_lite_kernel with NG 128-column groups for the launch's modes
+template <int NG>
+static auto rows_lite_kernel(bool det, bool dev_key, bool packed)
+{
+    return det ? (dev_key ? (packed ? backward_rows_lite_kernel<NG, true, true, true> : backward_rows_lite_kernel<NG, false, true, true>)
+                          : (packed ? backward_rows_lite_kernel<NG, true, false, true> : backward_rows_lite_kernel<NG, false, false, true>))
+               : (dev_key ? (packed ? backward_rows_lite_kernel<NG, true, true> : backward_rows_lite_kernel<NG, false, true>)
+                          : (packed ? backward_rows_lite_kernel<NG, true> : backward_rows_lite_kernel<NG>));
+}
+
 int launch_encode_backward(const c2v_dims *d, const c2v_params *p, const EncodeArgs &a_in, int B,
                            const float *cv, const float *attention, const float *d_cv, const float *d_att,
                            const c2v_grads *g, void *ws, size_t ws_bytes, cudaStream_t st, const float *x_stash, int phase,
@@ -635,8 +691,8 @@ int launch_encode_backward(const c2v_dims *d, const c2v_params *p, const EncodeA
     // Deterministic mode (c2v_set_deterministic) keeps the same kernels and phases; the dC kernels store rows that
     // launch_det_embed_grads then sums per table row, and dW / d attention / d gamma / d beta come from per-CTA slabs.
     EncodeArgs a = a_in;
-    if (a.H > 32 * MAXC) {
-        set_error("encode backward supports encode_size <= %d (got %d)", 32 * MAXC, a.H);
+    if (a.H > 32 * MAXC_WIDE) {
+        set_error("encode backward supports encode_size <= %d (got %d)", 32 * MAXC_WIDE, a.H);
         return C2V_EUNSUPPORTED;
     }
     const bool packed = a.bag_off != nullptr;
@@ -653,7 +709,7 @@ int launch_encode_backward(const c2v_dims *d, const c2v_params *p, const EncodeA
     float *sb = reinterpret_cast<float *>(base + o); o += align_up((size_t)B * 4, 1024);
     float *w_t = reinterpret_cast<float *>(base + o); o += align_up((size_t)a.D * Hs * 4, 1024);
     unsigned *dx_absmax = reinterpret_cast<unsigned *>(base + o); o += 1024;
-    void *dc_ws = base + o; o += align_up(backward_dc_tc_workspace_bytes(), 1024);
+    void *dc_ws = base + o; o += align_up(backward_dc_tc_workspace_bytes(a.H, a.Et, a.Ep), 1024);
     int *row_bag = packed ? reinterpret_cast<int *>(base + o) : nullptr;
     const DetBackwardLayout dl = det_backward_layout(d, a.N, backward_base_bytes(d, B, a.N, packed));
     float *dc_rows = det ? reinterpret_cast<float *>(base + dl.dc) : nullptr;
@@ -726,20 +782,10 @@ int launch_encode_backward(const c2v_dims *d, const c2v_params *p, const EncodeA
     if (x_stash && dc_tc && (a.H & 3) == 0) {                  // no GEMM left in this kernel: one warp per row
         int grid = a.H <= 128 ? sms * 16 : sms * 8;
         if (det && grid > kDetRowSlabs) grid = kDetRowSlabs;
-        if (det) {
-            if (a.H <= 128)
-                (dev_key ? (packed ? backward_rows_lite_kernel<1, true, true, true> : backward_rows_lite_kernel<1, false, true, true>)
-                         : (packed ? backward_rows_lite_kernel<1, true, false, true> : backward_rows_lite_kernel<1, false, false, true>))
-                    <<<grid, 256, 0, st>>>(a, b);
-            else
-                (dev_key ? (packed ? backward_rows_lite_kernel<2, true, true, true> : backward_rows_lite_kernel<2, false, true, true>)
-                         : (packed ? backward_rows_lite_kernel<2, true, false, true> : backward_rows_lite_kernel<2, false, false, true>))
-                    <<<grid, 256, 0, st>>>(a, b);
-        } else if (dev_key) {
-            if (a.H <= 128) (packed ? backward_rows_lite_kernel<1, true, true> : backward_rows_lite_kernel<1, false, true>)<<<grid, 256, 0, st>>>(a, b);
-            else (packed ? backward_rows_lite_kernel<2, true, true> : backward_rows_lite_kernel<2, false, true>)<<<grid, 256, 0, st>>>(a, b);
-        } else if (a.H <= 128) (packed ? backward_rows_lite_kernel<1, true> : backward_rows_lite_kernel<1>)<<<grid, 256, 0, st>>>(a, b);
-        else (packed ? backward_rows_lite_kernel<2, true> : backward_rows_lite_kernel<2>)<<<grid, 256, 0, st>>>(a, b);
+        const int ng = (a.H + 127) / 128;
+        auto lite = ng == 1 ? rows_lite_kernel<1>(det, dev_key, packed) : ng == 2 ? rows_lite_kernel<2>(det, dev_key, packed)
+                  : ng == 3 ? rows_lite_kernel<3>(det, dev_key, packed) : rows_lite_kernel<4>(det, dev_key, packed);
+        lite<<<grid, 256, 0, st>>>(a, b);
         C2V_LAUNCH_OK("backward_rows_lite_kernel");
         if (det && (rc = det_ln_grads(ln_part, grid, a.H, g, st)) != C2V_OK) return rc;
         if (phase == 1) {                                       // path sub-vector + dW; start / end follow in phase 2
@@ -762,20 +808,8 @@ int launch_encode_backward(const c2v_dims *d, const c2v_params *p, const EncodeA
     {
     // (with dc_tc K3c scatters; in deterministic mode nothing is scattered here)
     const bool sparse = !dc_tc && !det && slots && (slots->terminal || slots->path);
-    auto kern = det
-        ? (dev_key ? (packed ? (vec ? backward_rows_kernel<true, true, false, true, true> : backward_rows_kernel<false, true, false, true, true>)
-                             : (vec ? backward_rows_kernel<true, false, false, true, true> : backward_rows_kernel<false, false, false, true, true>))
-                   : (packed ? (vec ? backward_rows_kernel<true, true, false, false, true> : backward_rows_kernel<false, true, false, false, true>)
-                             : (vec ? backward_rows_kernel<true, false, false, false, true> : backward_rows_kernel<false, false, false, false, true>)))
-        : dev_key
-        ? (sparse ? (packed ? (vec ? backward_rows_kernel<true, true, true, true> : backward_rows_kernel<false, true, true, true>)
-                            : (vec ? backward_rows_kernel<true, false, true, true> : backward_rows_kernel<false, false, true, true>))
-                  : (packed ? (vec ? backward_rows_kernel<true, true, false, true> : backward_rows_kernel<false, true, false, true>)
-                            : (vec ? backward_rows_kernel<true, false, false, true> : backward_rows_kernel<false, false, false, true>)))
-        : (sparse ? (packed ? (vec ? backward_rows_kernel<true, true, true> : backward_rows_kernel<false, true, true>)
-                            : (vec ? backward_rows_kernel<true, false, true> : backward_rows_kernel<false, false, true>))
-                  : (packed ? (vec ? backward_rows_kernel<true, true> : backward_rows_kernel<false, true>)
-                            : (vec ? backward_rows_kernel<true> : backward_rows_kernel<false>)));
+    auto kern = a.H <= 32 * MAXC ? rows_kernel<MAXC>(det, dev_key, sparse, packed, vec)
+                                 : rows_kernel<MAXC_WIDE>(det, dev_key, sparse, packed, vec);
     c2v_row_slots sl = {nullptr, nullptr};
     if (sparse) sl = *slots;
     C2V_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));

@@ -1,5 +1,5 @@
 // c2v_backward_dc_tc.cu -- K3c: dC = dX . W on the tensor cores (wgmma) + scatter into the embedding gradients
-// (terminal_embed = path_embed = E <= 256, encode = H <= 256, multiples of 4; zero-padded to 128 inside the panels).
+// (terminal_embed = path_embed = E <= 256, encode = H <= 512, multiples of 4; zero-padded to 128 inside the panels).
 //
 // The gradient of the gathered context vectors (autograd of model.py:48-54 under loss.backward(), main.py:174):
 //   dC[r, d] = sum_h dX[r, h] * W[h, d],  then  dE_t[starts_r] += dC[r, 0:128], dE_p[paths_r] += dC[r, 128:256],
@@ -17,7 +17,7 @@
 // 16 W^T producer | 17-19 idle.  Work items run (row tile, sub-vector, h block); the dX panels of a row tile are
 // re-staged for every sub-vector (L2 hits after the first).
 // Sizes above 128: blockIdx.y = db selects the 128-wide window of d inside every sub-vector (its own grid of CTAs over the
-// row tiles); the contraction over h runs as n_hb blocks of 128 through the same operand stages, accumulating in
+// row tiles); the contraction over h runs as n_hb <= 4 blocks of 128 through the same operand stages, accumulating in
 // registers, and the accumulator is scattered after the last block -- so every dC element is still added to the
 // embedding gradient exactly once.
 #include <cuda_fp16.h>
@@ -295,10 +295,20 @@ backward_dc_tc_kernel(const EncodeArgs a, const float *__restrict__ dx, const un
 }
 
 bool backward_dc_tc_ok(const EncodeArgs &a) {
-    return a.Et == a.Ep && a.Et <= 2 * dct::E && a.H <= 2 * dct::H && (a.Et & 3) == 0 && (a.H & 3) == 0 &&
+    return a.Et == a.Ep && a.Et <= 2 * dct::E && a.H <= 4 * dct::H && (a.Et & 3) == 0 && (a.H & 3) == 0 &&
            (long long)a.T * (a.Et / 4) < 0xFFFFFFFFll && (long long)a.P * (a.Et / 4) < 0xFFFFFFFFll;
 }
-size_t backward_dc_tc_workspace_bytes() { return 1024 + 4 * dct::IMG_BYTES; }      // up to 2 x 2 window pairs
+// room for n_db x n_hb W^T images: every shape reserves 2 x 2 (the most an encode size <= 256 needs), and a shape that
+// runs here above 256 up to 2 x 4
+size_t backward_dc_tc_workspace_bytes(int H, int Et, int Ep)
+{
+    int n = 4;
+    if (Et == Ep && Et <= 2 * dct::E) {
+        const int n_img = ((H + dct::H - 1) / dct::H) * ((Et + dct::E - 1) / dct::E);
+        if (n_img > n) n = n_img;
+    }
+    return 1024 + (size_t)n * dct::IMG_BYTES;
+}
 
 // ws: [0, 1024) header {1/scale, scale} | W^T images [db][hb]
 int launch_backward_dc_tc(const EncodeArgs &a_in, const float *W, const float *dx, const unsigned *dx_absmax, void *ws,

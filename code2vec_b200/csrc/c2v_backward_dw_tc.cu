@@ -1,5 +1,5 @@
 // c2v_backward_dw_tc.cu -- K3b: dW = dX^T . C on the tensor cores (wgmma; terminal_embed = path_embed = E <= 256,
-// encode = H <= 256, both multiples of 4: the reference's default 100/100/100 runs here with the panels zero-padded to 128;
+// encode = H <= 512, both multiples of 4: the reference's default 100/100/100 runs here with the panels zero-padded to 128;
 // sizes above 128 run as 128-wide windows of h and of d -- see "windows" below).
 //
 // The weight gradient of input_linear (what autograd computes for model.py:54 under loss.backward(), main.py:174):
@@ -17,7 +17,7 @@
 // split -> STS.64; a producer keeps two panels of loads in flight).
 // smem: 2 tile-stages of the dX operand {hi p0, hi p1, lo p0, lo p1} (128 KB) + 2 slots of one gathered panel {hi, lo}
 // (64 KB); per tile the two gathered panels of the window's sub-vector stream through the slots.
-// Windows: blockIdx.y = (hb * n_db + db) * 3 + sv selects rows h in [128 hb, 128 hb + 128) of dW and columns
+// Windows: blockIdx.y = (hb * n_db + db) * 3 + sv (n_hb <= 4, n_db <= 2) selects rows h in [128 hb, 128 hb + 128) of dW and columns
 // d in [128 db, 128 db + 128) of sub-vector sv (start / path / end); the CTAs of one window (gridDim.x of them) share the
 // row tiles.  dX is therefore read once per window.
 #include <cuda_fp16.h>
@@ -232,7 +232,7 @@ backward_dw_tc_kernel(const EncodeArgs a, const float *__restrict__ dx, const un
 }
 
 bool backward_dw_tc_ok(const EncodeArgs &a) {
-    return a.Et == a.Ep && a.Et <= 2 * dwt::E && a.H <= 2 * dwt::H && (a.Et & 3) == 0 && (a.H & 3) == 0 &&
+    return a.Et == a.Ep && a.Et <= 2 * dwt::E && a.H <= 4 * dwt::H && (a.Et & 3) == 0 && (a.H & 3) == 0 &&
            (long long)a.T * a.Et * 4 < (1ll << 32) && (long long)a.P * a.Et * 4 < (1ll << 32);
 }
 

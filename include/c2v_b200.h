@@ -473,7 +473,10 @@ int c2v_label_backward_ws(const c2v_dims *d, const c2v_params *p, const float *c
 /* Encode: gradients of every encode parameter given d_code_vector [B,H] and
  * (optionally, may be NULL) d_attention [B,L]; formulas in "Backward".
  * Recomputes the forward per context row (nothing but code_vector / attention is
- * stashed) and regenerates the dropout mask from `drop`. */
+ * stashed) and regenerates the dropout mask from `drop`.
+ * Envelope of every encode-backward entry point (padded, packed, sparse, phased): encode_size <= 512.  Above that they
+ * return C2V_EUNSUPPORTED.  dW and dC run on the tensor cores when terminal_embed == path_embed <= 256 and both it and
+ * encode_size are multiples of 4, else on the CUDA cores; the per-row work always runs on the CUDA cores. */
 size_t c2v_encode_backward_workspace_bytes(const c2v_dims *d, int32_t B, int32_t L);
 int c2v_encode_backward(const c2v_dims *d, const c2v_params *p,
                         const int64_t *starts, const int64_t *paths, const int64_t *ends,
