@@ -59,6 +59,15 @@ class LossOptions(ctypes.Structure):
                 ("row_grad", c_vp)]
 
 
+ADAM_MAX_GROUPS, ADAM_MAX_SEGMENTS = 16, 64   # C2V_ADAM_MAX_GROUPS / C2V_ADAM_MAX_SEGMENTS of c2v_adam_step_groups
+
+
+class AdamGroup(ctypes.Structure):
+    """c2v_adam_group: one parameter group's hyper-parameters (include/c2v_b200.h)"""
+    _fields_ = [("lr", c_f32), ("beta1", c_f32), ("beta2", c_f32), ("eps", c_f32), ("weight_decay", c_f32),
+                ("decoupled", c_i32), ("lr_dev", c_vp)]
+
+
 class DeviceInfo(ctypes.Structure):
     _fields_ = [("cc_major", c_i32), ("cc_minor", c_i32), ("sm_count", c_i32), ("reserved", c_i32),
                 ("global_mem_bytes", c_i64), ("smem_per_block_optin", c_i64)]
@@ -149,6 +158,14 @@ SYMBOLS = {
                                              c_f32, c_f32, c_f32, c_f32, c_f32, c_i64, c_f32, c_vp]),
     "c2v_adam_step_sharded_bulk": (ctypes.c_int, [c_vp, _P(c_vp), _P(c_vp), c_i32, c_vp, c_vp, c_i64, c_i64, c_f32, c_f32, c_f32,
                                                   c_f32, c_f32, c_i64, c_f32, c_i32, c_vp]),
+    "c2v_adam_step_groups": (ctypes.c_int, [c_vp, c_vp, c_vp, c_vp, c_i64, _P(AdamGroup), c_i32, _P(c_i64), _P(c_i32), c_i32,
+                                            c_i64, c_vp, c_f32, c_i32, c_vp, c_vp]),
+    "c2v_adam_step_sharded_groups": (ctypes.c_int, [c_vp, c_vp, c_vp, _P(c_vp), _P(c_vp), c_i32, c_vp, c_vp, c_i64, c_i64, c_vp,
+                                                    c_i64, _P(AdamGroup), c_i32, _P(c_i64), _P(c_i32), c_i32, c_i64, c_f32,
+                                                    c_vp]),
+    "c2v_adam_step_sharded_bulk_groups": (ctypes.c_int, [c_vp, _P(c_vp), _P(c_vp), c_i32, c_vp, c_vp, c_i64, c_i64,
+                                                         _P(AdamGroup), c_i32, _P(c_i64), _P(c_i32), c_i32, c_i64, c_f32,
+                                                         c_i32, c_vp]),
     "c2v_loss_argmax": (ctypes.c_int, [c_vp, c_vp, c_i32, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "c2v_loss_argmax_opts": (ctypes.c_int, [c_vp, c_vp, c_i32, c_i64, _P(LossOptions), c_vp, c_vp, c_vp, c_vp, c_vp]),
     "c2v_label_backward": (ctypes.c_int, [_P(Dims), _P(Params), c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp]),

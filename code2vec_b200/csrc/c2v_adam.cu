@@ -9,6 +9,7 @@
 //   g += wd * p;  m += (g - m) * (1 - b1);  v = v * b2 + (1 - b2) * g * g;
 //   p -= (lr / (1 - b1^t)) * m / (sqrt(v) / sqrt(1 - b2^t) + eps)
 #include <cstring>
+#include <type_traits>
 
 #include "c2v_common.cuh"
 
@@ -26,20 +27,133 @@ __device__ __forceinline__ float adam_grad(float g, float gscale, float wd, floa
     return fmaf(wd, p, gs) + fmaf(g, gscale, -gs);
 }
 
+// ------------------------------------------------------------------------------------------------------------------
+// Parameter groups (torch.optim.Adam's param_groups, AdamW's decoupled decay among the per-group settings): the update
+// kernels below take a trailing `Groups` argument.  NoGroups (empty) is the one-group step with the hyper-parameters as
+// launch parameters.  AdamGroups is a by-value table: per group its hyper-parameters, per segment (a maximal run of one
+// group in flat order) its first element in FLAT-BUFFER coordinates and its group.  Segment s covers
+// [begin[s], begin[s + 1]), the last one everything behind its begin; begin[0] = 0.  Each thread visits its elements in
+// ascending order, so it finds an element's segment by walking forward from the previous one (at most n_segments steps
+// over the whole launch); a float4 that crosses a boundary is updated element by element.
+// ------------------------------------------------------------------------------------------------------------------
+constexpr int ADAM_MAX_GROUPS = 16, ADAM_MAX_SEGMENTS = 64;
+
+// decay = 1 - lr * wd with wd = 0 for a decoupled (AdamW) group, decay = 1 (exact: p * 1 == p) with wd for a coupled one
+struct AdamHyper { float step_size, one_minus_b1, b2, one_minus_b2, inv_sqrt_bc2, eps, wd, decay; };
+
+struct AdamGroups {
+    AdamHyper hyper[ADAM_MAX_GROUPS];
+    long long seg_begin[ADAM_MAX_SEGMENTS];
+    int seg_group[ADAM_MAX_SEGMENTS];
+    int n_groups, n_segments;
+};
+
+struct NoGroups {};
+
+// the table in shared memory, with a sentinel segment begin behind the last segment
+struct AdamGroupsSmem {
+    AdamHyper hyper[ADAM_MAX_GROUPS];
+    long long begin[ADAM_MAX_SEGMENTS + 1];
+    int group[ADAM_MAX_SEGMENTS];
+};
+
+// every thread of the CTA calls it (it ends in __syncthreads).  dev_scalars != NULL (the capturable step): step_size,
+// inv_sqrt_bc2 and decay of group k are dev_scalars[3k .. 3k + 2], where adam_step_count_groups_kernel left them.
+__device__ __forceinline__ void load_groups(AdamGroupsSmem &s, const AdamGroups &t, const float *dev_scalars)
+{
+    for (int i = threadIdx.x; i < t.n_groups; i += blockDim.x) {
+        AdamHyper h = t.hyper[i];
+        if (dev_scalars) { h.step_size = dev_scalars[3 * i]; h.inv_sqrt_bc2 = dev_scalars[3 * i + 1]; h.decay = dev_scalars[3 * i + 2]; }
+        s.hyper[i] = h;
+    }
+    for (int i = threadIdx.x; i <= ADAM_MAX_SEGMENTS; i += blockDim.x) {
+        s.begin[i] = i < t.n_segments ? t.seg_begin[i] : 0x7fffffffffffffffLL;
+        if (i < ADAM_MAX_SEGMENTS) s.group[i] = t.seg_group[i];
+    }
+    __syncthreads();
+}
+
+// the table's shared memory, allocated only in the kernels that use it
+__device__ __forceinline__ AdamGroupsSmem &groups_smem()
+{
+    __shared__ AdamGroupsSmem tab;
+    return tab;
+}
+
+// the segment of flat element e >= begin[seg], walking forward from seg
+__device__ __forceinline__ int segment_of(const AdamGroupsSmem &s, int seg, long long e)
+{
+    while (s.begin[seg + 1] <= e) ++seg;
+    return seg;
+}
+
+// torch's single-tensor Adam / AdamW on one element with its group's hyper-parameters:
+//   p *= 1 - lr * wd (AdamW);  g += wd * p (Adam);  m, v, p as in adam_step_kernel
+__device__ __forceinline__ void adam_upd_group(const AdamHyper &h, float gscale, float &pp, float gg, float &mm, float &vv)
+{
+    pp *= h.decay;
+    const float gr = adam_grad(gg, gscale, h.wd, pp);
+    mm = mm + (gr - mm) * h.one_minus_b1;
+    vv = vv * h.b2 + h.one_minus_b2 * gr * gr;
+    const float denom = sqrtf(vv) * h.inv_sqrt_bc2 + h.eps;
+    pp = fmaf(-h.step_size, mm / denom, pp);
+}
+
+// the float4 at flat element e: one group's hyper-parameters for all four, or element by element across a boundary.
+// seg: the thread's cursor (in: the segment of an element <= e; out: the segment of e + 3)
+__device__ __forceinline__ void adam_upd4_group(const AdamGroupsSmem &s, int &seg, long long e, float gscale, float4 &P,
+                                                const float4 &G, float4 &M, float4 &V)
+{
+    seg = segment_of(s, seg, e);
+    if (s.begin[seg + 1] >= e + 4) {
+        const AdamHyper h = s.hyper[s.group[seg]];
+        adam_upd_group(h, gscale, P.x, G.x, M.x, V.x); adam_upd_group(h, gscale, P.y, G.y, M.y, V.y);
+        adam_upd_group(h, gscale, P.z, G.z, M.z, V.z); adam_upd_group(h, gscale, P.w, G.w, M.w, V.w);
+        return;
+    }
+    adam_upd_group(s.hyper[s.group[seg]], gscale, P.x, G.x, M.x, V.x);
+    seg = segment_of(s, seg, e + 1);
+    adam_upd_group(s.hyper[s.group[seg]], gscale, P.y, G.y, M.y, V.y);
+    seg = segment_of(s, seg, e + 2);
+    adam_upd_group(s.hyper[s.group[seg]], gscale, P.z, G.z, M.z, V.z);
+    seg = segment_of(s, seg, e + 3);
+    adam_upd_group(s.hyper[s.group[seg]], gscale, P.w, G.w, M.w, V.w);
+}
+
 // DEV_SCALARS (c2v_adam_step_capturable): step_size and inv_sqrt_bc2 are read from dev_scalars[0..1], where
-// adam_step_count_kernel left them, instead of the launch parameters.
+// adam_step_count_kernel left them, instead of the launch parameters (with AdamGroups: see load_groups).
 // DEV_COEF (c2v_adam_step_ex with coef_dev): the gradient is read as g * (gscale * *coef_dev), the clip coefficient that
 // grad_norm_finalize_kernel left on the device, formed once per thread: no host read between the norm and the update.
-template <bool DEV_SCALARS = false, bool DEV_COEF = false>
+// Groups = AdamGroups (c2v_adam_step_groups): the scalar hyper-parameters are unused, the table's apply.
+template <bool DEV_SCALARS = false, bool DEV_COEF = false, class Groups = NoGroups>
 __global__ void __launch_bounds__(256)
 adam_step_kernel(float4 *__restrict__ p, float4 *__restrict__ g, float4 *__restrict__ m, float4 *__restrict__ v,
                  long long n4, float *__restrict__ pt, float *__restrict__ gt, float *__restrict__ mt, float *__restrict__ vt,
                  int tail, float step_size, float one_minus_b1, float b2, float one_minus_b2, float inv_sqrt_bc2, float eps,
                  float wd, float gscale, int zero_grad, const float *__restrict__ dev_scalars,
-                 const float *__restrict__ coef_dev)
+                 const float *__restrict__ coef_dev, const Groups groups)
 {
     if (DEV_SCALARS) { step_size = dev_scalars[0]; inv_sqrt_bc2 = dev_scalars[1]; }
     if (DEV_COEF) gscale *= *coef_dev;
+    if constexpr (std::is_same<Groups, AdamGroups>::value) {
+        AdamGroupsSmem &tab = groups_smem();
+        load_groups(tab, groups, DEV_SCALARS ? dev_scalars : nullptr);
+        int seg = 0;
+        for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
+            float4 P = p[i], G = g[i], M = m[i], V = v[i];
+            adam_upd4_group(tab, seg, 4 * i, gscale, P, G, M, V);
+            p[i] = P; m[i] = M; v[i] = V;
+            if (zero_grad) g[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+        if (blockIdx.x == 0 && (int)threadIdx.x < tail) {
+            const int i = threadIdx.x;
+            float P = pt[i], M = mt[i], V = vt[i];
+            adam_upd_group(tab.hyper[tab.group[segment_of(tab, 0, 4 * n4 + i)]], gscale, P, gt[i], M, V);
+            pt[i] = P; mt[i] = M; vt[i] = V;
+            if (zero_grad) gt[i] = 0.0f;
+        }
+        return;
+    }
     auto upd = [&](float &pp, float &gg, float &mm, float &vv) {
         const float gr = adam_grad(gg, gscale, wd, pp);
         mm = mm + (gr - mm) * one_minus_b1;                 // exp_avg.lerp_(grad, 1 - beta1)
@@ -78,6 +192,40 @@ __global__ void adam_step_count_kernel(long long *state, float lr, float beta1, 
     float *f = reinterpret_cast<float *>(state + 1);
     f[0] = (float)((double)lr / bc1);
     f[1] = (float)(1.0 / sqrt(bc2));
+}
+
+// group g's hyper-parameters at step t with learning rate lr: the expressions of c2v_adam_step, on the host (host step
+// count) or in adam_step_count_groups_kernel; decay = 1 - lr * wd rounded once, as torch's param.mul_(1 - lr * wd)
+__host__ __device__ inline AdamHyper adam_hyper(const c2v_adam_group &g, float lr, long long t)
+{
+    const double bc1 = 1.0 - pow((double)g.beta1, (double)t), bc2 = 1.0 - pow((double)g.beta2, (double)t);
+    AdamHyper h;
+    h.step_size = (float)((double)lr / bc1);
+    h.one_minus_b1 = 1.0f - g.beta1;
+    h.b2 = g.beta2;
+    h.one_minus_b2 = 1.0f - g.beta2;
+    h.inv_sqrt_bc2 = (float)(1.0 / sqrt(bc2));
+    h.eps = g.eps;
+    h.wd = g.decoupled ? 0.0f : g.weight_decay;
+    h.decay = g.decoupled ? (float)(1.0 - (double)lr * (double)g.weight_decay) : 1.0f;
+    return h;
+}
+
+struct AdamGroupArgs { c2v_adam_group g[ADAM_MAX_GROUPS]; int n; };
+
+// The step count of c2v_adam_step_groups: state = {int64 step; float s[3 * n]}, s[3k .. 3k + 2] = group k's step_size,
+// inv_sqrt_bc2 and decay (load_groups reads them), each group's lr from its lr_dev when one is given.
+__global__ void adam_step_count_groups_kernel(long long *state, const AdamGroupArgs a)
+{
+    const long long t = state[0] + 1;
+    state[0] = t;
+    float *f = reinterpret_cast<float *>(state + 1);
+    for (int k = 0; k < a.n; ++k) {
+        const AdamHyper h = adam_hyper(a.g[k], a.g[k].lr_dev ? *a.g[k].lr_dev : a.g[k].lr, t);
+        f[3 * k] = h.step_size;
+        f[3 * k + 1] = h.inv_sqrt_bc2;
+        f[3 * k + 2] = h.decay;
+    }
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -160,14 +308,16 @@ __device__ __forceinline__ void mm_st(float *mc, float4 v) {
 
 // 128-thread CTAs (<= 64 registers): 8 K registers per CTA, so that the kernel can share SMs with the persistent tensor-core
 // backward kernels (22 warps x 72-80 registers leave ~9-15 K of the 64 K registers) when it runs on a side stream.
-template <bool MULTIMEM>
+// Groups = AdamGroups: c2v_adam_step_sharded_groups, the table's hyper-parameters instead of the scalar ones.
+template <bool MULTIMEM, class Groups = NoGroups>
 __global__ void __launch_bounds__(128)
 adam_step_sharded_kernel(const float *__restrict__ p_local, float *__restrict__ p_mc, const float *__restrict__ g_mc,
                          const AdamPeers peers, int world, float4 *__restrict__ m, float4 *__restrict__ v,
                          long long slice_begin, long long slice_n4, float4 *__restrict__ zero_buf, long long zero_n4,
                          float step_size, float one_minus_b1, float b2, float one_minus_b2, float inv_sqrt_bc2, float eps,
-                         float wd, float gscale)
+                         float wd, float gscale, const Groups groups)
 {
+    constexpr bool GROUPED = std::is_same<Groups, AdamGroups>::value;
     auto upd = [&](float &pp, float gg, float &mm, float &vv) {
         const float gr = adam_grad(gg, gscale, wd, pp);
         mm = mm + (gr - mm) * one_minus_b1;
@@ -186,6 +336,9 @@ adam_step_sharded_kernel(const float *__restrict__ p_local, float *__restrict__ 
         for (long long i = (long long)(blockIdx.x >> 2) * blockDim.x + threadIdx.x; i < zero_n4; i += zstride) zero_buf[i] = z;
         return;
     }
+    AdamGroupsSmem *tab = nullptr;                           // (NoGroups: no shared memory for the table)
+    int seg = 0;
+    if constexpr (GROUPED) { tab = &groups_smem(); load_groups(*tab, groups, nullptr); }
     const int wb = (int)blockIdx.x - (n_zero_cta > 0 ? (int)(blockIdx.x + 1) / 4 : 0);
     const long long stride = (long long)((int)gridDim.x - n_zero_cta) * blockDim.x, t0 = (long long)wb * blockDim.x + threadIdx.x;
     for (long long i0 = t0; i0 < slice_n4; i0 += 2 * stride) {
@@ -205,13 +358,15 @@ adam_step_sharded_kernel(const float *__restrict__ p_local, float *__restrict__ 
         }
         float4 P0 = *reinterpret_cast<const float4 *>(p_local + e0), M0 = m[i0], V0 = v[i0];
         float4 P1 = *reinterpret_cast<const float4 *>(p_local + e1), M1 = m[two ? i1 : i0], V1 = v[two ? i1 : i0];
-        upd(P0.x, G0.x, M0.x, V0.x); upd(P0.y, G0.y, M0.y, V0.y); upd(P0.z, G0.z, M0.z, V0.z); upd(P0.w, G0.w, M0.w, V0.w);
+        if constexpr (GROUPED) adam_upd4_group(*tab, seg, e0, gscale, P0, G0, M0, V0);
+        else { upd(P0.x, G0.x, M0.x, V0.x); upd(P0.y, G0.y, M0.y, V0.y); upd(P0.z, G0.z, M0.z, V0.z); upd(P0.w, G0.w, M0.w, V0.w); }
         m[i0] = M0; v[i0] = V0;
         if (MULTIMEM) mm_st(p_mc + e0, P0);
         else
             for (int r = 0; r < world; ++r) *reinterpret_cast<float4 *>(peers.param[r] + e0) = P0;
         if (two) {
-            upd(P1.x, G1.x, M1.x, V1.x); upd(P1.y, G1.y, M1.y, V1.y); upd(P1.z, G1.z, M1.z, V1.z); upd(P1.w, G1.w, M1.w, V1.w);
+            if constexpr (GROUPED) adam_upd4_group(*tab, seg, e1, gscale, P1, G1, M1, V1);
+            else { upd(P1.x, G1.x, M1.x, V1.x); upd(P1.y, G1.y, M1.y, V1.y); upd(P1.z, G1.z, M1.z, V1.z); upd(P1.w, G1.w, M1.w, V1.w); }
             m[i1] = M1; v[i1] = V1;
             if (MULTIMEM) mm_st(p_mc + e1, P1);
             else
@@ -237,14 +392,20 @@ __device__ __forceinline__ uint32_t ab_smem(const void *p) { return (uint32_t)__
 
 constexpr int AB_THREADS = 128;          // 4 warps x <= 48 registers = 6 K registers: fits beside the tensor-core backward kernels
 
+// Groups = AdamGroups: c2v_adam_step_sharded_bulk_groups, the table's hyper-parameters instead of the scalar ones.
+template <class Groups = NoGroups>
 __global__ void __launch_bounds__(AB_THREADS)
 adam_step_bulk_kernel(const float *__restrict__ p_local, const AdamPeers peers, int world, float *__restrict__ m,
                       float *__restrict__ v, long long slice_begin, long long slice_n, int chunk,
                       float step_size, float one_minus_b1, float b2, float one_minus_b2, float inv_sqrt_bc2, float eps,
-                      float wd, float gscale)
+                      float wd, float gscale, const Groups groups)
 {
+    constexpr bool GROUPED = std::is_same<Groups, AdamGroups>::value;
     extern __shared__ __align__(128) unsigned char ab_raw[];
     __shared__ __align__(8) unsigned long long ab_bar[AB_STAGES];
+    AdamGroupsSmem *tab = nullptr;                           // (NoGroups: no shared memory for the table)
+    int seg = 0;
+    if constexpr (GROUPED) { tab = &groups_smem(); load_groups(*tab, groups, nullptr); }
     const int tid = threadIdx.x;
     const long long n_chunks = (slice_n + chunk - 1) / chunk;
     const long long my_chunks = (n_chunks - (long long)blockIdx.x + (long long)gridDim.x - 1) / (long long)gridDim.x;
@@ -315,7 +476,8 @@ adam_step_bulk_kernel(const float *__restrict__ p_local, const AdamPeers peers, 
                 P = *reinterpret_cast<const float4 *>(p_local + slice_begin + e);
                 M = *reinterpret_cast<const float4 *>(m + e); V = *reinterpret_cast<const float4 *>(v + e);
             }
-            upd(P.x, G.x, M.x, V.x); upd(P.y, G.y, M.y, V.y); upd(P.z, G.z, M.z, V.z); upd(P.w, G.w, M.w, V.w);
+            if constexpr (GROUPED) adam_upd4_group(*tab, seg, slice_begin + e, gscale, P, G, M, V);
+            else { upd(P.x, G.x, M.x, V.x); upd(P.y, G.y, M.y, V.y); upd(P.z, G.z, M.z, V.z); upd(P.w, G.w, M.w, V.w); }
             *reinterpret_cast<float4 *>(m + e) = M; *reinterpret_cast<float4 *>(v + e) = V;
             *reinterpret_cast<float4 *>(stage + i) = P;            // rank 0's buffer becomes the output staging
         }
@@ -448,9 +610,11 @@ static bool adam_buffers_ok(const char *fn, const float *param, const float *gra
 }
 
 // the flat update kernel; dev_scalars != NULL: its DEV_SCALARS instantiation, coef_dev != NULL: its DEV_COEF one
+template <class Groups>
 static int launch_adam_flat(float *param, float *grad, float *exp_avg, float *exp_avg_sq, int64_t n, float step_size,
                             float beta1, float beta2, float inv_sqrt_bc2, float eps, float weight_decay, float grad_scale,
-                            int32_t zero_grad, const float *dev_scalars, const float *coef_dev, cudaStream_t st)
+                            int32_t zero_grad, const float *dev_scalars, const float *coef_dev, const Groups &groups,
+                            cudaStream_t st)
 {
     const long long n4 = n / 4;
     const int tail = (int)(n % 4);
@@ -460,13 +624,13 @@ static int launch_adam_flat(float *param, float *grad, float *exp_avg, float *ex
     long long blocks = (n4 + 255) / 256;
     if (blocks > (long long)sms * 16) blocks = (long long)sms * 16;
     if (blocks < 1) blocks = 1;
-    auto kernel = dev_scalars ? (coef_dev ? adam_step_kernel<true, true> : adam_step_kernel<true>)
-                              : (coef_dev ? adam_step_kernel<false, true> : adam_step_kernel<false>);
+    auto kernel = dev_scalars ? (coef_dev ? adam_step_kernel<true, true, Groups> : adam_step_kernel<true, false, Groups>)
+                              : (coef_dev ? adam_step_kernel<false, true, Groups> : adam_step_kernel<false, false, Groups>);
     kernel<<<(unsigned)blocks, 256, 0, st>>>(
         reinterpret_cast<float4 *>(param), reinterpret_cast<float4 *>(grad), reinterpret_cast<float4 *>(exp_avg),
         reinterpret_cast<float4 *>(exp_avg_sq), n4, param + n4 * 4, grad + n4 * 4, exp_avg + n4 * 4, exp_avg_sq + n4 * 4, tail,
         step_size, 1.0f - beta1, beta2, 1.0f - beta2, inv_sqrt_bc2, eps, weight_decay, grad_scale, zero_grad, dev_scalars,
-        coef_dev);
+        coef_dev, groups);
     C2V_LAUNCH_OK("adam_step_kernel");
     return C2V_OK;
 }
@@ -496,7 +660,7 @@ static int adam_step_flat(const char *fn, float *param, float *grad, float *exp_
         const float step_size = (float)((double)lr / bc1);
         const float inv_sqrt_bc2 = (float)(1.0 / sqrt(bc2));
         return launch_adam_flat(param, grad, exp_avg, exp_avg_sq, n, step_size, beta1, beta2, inv_sqrt_bc2, eps,
-                                weight_decay, grad_scale, zero_grad, nullptr, coef_dev, st);
+                                weight_decay, grad_scale, zero_grad, nullptr, coef_dev, NoGroups{}, st);
     }
     if (reinterpret_cast<uintptr_t>(step_state) & 7) {
         set_error("%s: step_state must be an 8-byte aligned device buffer of 16 bytes", fn);
@@ -506,7 +670,7 @@ static int adam_step_flat(const char *fn, float *param, float *grad, float *exp_
     adam_step_count_kernel<<<1, 1, 0, st>>>(state, lr, beta1, beta2, lr_dev);
     C2V_LAUNCH_OK("adam_step_count_kernel");
     return launch_adam_flat(param, grad, exp_avg, exp_avg_sq, n, 0.0f, beta1, beta2, 0.0f, eps, weight_decay, grad_scale,
-                            zero_grad, reinterpret_cast<const float *>(state + 1), coef_dev, st);
+                            zero_grad, reinterpret_cast<const float *>(state + 1), coef_dev, NoGroups{}, st);
 }
 
 extern "C" int c2v_adam_step(float *param, float *grad, float *exp_avg, float *exp_avg_sq, int64_t n, float lr,
@@ -572,24 +736,92 @@ extern "C" int c2v_grad_clip_coef(const float *grad, int64_t n, float grad_scale
     return C2V_OK;
 }
 
-extern "C" int c2v_adam_step_sharded(const float *param_local, float *param_multicast, const float *grad_multicast,
-                                     float *const *param_peers, const float *const *grad_peers, int32_t world,
-                                     float *exp_avg_slice, float *exp_avg_sq_slice, int64_t slice_begin, int64_t slice_n,
-                                     float *zero_buffer, int64_t zero_n, float lr, float beta1, float beta2, float eps,
-                                     float weight_decay, int64_t step, float grad_scale, void *stream)
+// ---- parameter groups: the table of c2v_adam_step_groups and its sharded counterparts --------------------------------
+// Checks the table (C2V_EINVAL before any CUDA call) and fills `args` (the groups, for the step-count kernel) and `tab`
+// (the segments; the hyper-parameters at host step `step` when step >= 1)
+static bool adam_groups_ok(const char *fn, const c2v_adam_group *groups, int32_t n_groups, const int64_t *seg_begin,
+                           const int32_t *seg_group, int32_t n_segments, bool device_lr, int64_t step,
+                           AdamGroupArgs &args, AdamGroups &tab)
+{
+    if (!groups || !seg_begin || !seg_group || n_groups < 1 || n_groups > ADAM_MAX_GROUPS || n_segments < 1 ||
+        n_segments > ADAM_MAX_SEGMENTS) {
+        set_error("%s: bad group table (%d groups, %d segments; 1 to %d groups and 1 to %d segments, no NULL pointer)", fn,
+                  n_groups, n_segments, ADAM_MAX_GROUPS, ADAM_MAX_SEGMENTS);
+        return false;
+    }
+    memset(&args, 0, sizeof(args));
+    memset(&tab, 0, sizeof(tab));
+    for (int s = 0; s < n_segments; ++s) {
+        if ((s == 0 ? seg_begin[0] != 0 : seg_begin[s] <= seg_begin[s - 1]) || seg_group[s] < 0 || seg_group[s] >= n_groups) {
+            set_error("%s: segment %d (begin %lld, group %d): segments must begin at 0, ascend strictly and name a group "
+                      "in [0, %d)", fn, s, (long long)seg_begin[s], seg_group[s], n_groups);
+            return false;
+        }
+        tab.seg_begin[s] = seg_begin[s];
+        tab.seg_group[s] = seg_group[s];
+    }
+    for (int k = 0; k < n_groups; ++k) {
+        if (groups[k].lr_dev && (!device_lr || misaligned(groups[k].lr_dev, 4))) {
+            set_error("%s: group %d: lr_dev needs the step count on the device (step_state) and 4-byte alignment", fn, k);
+            return false;
+        }
+        args.g[k] = groups[k];
+        if (step >= 1) tab.hyper[k] = adam_hyper(groups[k], groups[k].lr, step);
+        else tab.hyper[k] = adam_hyper(groups[k], 0.0f, 1);    // step_size, inv_sqrt_bc2, decay: from the device
+    }
+    args.n = tab.n_groups = n_groups;
+    tab.n_segments = n_segments;
+    return true;
+}
+
+extern "C" int c2v_adam_step_groups(float *param, float *grad, float *exp_avg, float *exp_avg_sq, int64_t n,
+                                    const c2v_adam_group *groups, int32_t n_groups, const int64_t *seg_begin,
+                                    const int32_t *seg_group, int32_t n_segments, int64_t step, void *step_state,
+                                    float grad_scale, int32_t zero_grad, const float *coef_dev, void *stream)
+{
+    const char *fn = "c2v_adam_step_groups";
+    if (!adam_buffers_ok(fn, param, grad, exp_avg, exp_avg_sq, n)) return C2V_EINVAL;
+    if (misaligned(coef_dev, 4) || (reinterpret_cast<uintptr_t>(step_state) & 7) || (!step_state && step < 1)) {
+        set_error("%s: bad argument (coef_dev: 4-byte aligned, step_state: 8-byte aligned, else step >= 1)", fn);
+        return C2V_EINVAL;
+    }
+    AdamGroupArgs args;
+    AdamGroups tab;
+    if (!adam_groups_ok(fn, groups, n_groups, seg_begin, seg_group, n_segments, step_state != nullptr,
+                        step_state ? 0 : step, args, tab))
+        return C2V_EINVAL;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const float *dev_scalars = nullptr;
+    if (step_state) {
+        long long *state = static_cast<long long *>(step_state);
+        adam_step_count_groups_kernel<<<1, 1, 0, st>>>(state, args);
+        C2V_LAUNCH_OK("adam_step_count_groups_kernel");
+        dev_scalars = reinterpret_cast<const float *>(state + 1);
+    }
+    return launch_adam_flat(param, grad, exp_avg, exp_avg_sq, n, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, grad_scale, zero_grad,
+                            dev_scalars, coef_dev, tab, st);
+}
+
+// c2v_adam_step_sharded (Groups = NoGroups: the scalar hyper-parameters) and c2v_adam_step_sharded_groups
+template <class Groups>
+static int adam_step_sharded(const char *fn, const float *param_local, float *param_multicast, const float *grad_multicast,
+                             float *const *param_peers, const float *const *grad_peers, int32_t world,
+                             float *exp_avg_slice, float *exp_avg_sq_slice, int64_t slice_begin, int64_t slice_n,
+                             float *zero_buffer, int64_t zero_n, float lr, float beta1, float beta2, float eps,
+                             float weight_decay, int64_t step, float grad_scale, const Groups &groups, void *stream)
 {
     if (!param_local || !exp_avg_slice || !exp_avg_sq_slice || slice_n < 0 || slice_begin < 0 || step < 1 || world < 1 ||
         world > 16) {
-        set_error("c2v_adam_step_sharded: bad argument");
+        set_error("%s: bad argument", fn);
         return C2V_EINVAL;
     }
     const bool mm = param_multicast != nullptr && grad_multicast != nullptr;
     if (!mm && (!param_peers || !grad_peers)) {
-        set_error("c2v_adam_step_sharded: needs either the multicast pointers or the peer pointer tables");
+        set_error("%s: needs either the multicast pointers or the peer pointer tables", fn);
         return C2V_EINVAL;
     }
     if ((slice_begin | slice_n | zero_n) & 3) {
-        set_error("c2v_adam_step_sharded: slice_begin, slice_n and zero_n must be multiples of 4 elements");
+        set_error("%s: slice_begin, slice_n and zero_n must be multiples of 4 elements", fn);
         return C2V_EINVAL;
     }
     AdamPeers peers;
@@ -599,11 +831,11 @@ extern "C" int c2v_adam_step_sharded(const float *param_local, float *param_mult
                       reinterpret_cast<uintptr_t>(param_multicast) | reinterpret_cast<uintptr_t>(grad_multicast);
     if (!mm)
         for (int r = 0; r < world; ++r) {
-            if (!param_peers[r] || !grad_peers[r]) { set_error("c2v_adam_step_sharded: NULL peer pointer %d", r); return C2V_EINVAL; }
+            if (!param_peers[r] || !grad_peers[r]) { set_error("%s: NULL peer pointer %d", fn, r); return C2V_EINVAL; }
             peers.param[r] = param_peers[r]; peers.grad[r] = grad_peers[r];
             align |= reinterpret_cast<uintptr_t>(param_peers[r]) | reinterpret_cast<uintptr_t>(grad_peers[r]);
         }
-    if (align & 15) { set_error("c2v_adam_step_sharded: buffers must be 16-byte aligned"); return C2V_EINVAL; }
+    if (align & 15) { set_error("%s: buffers must be 16-byte aligned", fn); return C2V_EINVAL; }
     const double bc1 = 1.0 - pow((double)beta1, (double)step), bc2 = 1.0 - pow((double)beta2, (double)step);
     const float step_size = (float)((double)lr / bc1);
     const float inv_sqrt_bc2 = (float)(1.0 / sqrt(bc2));
@@ -617,27 +849,58 @@ extern "C" int c2v_adam_step_sharded(const float *param_local, float *param_mult
     blocks = blocks / 4 * 4;                                  // every 4th CTA zero-fills
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     if (mm)
-        adam_step_sharded_kernel<true><<<(unsigned)blocks, 128, 0, st>>>(
+        adam_step_sharded_kernel<true, Groups><<<(unsigned)blocks, 128, 0, st>>>(
             param_local, param_multicast, grad_multicast, peers, world, reinterpret_cast<float4 *>(exp_avg_slice),
             reinterpret_cast<float4 *>(exp_avg_sq_slice), slice_begin, n4, reinterpret_cast<float4 *>(zero_buffer), z4,
-            step_size, 1.0f - beta1, beta2, 1.0f - beta2, inv_sqrt_bc2, eps, weight_decay, grad_scale);
+            step_size, 1.0f - beta1, beta2, 1.0f - beta2, inv_sqrt_bc2, eps, weight_decay, grad_scale, groups);
     else
-        adam_step_sharded_kernel<false><<<(unsigned)blocks, 128, 0, st>>>(
+        adam_step_sharded_kernel<false, Groups><<<(unsigned)blocks, 128, 0, st>>>(
             param_local, param_multicast, grad_multicast, peers, world, reinterpret_cast<float4 *>(exp_avg_slice),
             reinterpret_cast<float4 *>(exp_avg_sq_slice), slice_begin, n4, reinterpret_cast<float4 *>(zero_buffer), z4,
-            step_size, 1.0f - beta1, beta2, 1.0f - beta2, inv_sqrt_bc2, eps, weight_decay, grad_scale);
+            step_size, 1.0f - beta1, beta2, 1.0f - beta2, inv_sqrt_bc2, eps, weight_decay, grad_scale, groups);
     C2V_LAUNCH_OK("adam_step_sharded_kernel");
     return C2V_OK;
 }
 
-extern "C" int c2v_adam_step_sharded_bulk(const float *param_local, float *const *param_peers, const float *const *grad_peers,
-                                          int32_t world, float *exp_avg_slice, float *exp_avg_sq_slice, int64_t slice_begin,
-                                          int64_t slice_n, float lr, float beta1, float beta2, float eps, float weight_decay,
-                                          int64_t step, float grad_scale, int32_t max_ctas, void *stream)
+extern "C" int c2v_adam_step_sharded(const float *param_local, float *param_multicast, const float *grad_multicast,
+                                     float *const *param_peers, const float *const *grad_peers, int32_t world,
+                                     float *exp_avg_slice, float *exp_avg_sq_slice, int64_t slice_begin, int64_t slice_n,
+                                     float *zero_buffer, int64_t zero_n, float lr, float beta1, float beta2, float eps,
+                                     float weight_decay, int64_t step, float grad_scale, void *stream)
+{
+    return adam_step_sharded("c2v_adam_step_sharded", param_local, param_multicast, grad_multicast, param_peers, grad_peers,
+                             world, exp_avg_slice, exp_avg_sq_slice, slice_begin, slice_n, zero_buffer, zero_n, lr, beta1,
+                             beta2, eps, weight_decay, step, grad_scale, NoGroups{}, stream);
+}
+
+extern "C" int c2v_adam_step_sharded_groups(const float *param_local, float *param_multicast, const float *grad_multicast,
+                                            float *const *param_peers, const float *const *grad_peers, int32_t world,
+                                            float *exp_avg_slice, float *exp_avg_sq_slice, int64_t slice_begin,
+                                            int64_t slice_n, float *zero_buffer, int64_t zero_n,
+                                            const c2v_adam_group *groups, int32_t n_groups, const int64_t *seg_begin,
+                                            const int32_t *seg_group, int32_t n_segments, int64_t step, float grad_scale,
+                                            void *stream)
+{
+    const char *fn = "c2v_adam_step_sharded_groups";
+    AdamGroupArgs args;
+    AdamGroups tab;
+    if (!adam_groups_ok(fn, groups, n_groups, seg_begin, seg_group, n_segments, false, step, args, tab)) return C2V_EINVAL;
+    return adam_step_sharded(fn, param_local, param_multicast, grad_multicast, param_peers, grad_peers, world, exp_avg_slice,
+                             exp_avg_sq_slice, slice_begin, slice_n, zero_buffer, zero_n, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, step,
+                             grad_scale, tab, stream);
+}
+
+// c2v_adam_step_sharded_bulk (Groups = NoGroups) and c2v_adam_step_sharded_bulk_groups
+template <class Groups>
+static int adam_step_bulk(const char *fn, const float *param_local, float *const *param_peers,
+                          const float *const *grad_peers, int32_t world, float *exp_avg_slice, float *exp_avg_sq_slice,
+                          int64_t slice_begin, int64_t slice_n, float lr, float beta1, float beta2, float eps,
+                          float weight_decay, int64_t step, float grad_scale, int32_t max_ctas, const Groups &groups,
+                          void *stream)
 {
     if (!param_local || !param_peers || !grad_peers || !exp_avg_slice || !exp_avg_sq_slice || slice_n < 0 || slice_begin < 0 ||
         step < 1 || world < 1 || world > 16 || ((slice_begin | slice_n) & 3)) {
-        set_error("c2v_adam_step_sharded_bulk: bad argument");
+        set_error("%s: bad argument", fn);
         return C2V_EINVAL;
     }
     AdamPeers peers;
@@ -645,11 +908,11 @@ extern "C" int c2v_adam_step_sharded_bulk(const float *param_local, float *const
     uintptr_t align = reinterpret_cast<uintptr_t>(param_local) | reinterpret_cast<uintptr_t>(exp_avg_slice) |
                       reinterpret_cast<uintptr_t>(exp_avg_sq_slice);
     for (int r = 0; r < world; ++r) {
-        if (!param_peers[r] || !grad_peers[r]) { set_error("c2v_adam_step_sharded_bulk: NULL peer pointer %d", r); return C2V_EINVAL; }
+        if (!param_peers[r] || !grad_peers[r]) { set_error("%s: NULL peer pointer %d", fn, r); return C2V_EINVAL; }
         peers.param[r] = param_peers[r]; peers.grad[r] = grad_peers[r];
         align |= reinterpret_cast<uintptr_t>(param_peers[r]) | reinterpret_cast<uintptr_t>(grad_peers[r]);
     }
-    if (align & 15) { set_error("c2v_adam_step_sharded_bulk: buffers must be 16-byte aligned"); return C2V_EINVAL; }
+    if (align & 15) { set_error("%s: buffers must be 16-byte aligned", fn); return C2V_EINVAL; }
     if (slice_n == 0) return C2V_OK;
     const double bc1 = 1.0 - pow((double)beta1, (double)step), bc2 = 1.0 - pow((double)beta2, (double)step);
     const float step_size = (float)((double)lr / bc1);
@@ -662,12 +925,37 @@ extern "C" int c2v_adam_step_sharded_bulk(const float *param_local, float *const
     long long grid = max_ctas > 0 ? max_ctas : sms;
     if (grid > n_chunks) grid = n_chunks;
     const int smem = AB_STAGES * AB_STAGE_BYTES;
-    C2V_CUDA_OK(cudaFuncSetAttribute(adam_step_bulk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    adam_step_bulk_kernel<<<(unsigned)grid, AB_THREADS, smem, static_cast<cudaStream_t>(stream)>>>(
+    C2V_CUDA_OK(cudaFuncSetAttribute(adam_step_bulk_kernel<Groups>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    adam_step_bulk_kernel<Groups><<<(unsigned)grid, AB_THREADS, smem, static_cast<cudaStream_t>(stream)>>>(
         param_local, peers, world, exp_avg_slice, exp_avg_sq_slice, slice_begin, slice_n, chunk, step_size, 1.0f - beta1, beta2,
-        1.0f - beta2, inv_sqrt_bc2, eps, weight_decay, grad_scale);
+        1.0f - beta2, inv_sqrt_bc2, eps, weight_decay, grad_scale, groups);
     C2V_LAUNCH_OK("adam_step_bulk_kernel");
     return C2V_OK;
+}
+
+extern "C" int c2v_adam_step_sharded_bulk(const float *param_local, float *const *param_peers, const float *const *grad_peers,
+                                          int32_t world, float *exp_avg_slice, float *exp_avg_sq_slice, int64_t slice_begin,
+                                          int64_t slice_n, float lr, float beta1, float beta2, float eps, float weight_decay,
+                                          int64_t step, float grad_scale, int32_t max_ctas, void *stream)
+{
+    return adam_step_bulk("c2v_adam_step_sharded_bulk", param_local, param_peers, grad_peers, world, exp_avg_slice,
+                          exp_avg_sq_slice, slice_begin, slice_n, lr, beta1, beta2, eps, weight_decay, step, grad_scale,
+                          max_ctas, NoGroups{}, stream);
+}
+
+extern "C" int c2v_adam_step_sharded_bulk_groups(const float *param_local, float *const *param_peers,
+                                                 const float *const *grad_peers, int32_t world, float *exp_avg_slice,
+                                                 float *exp_avg_sq_slice, int64_t slice_begin, int64_t slice_n,
+                                                 const c2v_adam_group *groups, int32_t n_groups, const int64_t *seg_begin,
+                                                 const int32_t *seg_group, int32_t n_segments, int64_t step,
+                                                 float grad_scale, int32_t max_ctas, void *stream)
+{
+    const char *fn = "c2v_adam_step_sharded_bulk_groups";
+    AdamGroupArgs args;
+    AdamGroups tab;
+    if (!adam_groups_ok(fn, groups, n_groups, seg_begin, seg_group, n_segments, false, step, args, tab)) return C2V_EINVAL;
+    return adam_step_bulk(fn, param_local, param_peers, grad_peers, world, exp_avg_slice, exp_avg_sq_slice, slice_begin,
+                          slice_n, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, step, grad_scale, max_ctas, tab, stream);
 }
 
 extern "C" int c2v_sparse_adam_step(float *param, float *exp_avg, float *exp_avg_sq, const float *values,

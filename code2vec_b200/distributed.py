@@ -74,32 +74,96 @@ class FlatGradBucket:
                 self.flat.mul_(1.0 / dist.get_world_size())
 
 
-class _FlatAdamBase(torch.optim.Optimizer):
-    """What FlatAdam and ShardedFlatAdam share as torch.optim.Optimizers: ONE parameter group (a flat launch has one set of
-    hyper-parameters) that is the source of truth for lr, betas, eps, weight_decay and max_grad_norm, so that the
-    torch.optim.lr_scheduler classes drive them (the group's `capturable` records the `capturable` attribute, which is
-    fixed at construction); state_dict() / load_state_dict() in torch.optim.Adam's format; and the flat launch itself.  Subclasses provide `_flat_offsets` (caller-order parameter -> offset in the flat buffers),
-    `_gather_state()` and `_scatter_state()`."""
+# the parameter-group keys of FlatAdam / ShardedFlatAdam; torch.optim.Adam's amsgrad and maximize are accepted as False
+_GROUP_KEYS = ("params", "lr", "betas", "eps", "weight_decay", "decoupled_weight_decay", "max_grad_norm", "capturable")
+_FALSE_KEYS = ("amsgrad", "maximize")
+# settings of the whole optimizer: one global norm for clipping, one place for the step count
+_WHOLE_KEYS = ("max_grad_norm", "capturable")
 
-    def _init_optimizer(self, params, dev, lr, betas, eps, weight_decay, max_grad_norm, capturable):
-        if isinstance(lr, torch.Tensor):
-            if not capturable:
-                raise ValueError("a tensor lr is read by the captured step-count kernel: it needs capturable=True")
-            if lr.device != dev or lr.dtype != torch.float32 or lr.numel() != 1:
-                raise ValueError(f"a tensor lr must be a one-element fp32 tensor on {dev}, got {lr.dtype} "
-                                 f"{tuple(lr.shape)} on {lr.device}")
-        else:
-            lr = float(lr)
+
+class _FlatAdamBase(torch.optim.Optimizer):
+    """What FlatAdam and ShardedFlatAdam share as torch.optim.Optimizers: parameter groups that are the source of truth
+    for lr, betas, eps, weight_decay, decoupled_weight_decay (per group) and max_grad_norm (the same in every group: one
+    global norm), so that the torch.optim.lr_scheduler classes drive them (a group's `capturable` records the `capturable`
+    attribute, which is fixed at construction); state_dict() / load_state_dict() in torch.optim.Adam's format; and the flat
+    launch itself.  The groups are fixed at construction: the flat layout is.  One group without decoupled weight decay
+    launches the one-group kernels; otherwise the grouped ones (c2v_adam_step_groups), whose segment table maps the flat
+    buffers to the groups.  Subclasses provide `_flat_offsets` (parameter in group order -> offset in the flat buffers),
+    call `_layout_groups`, and provide `_gather_state()` and `_scatter_state()`."""
+
+    def _init_optimizer(self, params, dev, lr, betas, eps, weight_decay, max_grad_norm, capturable,
+                        decoupled_weight_decay=False):
         if max_grad_norm is not None and not float(max_grad_norm) > 0.0:
             raise ValueError(f"max_grad_norm must be None or > 0, got {max_grad_norm}")
-        super().__init__(params, dict(lr=lr, betas=(float(betas[0]), float(betas[1])), eps=float(eps),
-                                      weight_decay=float(weight_decay),
-                                      max_grad_norm=None if max_grad_norm is None else float(max_grad_norm),
-                                      capturable=bool(capturable)))
         self.capturable = bool(capturable)               # fixed at construction: it decides where the step count lives
+        self._dev = dev
+        self._building = True
+        super().__init__(params, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay,
+                                      decoupled_weight_decay=decoupled_weight_decay, max_grad_norm=max_grad_norm,
+                                      capturable=capturable))
+        self._building = False
+        for group in self.param_groups:
+            self._check_group(group)
+        for k in _WHOLE_KEYS:
+            self._whole(k)
+        self._ordered = [p for g in self.param_groups for p in g["params"]]     # state_dict()'s numbering
+        if len({id(p) for p in self._ordered}) != len(self._ordered):
+            raise ValueError(f"{type(self).__name__}: a parameter appears more than once in the parameter groups")
         # {norm, coef} of the last clipped step (c2v_grad_clip_coef) and the per-CTA partials of its norm pass
         self._norm_coef = torch.zeros(2, dtype=torch.float32, device=dev)
         self._norm_ws = torch.empty(1024, dtype=torch.float32, device=dev)
+
+    def _check_group(self, group):
+        name = type(self).__name__
+        for k in group:
+            if k in _FALSE_KEYS:
+                if group[k]:
+                    raise ValueError(f"{name}: {k}=True is not this optimizer's update rule")
+            elif k not in _GROUP_KEYS:
+                raise ValueError(f"{name}: unknown parameter-group key {k!r} (the keys are {', '.join(_GROUP_KEYS)})")
+        lr = group["lr"]
+        if isinstance(lr, torch.Tensor):
+            if not self.capturable:
+                raise ValueError("a tensor lr is read by the captured step-count kernel: it needs capturable=True")
+            if lr.device != self._dev or lr.dtype != torch.float32 or lr.numel() != 1:
+                raise ValueError(f"a tensor lr must be a one-element fp32 tensor on {self._dev}, got {lr.dtype} "
+                                 f"{tuple(lr.shape)} on {lr.device}")
+        else:
+            group["lr"] = float(lr)
+        mgn = group["max_grad_norm"]
+        if mgn is not None and not float(mgn) > 0.0:
+            raise ValueError(f"max_grad_norm must be None or > 0, got {mgn}")
+        group.update(betas=(float(group["betas"][0]), float(group["betas"][1])), eps=float(group["eps"]),
+                     weight_decay=float(group["weight_decay"]),
+                     decoupled_weight_decay=bool(group["decoupled_weight_decay"]),
+                     max_grad_norm=None if mgn is None else float(mgn), capturable=bool(group["capturable"]))
+        if group["capturable"] != self.capturable:
+            raise ValueError(f"{name}: capturable is a setting of the whole optimizer, a group has "
+                             f"capturable={group['capturable']}")
+
+    def _whole(self, key):
+        """the value of a setting of the whole optimizer; ValueError when the groups disagree"""
+        values = [g[key] for g in self.param_groups]
+        if any(v != values[0] for v in values):
+            raise ValueError(f"{type(self).__name__}: {key} is a setting of the whole optimizer (clipping uses one "
+                             f"global norm, the step count is shared), but the parameter groups have {values}")
+        return values[0]
+
+    def _layout_groups(self, flat_params, offsets):
+        """the segment table: maximal runs of one group over `flat_params` (flat order, at `offsets`), as
+        [(first flat element, group)], the first at 0"""
+        gid = {id(p): k for k, g in enumerate(self.param_groups) for p in g["params"]}
+        segs = []
+        for p, o in zip(flat_params, offsets):
+            if p.numel() and (not segs or segs[-1][1] != gid[id(p)]):
+                segs.append((o, gid[id(p)]))
+        segs = [(0, segs[0][1] if segs else 0)] + segs[1:]
+        from . import _lib
+        if len(self.param_groups) > _lib.ADAM_MAX_GROUPS or len(segs) > _lib.ADAM_MAX_SEGMENTS:
+            raise ValueError(f"{type(self).__name__}: {len(self.param_groups)} parameter groups in {len(segs)} runs of "
+                             f"the flat buffers; the grouped kernels take up to {_lib.ADAM_MAX_GROUPS} groups and "
+                             f"{_lib.ADAM_MAX_SEGMENTS} runs")
+        self._segments = segs
 
     def _patch_step_function(self):
         # torch wraps the class's step() with the step hooks when the first instance is built; wrap this instance's
@@ -108,17 +172,26 @@ class _FlatAdamBase(torch.optim.Optimizer):
         self.step = torch.optim.Optimizer.profile_hook_step(type(self).step).__get__(self)
 
     def add_param_group(self, param_group):
-        if self.param_groups:
-            raise ValueError(f"{type(self).__name__} has one parameter group: one flat launch has one set of "
-                             "hyper-parameters")
+        if not self._building:
+            if len(self.param_groups) == 1:
+                raise ValueError(f"{type(self).__name__} has one parameter group: one flat launch has one set of "
+                                 "hyper-parameters")
+            raise ValueError(f"{type(self).__name__}: the parameter groups are fixed at construction, where the flat "
+                             "buffers are laid out")
         super().add_param_group(param_group)
 
     def _group_value(name):
+        def one(self):
+            if len(self.param_groups) > 1:
+                raise AttributeError(f"{type(self).__name__} has {len(self.param_groups)} parameter groups: "
+                                     f"use param_groups[k][{name!r}]")
+            return self.param_groups[0]
+
         def get(self):
-            return self.param_groups[0][name]
+            return one(self)[name]
 
         def put(self, value):
-            g = self.param_groups[0]
+            g = one(self)
             if name == "lr" and isinstance(g["lr"], torch.Tensor):
                 g["lr"].fill_(float(value))              # a captured graph reads this address
             else:
@@ -126,8 +199,20 @@ class _FlatAdamBase(torch.optim.Optimizer):
         return property(get, put)
 
     lr, betas, eps, weight_decay = _group_value("lr"), _group_value("betas"), _group_value("eps"), _group_value("weight_decay")
-    max_grad_norm = _group_value("max_grad_norm")
     del _group_value
+
+    @property
+    def max_grad_norm(self):
+        return self._whole("max_grad_norm")
+
+    @max_grad_norm.setter
+    def max_grad_norm(self, value):
+        for g in self.param_groups:
+            g["max_grad_norm"] = value
+
+    def _grouped(self):
+        """whether the step takes the grouped kernels: more than one group, or decoupled weight decay"""
+        return len(self.param_groups) > 1 or self.param_groups[0]["decoupled_weight_decay"]
 
     def step_count(self):
         """the number of steps taken (synchronises in capturable mode)"""
@@ -139,17 +224,36 @@ class _FlatAdamBase(torch.optim.Optimizer):
         the clip: what clip_grad_norm_ returns); written only by steps with max_grad_norm set.  No synchronise."""
         return self._norm_coef[:1]
 
-    def _launch(self, p, g, m, v, step, grad_scale, zero_grad):
+    def _group_table(self, lo=0, n=None):
+        """the groups (c2v_adam_group[]) and the segments that meet flat elements [lo, lo + n), rebased to lo:
+        (groups, n_groups, seg_begin, seg_group, n_segments) for the *_groups entry points"""
+        import ctypes
+        from . import _lib
+        groups = (_lib.AdamGroup * len(self.param_groups))()
+        for a, g in zip(groups, self.param_groups):
+            lr = g["lr"]
+            a.lr, a.lr_dev = (0.0, lr.data_ptr()) if isinstance(lr, torch.Tensor) else (float(lr), None)
+            a.beta1, a.beta2 = g["betas"]
+            a.eps, a.weight_decay, a.decoupled = g["eps"], g["weight_decay"], 1 if g["decoupled_weight_decay"] else 0
+        segs = self._segments
+        if lo:
+            hi = lo + n
+            segs = [(max(b - lo, 0), k) for i, (b, k) in enumerate(segs)
+                    if b < hi and (i + 1 == len(segs) or segs[i + 1][0] > lo)]
+        begin = (ctypes.c_int64 * len(segs))(*[b for b, _ in segs])
+        group = (ctypes.c_int32 * len(segs))(*[k for _, k in segs])
+        return groups, len(groups), begin, group, len(segs)
+
+    def _launch(self, p, g, m, v, step, grad_scale, zero_grad, lo=0):
         """c2v_adam_step_ex on flat fp32 buffers with the group's hyper-parameters, behind c2v_grad_clip_coef on the same
         gradient when max_grad_norm is set.  With max_grad_norm None and a float lr it is c2v_adam_step /
-        c2v_adam_step_capturable: same kernels, same launch parameters."""
+        c2v_adam_step_capturable: same kernels, same launch parameters.  With parameter groups (or decoupled weight
+        decay) c2v_adam_step_groups; p begins at flat element `lo`."""
         import ctypes
         from . import _lib
         lib = _lib.load()
         P = lambda t: ctypes.c_void_p(t.data_ptr())
-        group = self.param_groups[0]
-        lr, (beta1, beta2), max_norm = group["lr"], group["betas"], group["max_grad_norm"]
-        lr_dev = P(lr) if isinstance(lr, torch.Tensor) else None
+        max_norm = self.max_grad_norm
         dev = p.device
         with torch.cuda.device(dev):
             stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
@@ -159,54 +263,70 @@ class _FlatAdamBase(torch.optim.Optimizer):
                                             P(self._norm_ws), 4 * self._norm_ws.numel(), stream)
                 _lib.check(rc, "c2v_grad_clip_coef")
                 coef_dev = ctypes.c_void_p(self._norm_coef.data_ptr() + 4)
+            state = P(self.step_state) if self.capturable else None
+            if self._grouped():
+                rc = lib.c2v_adam_step_groups(P(p), P(g), P(m), P(v), p.numel(), *self._group_table(lo, p.numel()), step,
+                                              state, float(grad_scale), 1 if zero_grad else 0, coef_dev, stream)
+                _lib.check(rc, "c2v_adam_step_groups")
+                return
+            group = self.param_groups[0]
+            lr, (beta1, beta2) = group["lr"], group["betas"]
+            lr_dev = P(lr) if isinstance(lr, torch.Tensor) else None
             rc = lib.c2v_adam_step_ex(P(p), P(g), P(m), P(v), p.numel(), 0.0 if lr_dev else float(lr), beta1, beta2,
-                                      group["eps"], group["weight_decay"], step,
-                                      P(self.step_state) if self.capturable else None, float(grad_scale),
+                                      group["eps"], group["weight_decay"], step, state, float(grad_scale),
                                       1 if zero_grad else 0, lr_dev, coef_dev, stream)
         _lib.check(rc, "c2v_adam_step_ex")
 
     # ---- checkpoints ---------------------------------------------------------------------------------------------------
     def state_dict(self):
-        """torch.optim.Adam's state_dict for the same parameters in the order the caller passed them:
-        state[i] = {"step", "exp_avg", "exp_avg_sq"} (copies shaped like parameter i; step a tensor as in torch: on the
-        device and without a host read when capturable, a CPU fp32 scalar otherwise) and one group with integer
-        `params`, plus the key max_grad_norm.  torch.optim.Adam loads it and continues.  ShardedFlatAdam at world
-        size > 1: a collective, every rank returns the full dict."""
+        """torch.optim.Adam's (or, with decoupled_weight_decay, torch.optim.AdamW's) state_dict for the same parameter
+        groups: state[i] = {"step", "exp_avg", "exp_avg_sq"} for the parameters numbered across the groups in order
+        (copies shaped like parameter i; step a tensor as in torch: on the device and without a host read when
+        capturable, a CPU fp32 scalar otherwise) and one dict per group with integer `params`, plus the key
+        max_grad_norm.  torch.optim.Adam / AdamW load it and continue.  ShardedFlatAdam at world size > 1: a collective,
+        every rank returns the full dict."""
         exp_avg, exp_avg_sq = self._gather_state()
         if self.capturable:
             step = self.step_state[0].to(torch.float32)
         else:
             step = torch.tensor(float(self.t), dtype=torch.float32)
-        params = self.param_groups[0]["params"]
         state = {}
-        for i, (p, o) in enumerate(zip(params, self._flat_offsets)):
+        for i, (p, o) in enumerate(zip(self._ordered, self._flat_offsets)):
             n = p.numel()
             state[i] = {"step": step.clone(), "exp_avg": exp_avg[o:o + n].view_as(p).clone(),
                         "exp_avg_sq": exp_avg_sq[o:o + n].view_as(p).clone()}
-        group = {k: (v.clone() if isinstance(v, torch.Tensor) else v) for k, v in self.param_groups[0].items()
-                 if k != "params"}
-        group["params"] = list(range(len(params)))
-        return {"state": state, "param_groups": [group]}
+        groups, i = [], 0
+        for g in self.param_groups:
+            group = {k: (v.clone() if isinstance(v, torch.Tensor) else v) for k, v in g.items() if k != "params"}
+            group["params"] = list(range(i, i + len(g["params"])))
+            i += len(g["params"])
+            groups.append(group)
+        return {"state": state, "param_groups": groups}
 
     def load_state_dict(self, state_dict):
-        """Loads state_dict()'s output or torch.optim.Adam's for the same parameters.  The group's hyper-parameters are
-        taken over (a tensor lr is filled in place, capturable stays as constructed, max_grad_norm defaults to None),
-        the moments are copied into the flat buffers (at world size > 1: this rank's slices of them) and the step count
-        is set.  Parameters without state load as zeros and step 0; per-parameter steps that differ raise ValueError:
-        the flat kernel has one step count."""
-        groups = state_dict["param_groups"]
-        params = self.param_groups[0]["params"]
-        if len(groups) != 1 or len(groups[0]["params"]) != len(params):
-            raise ValueError(f"{type(self).__name__}.load_state_dict: expected one parameter group of {len(params)} "
-                             f"parameters, got {[len(g['params']) for g in groups]}")
-        saved = groups[0]
-        for k in ("amsgrad", "maximize", "decoupled_weight_decay"):
-            if saved.get(k):
-                raise ValueError(f"{type(self).__name__}.load_state_dict: {k}=True is not this optimizer's update rule")
+        """Loads state_dict()'s output, torch.optim.Adam's or torch.optim.AdamW's for the same parameter groups (the
+        same count, with the same number of parameters each).  Each group's hyper-parameters are taken over (a tensor
+        lr is filled in place, capturable stays as constructed, decoupled_weight_decay defaults to False and
+        max_grad_norm to None), the moments are copied into the flat buffers (at world size > 1: this rank's slices of
+        them) and the step count is set.  Parameters without state load as zeros and step 0; per-parameter steps that
+        differ raise ValueError: the flat kernel has one step count."""
+        saved_groups, mine = state_dict["param_groups"], self.param_groups
+        if len(saved_groups) != len(mine) or any(len(s["params"]) != len(g["params"])
+                                                 for s, g in zip(saved_groups, mine)):
+            want = (f"one parameter group of {len(mine[0]['params'])} parameters" if len(mine) == 1 else
+                    f"{len(mine)} parameter groups of {[len(g['params']) for g in mine]} parameters")
+            raise ValueError(f"{type(self).__name__}.load_state_dict: expected {want}, got "
+                             f"{[len(g['params']) for g in saved_groups]}")
+        for saved in saved_groups:
+            for k in _FALSE_KEYS:
+                if saved.get(k):
+                    raise ValueError(f"{type(self).__name__}.load_state_dict: {k}=True is not this optimizer's update "
+                                     "rule")
         state, steps = state_dict["state"], set()
         exp_avg, exp_avg_sq = (torch.zeros(self._flat_numel, dtype=torch.float32, device=self._norm_coef.device)
                                for _ in range(2))
-        for i, (p, o, key) in enumerate(zip(params, self._flat_offsets, saved["params"])):
+        keys = [key for saved in saved_groups for key in saved["params"]]
+        for i, (p, o, key) in enumerate(zip(self._ordered, self._flat_offsets, keys)):
             st = state.get(key)
             if not st:
                 steps.add(0)
@@ -221,18 +341,22 @@ class _FlatAdamBase(torch.optim.Optimizer):
         if len(steps) != 1:
             raise ValueError(f"{type(self).__name__}.load_state_dict: the parameters have different step counts "
                              f"{sorted(steps)}; the flat kernel has one")
-        group = self.param_groups[0]
-        for k, v in saved.items():
-            if k in ("params", "capturable", "amsgrad", "maximize", "foreach", "differentiable", "fused",
-                     "decoupled_weight_decay"):             # ours, or torch.optim.Adam's switches
-                continue
-            if k == "lr":
-                self.lr = float(v)
-            elif k == "betas":
-                group[k] = (float(v[0]), float(v[1]))
-            else:
-                group[k] = v.clone() if isinstance(v, torch.Tensor) else v
-        group["max_grad_norm"] = saved.get("max_grad_norm")
+        for group, saved in zip(mine, saved_groups):
+            for k, v in saved.items():
+                if k in ("params", "capturable", "foreach", "differentiable", "fused") + _FALSE_KEYS:
+                    continue                             # ours, or torch.optim.Adam's switches
+                if k == "lr":
+                    if isinstance(group["lr"], torch.Tensor):
+                        group["lr"].fill_(float(v))
+                    else:
+                        group["lr"] = float(v)
+                elif k == "betas":
+                    group[k] = (float(v[0]), float(v[1]))
+                else:
+                    group[k] = v.clone() if isinstance(v, torch.Tensor) else v
+            group["decoupled_weight_decay"] = bool(saved.get("decoupled_weight_decay", False))
+            group["max_grad_norm"] = saved.get("max_grad_norm")
+        self._whole("max_grad_norm")
         self._scatter_state(exp_avg, exp_avg_sq)
         if self.capturable:
             self.step_state[0] = steps.pop()
@@ -246,8 +370,16 @@ class FlatAdam(_FlatAdamBase):
     p, g, m, v once, writes p, m, v and leaves the gradient zeroed for the next backward (main.py:171), folding the
     1/world of the data-parallel mean into the read.  Dense, same update rule and operation order as torch's Adam.
 
-    A torch.optim.Optimizer with one parameter group: the torch.optim.lr_scheduler classes drive `lr` (and OneCycleLR
-    `betas[0]`), and state_dict() / load_state_dict() interchange with torch.optim.Adam's.
+    A torch.optim.Optimizer: the torch.optim.lr_scheduler classes drive `lr` (and OneCycleLR `betas[0]`), and
+    state_dict() / load_state_dict() interchange with torch.optim.Adam's and torch.optim.AdamW's.
+
+    groups: None (one group of bucket.params) or torch's parameter-group dicts {"params": [...], "lr", "betas", "eps",
+    "weight_decay", "decoupled_weight_decay", "max_grad_norm"}, a missing key taking the constructor's value.  Their
+    parameters must be bucket.params, each once, in any grouping (the flat layout stays bucket.params' order, so groups
+    may interleave).  lr (a float, or a tensor with capturable=True), betas, eps, weight_decay and
+    decoupled_weight_decay are per group; max_grad_norm and capturable are for the whole optimizer.  All groups share
+    one step count, each group's bias corrections use its betas.  decoupled_weight_decay=True is torch.optim.AdamW's
+    rule: p *= 1 - lr * weight_decay before the moments.  Still one launch per step (c2v_adam_step_groups).
 
     capturable=True (torch.optim.Adam's flag): the step count lives on the device (`step_state`, see
     c2v_adam_step_capturable) and every step, eager or inside a CUDA graph, runs the capturable kernels; `t` is then not
@@ -263,23 +395,29 @@ class FlatAdam(_FlatAdamBase):
     as in torch.  `grad_norm` holds the last norm."""
 
     def __init__(self, bucket, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, capturable=False,
-                 max_grad_norm=None):
+                 max_grad_norm=None, decoupled_weight_decay=False, groups=None):
         self.bucket = bucket
-        self._init_optimizer(bucket.params, bucket.flat.device, lr, betas, eps, weight_decay, max_grad_norm, capturable)
+        self._init_optimizer(bucket.params if groups is None else groups, bucket.flat.device, lr, betas, eps, weight_decay,
+                             max_grad_norm, capturable, decoupled_weight_decay)
+        if {id(p) for p in self._ordered} != {id(p) for p in bucket.params} or len(self._ordered) != len(bucket.params):
+            raise ValueError("FlatAdam: the parameter groups must hold exactly the bucket's parameters, each once")
         flat = torch.empty_like(bucket.flat)
-        o, self._flat_offsets = 0, []
+        o, offsets = 0, []
         for p in bucket.params:                                  # same order as the gradient bucket
             n = p.numel()
             flat[o:o + n].copy_(p.data.reshape(-1))
             p.data = flat[o:o + n].view_as(p)
-            self._flat_offsets.append(o)
+            offsets.append(o)
             o += n
+        self._layout_groups(bucket.params, offsets)
+        at = {id(p): o for p, o in zip(bucket.params, offsets)}
+        self._flat_offsets = [at[id(p)] for p in self._ordered]
         self._flat_numel = o
         self.flat_param = flat
         self.exp_avg = torch.zeros_like(flat)
         self.exp_avg_sq = torch.zeros_like(flat)
         self.t = 0
-        self.step_state = _step_state(flat.device) if self.capturable else None
+        self.step_state = _step_state(flat.device, len(self.param_groups)) if self.capturable else None
 
     def step(self, grad_scale=1.0, zero_grad=True):
         _check_capturable(self.capturable, "FlatAdam")
@@ -303,9 +441,10 @@ class FlatAdam(_FlatAdamBase):
         self.exp_avg_sq.copy_(exp_avg_sq)
 
 
-def _step_state(device):
-    """the device step-state of c2v_adam_step_capturable: {int64 step; float step_size; float inv_sqrt_bc2}, step 0"""
-    return torch.zeros(2, dtype=torch.int64, device=device)
+def _step_state(device, n_groups):
+    """the device step-state, step 0: {int64 step; float s[3 * n_groups]} (c2v_adam_step_groups), which begins with the
+    one of c2v_adam_step_capturable, {int64 step; float step_size; float inv_sqrt_bc2}"""
+    return torch.zeros(1 + (3 * n_groups + 1) // 2, dtype=torch.int64, device=device)
 
 
 def _check_capturable(capturable, name):
@@ -372,8 +511,10 @@ class ShardedFlatAdam(_FlatAdamBase):
               symmetric memory is unavailable, and what the gloo CPU tests drive with a stand-in kernel).
       "auto"  nvls or p2p, whichever is faster on this group (timed at construction), else nccl.
 
-    A torch.optim.Optimizer with one parameter group, like FlatAdam: lr schedulers, and state_dict() /
-    load_state_dict() in torch.optim.Adam's format.  At world size > 1 state_dict() is a collective (it all-gathers the
+    A torch.optim.Optimizer like FlatAdam: parameter groups (`params` in torch's forms: parameters or group dicts, a
+    missing key taking the constructor's value), lr schedulers, and state_dict() / load_state_dict() in
+    torch.optim.Adam's / AdamW's format.  The flat order is the groups' parameters in order, the early ones first; with
+    more than one group every parameter starts at a multiple of 4 elements.  At world size > 1 state_dict() is a collective (it all-gathers the
     owned slices) that returns the full dict on every rank, and load_state_dict() keeps this rank's slices of the full
     dict: a checkpoint saved at one world size loads at another.  At world size 1 a tensor `lr` (capturable=True) and
     `max_grad_norm` work as in FlatAdam.  max_grad_norm at world size > 1 raises NotImplementedError: the fused kernel
@@ -382,8 +523,14 @@ class ShardedFlatAdam(_FlatAdamBase):
     """
 
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, group=None, transport="auto",
-                 early=(), capturable=False, max_grad_norm=None):
-        params = [p for p in params if p.requires_grad]
+                 early=(), capturable=False, max_grad_norm=None, decoupled_weight_decay=False):
+        params = list(params)
+        if params and isinstance(params[0], dict):               # parameter groups: their trainable parameters
+            groups = [dict(g, params=[p for p in ([g["params"]] if isinstance(g["params"], torch.Tensor) else g["params"])
+                                      if p.requires_grad]) for g in params]
+            params = [p for g in groups for p in g["params"]]
+        else:
+            params = groups = [p for p in params if p.requires_grad]
         if not params:
             raise ValueError("no trainable parameters")
         early_ids = {id(p) for p in early}
@@ -402,12 +549,17 @@ class ShardedFlatAdam(_FlatAdamBase):
         dev, dt = self.params[0].device, self.params[0].dtype
         if dt != torch.float32:
             raise TypeError("parameters must be fp32")
-        self._init_optimizer(params, dev, lr, betas, eps, weight_decay, max_grad_norm, capturable)
+        self._init_optimizer(groups, dev, lr, betas, eps, weight_decay, max_grad_norm, capturable, decoupled_weight_decay)
         self.numel = sum(p.numel() for p in self.params)
-        n_early = sum(p.numel() for p in first)
+        # with several groups the flat order is the groups', and a parameter whose size is not a multiple of 4 (the
+        # output bias at C = 195,299) may come before an embedding table, which the model's kernels read 16 bytes at a
+        # time: there every parameter starts at a multiple of 4 elements (the gaps are zero and stay zero)
+        span = (lambda p: (p.numel() + 3) // 4 * 4) if len(self.param_groups) > 1 else (lambda p: p.numel())
+        n_early = sum(span(p) for p in first)
         # regions: (begin, length) in the flat buffers; region 0 = the early parameters (absent when there are none);
         # this rank's slice of every region, and where its optimizer state sits in exp_avg / exp_avg_sq
-        self.regions, self.slices, self.state_numel = sharded_layout(n_early, self.numel, self.world, self.rank)
+        self.regions, self.slices, self.state_numel = sharded_layout(n_early, sum(span(p) for p in self.params),
+                                                                     self.world, self.rank)
         self.padded = sum(n for _, n in self.regions)
         self._auto = transport == "auto"
         self._auto_nvls = nvls_allowed(transport, self.world)
@@ -422,9 +574,10 @@ class ShardedFlatAdam(_FlatAdamBase):
             if n_early and i == len(first):
                 o = self.regions[1][0]                           # region 1 starts after region 0's padding
             pos[i] = o
-            o += p.numel()
+            o += span(p)
         flat_pos = {id(p): pos[i] for i, p in enumerate(self.params)}
-        self._flat_offsets = [flat_pos[id(p)] for p in params]      # in the caller's order, which state_dict() keeps
+        self._flat_offsets = [flat_pos[id(p)] for p in self._ordered]      # in the caller's order, which state_dict() keeps
+        self._layout_groups(self.params, [pos[i] for i in range(len(self.params))])
         self._flat_numel = self.padded
         for i, p in enumerate(self.params):
             n, o = p.numel(), pos[i]
@@ -435,7 +588,7 @@ class ShardedFlatAdam(_FlatAdamBase):
         self.exp_avg = torch.zeros(self.state_numel, dtype=dt, device=dev)
         self.exp_avg_sq = torch.zeros(self.state_numel, dtype=dt, device=dev)
         self.t, self.cur = 0, 0
-        self.step_state = _step_state(dev) if self.capturable else None
+        self.step_state = _step_state(dev, len(self.param_groups)) if self.capturable else None
         self._early_done = False
         self._side = torch.cuda.Stream(dev) if (dev.type == "cuda" and len(self.regions) > 1) else None
         self._point_grads(0)
@@ -451,8 +604,9 @@ class ShardedFlatAdam(_FlatAdamBase):
         number of GPUs and the fabric."""
         dev = self.flat_param.device
         res = {}
-        saved = (self.lr, self.weight_decay)
-        self.lr, self.weight_decay = 0.0, 0.0
+        saved = [(g["lr"], g["weight_decay"]) for g in self.param_groups]
+        for g in self.param_groups:
+            g["lr"], g["weight_decay"] = 0.0, 0.0
         try:
             for tr in ("nvls", "p2p"):
                 self.transport = tr
@@ -469,7 +623,8 @@ class ShardedFlatAdam(_FlatAdamBase):
                 dist.all_reduce(t, op=dist.ReduceOp.MAX, group=self.group)
                 res[tr] = float(t.item())
         finally:
-            self.lr, self.weight_decay = saved
+            for g, (lr, wd) in zip(self.param_groups, saved):
+                g["lr"], g["weight_decay"] = lr, wd
             self.t = 0
         self.transport = min(res, key=res.get)
         self.calibration = res
@@ -538,7 +693,8 @@ class ShardedFlatAdam(_FlatAdamBase):
     def _adam_slice(self, p_slice, g_slice, zero_grad=False, state=None):
         """the flat step on an owned slice (the gloo CPU tests replace this method with a torch stand-in)"""
         m, v = state if state is not None else (self.exp_avg, self.exp_avg_sq)
-        self._launch(p_slice, g_slice, m, v, self.t, 1.0 / self.world, zero_grad)
+        lo = (p_slice.data_ptr() - self.flat_param.data_ptr()) // p_slice.element_size()   # where the slice begins
+        self._launch(p_slice, g_slice, m, v, self.t, 1.0 / self.world, zero_grad, lo=lo)
 
     def _reduce_scatter(self, out, full):
         try:
@@ -563,10 +719,17 @@ class ShardedFlatAdam(_FlatAdamBase):
         lo, n, so = self.slices[r]
         with torch.cuda.device(dev):
             hg.barrier(channel=2 * r)
-            rc = lib.c2v_adam_step_sharded_bulk(
-                V(self.flat_param.data_ptr()), pp, gp, self.world, V(self.exp_avg.data_ptr() + 4 * so),
-                V(self.exp_avg_sq.data_ptr() + 4 * so), lo, n, self.lr, self.betas[0], self.betas[1], self.eps,
-                self.weight_decay, self.t, 1.0 / self.world, 0, V(torch.cuda.current_stream(dev).cuda_stream))
+            stream = V(torch.cuda.current_stream(dev).cuda_stream)
+            if self._grouped():
+                rc = lib.c2v_adam_step_sharded_bulk_groups(
+                    V(self.flat_param.data_ptr()), pp, gp, self.world, V(self.exp_avg.data_ptr() + 4 * so),
+                    V(self.exp_avg_sq.data_ptr() + 4 * so), lo, n, *self._group_table(), self.t, 1.0 / self.world, 0,
+                    stream)
+            else:
+                rc = lib.c2v_adam_step_sharded_bulk(
+                    V(self.flat_param.data_ptr()), pp, gp, self.world, V(self.exp_avg.data_ptr() + 4 * so),
+                    V(self.exp_avg_sq.data_ptr() + 4 * so), lo, n, self.lr, self.betas[0], self.betas[1], self.eps,
+                    self.weight_decay, self.t, 1.0 / self.world, 0, stream)
             _lib.check(rc, "c2v_adam_step_sharded_bulk")
             hp.barrier(channel=2 * r + 1)
 
@@ -585,12 +748,15 @@ class ShardedFlatAdam(_FlatAdamBase):
         rb, rn = (0, self.padded) if zero_all else self.regions[r]     # which part of the OTHER bucket this launch zero-fills
         with torch.cuda.device(dev):
             hg.barrier(channel=2 * r)                        # every rank's backward has finished writing this region
-            rc = lib.c2v_adam_step_sharded(
-                V(self.flat_param.data_ptr()), V(int(hp.multicast_ptr)) if use_mc else None,
-                V(int(hg.multicast_ptr)) if use_mc else None, pp, gp, self.world, V(self.exp_avg.data_ptr() + 4 * so),
-                V(self.exp_avg_sq.data_ptr() + 4 * so), lo, n, V(self.buckets[nxt].data_ptr() + 4 * rb), rn, self.lr,
-                self.betas[0], self.betas[1], self.eps, self.weight_decay, self.t, 1.0 / self.world,
-                V(torch.cuda.current_stream(dev).cuda_stream))
+            head = (V(self.flat_param.data_ptr()), V(int(hp.multicast_ptr)) if use_mc else None,
+                    V(int(hg.multicast_ptr)) if use_mc else None, pp, gp, self.world, V(self.exp_avg.data_ptr() + 4 * so),
+                    V(self.exp_avg_sq.data_ptr() + 4 * so), lo, n, V(self.buckets[nxt].data_ptr() + 4 * rb), rn)
+            stream = V(torch.cuda.current_stream(dev).cuda_stream)
+            if self._grouped():
+                rc = lib.c2v_adam_step_sharded_groups(*head, *self._group_table(), self.t, 1.0 / self.world, stream)
+            else:
+                rc = lib.c2v_adam_step_sharded(*head, self.lr, self.betas[0], self.betas[1], self.eps, self.weight_decay,
+                                               self.t, 1.0 / self.world, stream)
             _lib.check(rc, "c2v_adam_step_sharded")
             hp.barrier(channel=2 * r + 1)                    # every rank's parameter stores of this region have landed here
 

@@ -112,8 +112,10 @@ class GraphedTrainStep(_Graphed):
     def _settings(self):
         o = self.optimizer
         if isinstance(o, (FlatAdam, ShardedFlatAdam)):
-            # a tensor lr is read on the device at every replay (a scheduler fills it); the rest are launch parameters
-            hyper = (None if isinstance(o.lr, torch.Tensor) else o.lr, o.betas, o.eps, o.weight_decay, o.max_grad_norm)
+            # per group: a tensor lr is read on the device at every replay (a scheduler fills it); the rest are launch
+            # parameters
+            hyper = tuple((None if isinstance(g["lr"], torch.Tensor) else g["lr"], g["betas"], g["eps"], g["weight_decay"],
+                           g["decoupled_weight_decay"], g["max_grad_norm"]) for g in o.param_groups)
         else:
             hyper = tuple(tuple((k, v) for k, v in sorted(g.items()) if k != "params" and not isinstance(v, torch.Tensor))
                           for g in o.param_groups)

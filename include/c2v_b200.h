@@ -740,6 +740,49 @@ int c2v_adam_step_sharded_bulk(const float *param_local, float *const *param_pee
                                int64_t slice_n, float lr, float beta1, float beta2, float eps, float weight_decay,
                                int64_t step, float grad_scale, int32_t max_ctas, void *stream);
 
+/* Parameter groups (torch.optim.Adam's param_groups) for the three flat steps above, still one launch per call:
+ * groups[k] holds group k's hyper-parameters; decoupled != 0 is AdamW (torch.optim.Adam(decoupled_weight_decay=True)):
+ * param *= 1 - lr * weight_decay before the moments, the gradient without weight decay.  lr_dev (fp32 device scalar,
+ * 4-byte aligned, or NULL) is read instead of lr by the step-count kernel, so it needs step_state.  The flat buffers are
+ * divided into segments, maximal runs of one group: segment s begins at flat element seg_begin[s] (seg_begin[0] = 0,
+ * strictly ascending) and belongs to group seg_group[s] (in [0, n_groups)); the last segment reaches to the end.  A
+ * segment may begin at any element.  1 <= n_groups <= C2V_ADAM_MAX_GROUPS and 1 <= n_segments <= C2V_ADAM_MAX_SEGMENTS,
+ * otherwise C2V_EINVAL before any CUDA call.  The table is passed to the kernel by value (no device buffer: capturable).
+ * The bias corrections of group k use its betas and the one shared step count.  grad_scale, zero_grad and coef_dev are
+ * c2v_adam_step_ex's and apply to every group. */
+#define C2V_ADAM_MAX_GROUPS 16
+#define C2V_ADAM_MAX_SEGMENTS 64
+typedef struct c2v_adam_group {
+    float lr, beta1, beta2, eps, weight_decay;
+    int32_t decoupled;
+    const float *lr_dev;
+} c2v_adam_group;
+
+/* c2v_adam_step_ex with parameter groups.  step_state NULL: `step` is the 1-based step count.  step_state not NULL: the
+ * step count lives on the device, (8 + 12 * n_groups) bytes, 8-byte aligned: {int64 step; float s[3 * n_groups]}; a
+ * single-thread kernel increments step, then stores per group s[3k] = lr / (1 - beta1^step),
+ * s[3k + 1] = 1 / sqrt(1 - beta2^step) (in double, as c2v_adam_step_capturable) and s[3k + 2] = 1 - lr * weight_decay
+ * for a decoupled group, 1 otherwise; the update kernel reads them.  step starts at 0 and counts as in
+ * c2v_adam_step_capturable's 16-byte state. */
+int c2v_adam_step_groups(float *param, float *grad, float *exp_avg, float *exp_avg_sq, int64_t n,
+                         const c2v_adam_group *groups, int32_t n_groups, const int64_t *seg_begin,
+                         const int32_t *seg_group, int32_t n_segments, int64_t step, void *step_state, float grad_scale,
+                         int32_t zero_grad, const float *coef_dev, void *stream);
+/* c2v_adam_step_sharded and c2v_adam_step_sharded_bulk with parameter groups.  seg_begin is in flat-buffer
+ * coordinates, like slice_begin: a slice may begin inside a segment.  Host step counts only (lr_dev must be NULL). */
+int c2v_adam_step_sharded_groups(const float *param_local, float *param_multicast, const float *grad_multicast,
+                                 float *const *param_peers, const float *const *grad_peers, int32_t world,
+                                 float *exp_avg_slice, float *exp_avg_sq_slice, int64_t slice_begin, int64_t slice_n,
+                                 float *zero_buffer, int64_t zero_n, const c2v_adam_group *groups, int32_t n_groups,
+                                 const int64_t *seg_begin, const int32_t *seg_group, int32_t n_segments, int64_t step,
+                                 float grad_scale, void *stream);
+int c2v_adam_step_sharded_bulk_groups(const float *param_local, float *const *param_peers,
+                                      const float *const *grad_peers, int32_t world, float *exp_avg_slice,
+                                      float *exp_avg_sq_slice, int64_t slice_begin, int64_t slice_n,
+                                      const c2v_adam_group *groups, int32_t n_groups, const int64_t *seg_begin,
+                                      const int32_t *seg_group, int32_t n_segments, int64_t step, float grad_scale,
+                                      int32_t max_ctas, void *stream);
+
 /* ---- corpus reader / code-vector writer: the data formats either side of the path ----------
  * c2v_corpus_parse_*: DatasetReader.load (/root/reference/model/dataset_reader.py:72-128) for the `corpus.txt` format
  * (`#id`, `label:`, `class:`, `paths:` + `start\tpath\tend` lines, `vars:` + `original\talias` lines, blank line between
