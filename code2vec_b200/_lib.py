@@ -15,6 +15,7 @@ ABI_VERSION = 1
 TOPK_MAX = 16                # C2V_TOPK_MAX: the largest k of the fused top-k (c2v_label_topk / c2v_angular_topk)
 KNN_EXCLUDE_MAX = 4          # C2V_KNN_EXCLUDE_MAX: excluded bank rows per query of c2v_knn_topk / c2v_knn_pairs
 KNN_MAX_Q = 2048             # queries per c2v_knn_* call
+SAMPLED_MAX = 65536          # C2V_SAMPLED_MAX: the most candidates of one sampled-softmax step
 DROPOUT_SEED_ON_DEVICE = 2   # C2V_DROPOUT_SEED_ON_DEVICE: c2v_dropout.seed is the device address of the key
 MATMUL_IEEE, MATMUL_TF32 = 0, 1   # C2V_MATMUL_*: modes of c2v_set_matmul_precision
 # c2v_eval_accumulate's counters (C2V_EVAL_*): n, skipped, k rank hits, then tp, fp, fn and the fixed-point sums
@@ -192,6 +193,12 @@ SYMBOLS = {
     "c2v_sparse_adam_step_merged": (ctypes.c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_i64, c_vp, c_vp, c_i64, c_i32,
                                                    c_f32, ctypes.c_double, ctypes.c_double, ctypes.c_double,
                                                    ctypes.c_double, c_i64, c_vp]),
+    "c2v_sampled_candidates": (ctypes.c_int, [c_vp, c_i64, c_i32, ctypes.c_uint64, c_vp, c_vp, c_vp]),
+    "c2v_sampled_gather": (ctypes.c_int, [c_vp, c_vp, c_vp, c_i64, c_i32, c_vp, c_i32, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp]),
+    "c2v_sampled_loss": (ctypes.c_int, [c_vp, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp]),
+    "c2v_sampled_dlogits": (ctypes.c_int, [c_vp, c_vp, c_vp, c_i32, c_i32, c_f32, c_vp, c_vp]),
+    "c2v_scatter_rows_add_workspace_bytes": (c_sz, [c_i64]),
+    "c2v_scatter_rows_add": (ctypes.c_int, [c_vp, c_i64, c_vp, c_vp, c_i32, c_i64, c_vp, c_vp, c_vp, c_sz, c_vp]),
     "c2v_session_create": (ctypes.c_int, [ctypes.c_int, _P(Dims), c_i32, c_i32, _P(c_vp)]),
     "c2v_session_destroy": (None, [c_vp]),
     "c2v_forward_host": (ctypes.c_int, [c_vp, _P(Params), c_vp, c_vp, c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp,

@@ -12,7 +12,7 @@ OUT = os.environ.get("C2V_LIB_OUT", os.path.join(HERE, "libc2v_b200.so"))   # ex
 EXTRA = os.environ.get("C2V_NVCC_EXTRA", "").split()
 SOURCES = ["c2v_api.cu", "c2v_session.cu", "c2v_encode_ffma.cu", "c2v_encode_wgmma.cu", "c2v_label_tcgen05.cu", "c2v_label_backward_tc.cu", "c2v_head.cu",
            "c2v_backward.cu", "c2v_backward_dw_tc.cu", "c2v_backward_dc_tc.cu", "c2v_batch.cu", "c2v_adam.cu", "c2v_sparse.cu",
-           "c2v_deterministic.cu", "c2v_eval.cu", "c2v_corpus.cpp"]
+           "c2v_deterministic.cu", "c2v_eval.cu", "c2v_sampled.cu", "c2v_corpus.cpp"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
          "-Xcompiler", "-fPIC", "-Xcompiler", "-Wall", "--expt-relaxed-constexpr"]

@@ -809,17 +809,23 @@ class ShardedFlatAdam(_FlatAdamBase):
             torch.autograd.graph.increment_version(p)
 
 
-def _forward_loss(model, starts, paths, ends, label, criterion):
+def _forward_loss(model, starts, paths, ends, label, criterion, sampler=None):
     # criterion None: the call without it, for any forward_loss of the (starts, paths, ends, label) form
+    if sampler is not None:
+        return model.forward_sampled_loss(starts, paths, ends, label, sampler)[0]
     if criterion is None:
         return model.forward_loss(starts, paths, ends, label)[0]
     return model.forward_loss(starts, paths, ends, label, criterion=criterion)[0]
 
 
-def ddp_step(model, optimizer, bucket, starts, paths, ends, label, loss_fn, criterion=None):
+def ddp_step(model, optimizer, bucket, starts, paths, ends, label, loss_fn, criterion=None, sampler=None):
     """One training step of main.py:171-175 on this rank's shard of the global batch.  loss_fn None: the fused loss of
     Code2Vec.forward_loss with `criterion` (None, nn.NLLLoss or nn.CrossEntropyLoss; a mean is this rank's own, as with
-    DDP); else forward() and loss_fn(outputs, label)."""
+    DDP); else forward() and loss_fn(outputs, label).  sampler (a functional.SampledSoftmax): the step's loss is
+    Code2Vec.forward_sampled_loss(...)[0] instead, its candidates drawn from this rank's own generator; it takes neither
+    loss_fn nor criterion (ValueError)."""
+    if sampler is not None and (loss_fn is not None or criterion is not None):
+        raise ValueError("ddp_step: sampler= replaces the loss; pass loss_fn=None and no criterion with it")
     if isinstance(optimizer, (ShardedFlatAdam, FlatAdam)) and hasattr(model, "fuse_grad_accumulation"):
         model.fuse_grad_accumulation = True                  # .grad are persistent views into a flat bucket: accumulate in place
         if isinstance(optimizer, ShardedFlatAdam) and len(optimizer.regions) > 1 and optimizer.world > 1 and \
@@ -827,7 +833,7 @@ def ddp_step(model, optimizer, bucket, starts, paths, ends, label, loss_fn, crit
             model.on_path_grads_ready = optimizer.early_step # region 0 is reduced while the backward is still running
     if isinstance(optimizer, ShardedFlatAdam):               # reduction + optimizer + broadcast are one kernel per rank
         if loss_fn is None:                                  # fused loss: the [b, C] logits are never written
-            loss = _forward_loss(model, starts, paths, ends, label, criterion)
+            loss = _forward_loss(model, starts, paths, ends, label, criterion, sampler)
         else:
             outputs, code_vector, attention = model.forward(starts, paths, ends, label)
             loss = loss_fn(outputs, label)
@@ -838,7 +844,7 @@ def ddp_step(model, optimizer, bucket, starts, paths, ends, label, loss_fn, crit
     if not fused:
         bucket.zero()                       # (FlatAdam leaves the bucket zeroed at the end of its step)
     if loss_fn is None:                     # fused loss (Code2Vec.forward_loss)
-        loss = _forward_loss(model, starts, paths, ends, label, criterion)
+        loss = _forward_loss(model, starts, paths, ends, label, criterion, sampler)
     else:
         outputs, code_vector, attention = model.forward(starts, paths, ends, label)
         loss = loss_fn(outputs, label)

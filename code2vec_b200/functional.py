@@ -943,3 +943,150 @@ def sparse_adam_step_merged(param, exp_avg, exp_avg_sq, values, rows, counts, un
             _ptr(counts), world, u_max, _ptr(union_rows) if union_rows.numel() else None, _ptr(union_count), n, E,
             float(scale), float(lr), float(beta1), float(beta2), float(eps), int(step), _stream(dev))
         _lib.check(rc, "c2v_sparse_adam_step_merged")
+
+
+class SampledSoftmax:
+    """The proposal distribution of a sampled-softmax loss (Code2Vec.forward_sampled_loss) over `label_count` labels:
+    q(c) = counts[c]^power / sum_k counts[k]^power, uniform when counts is None.  Every step draws num_sampled candidates
+    i.i.d. with replacement from q.  The usual counts are the training set's label frequencies
+    (Vocab.get_freq_list()); pass counts + 1 when some label never occurs, since the true label's correction log q needs
+    q > 0.
+
+    The fp64 CDF (numpy.cumsum of the weights over their total) and log q [label_count] are built once on the host and
+    uploaded to each device on its first use.  ValueError: label_count < 1, num_sampled outside [1, 65536], counts not
+    1-D of length label_count or with a non-finite or non-positive entry, power not finite and > 0."""
+
+    def __init__(self, label_count, num_sampled, counts=None, power=1.0):
+        import math
+        import numpy as np
+        C, S, power = int(label_count), int(num_sampled), float(power)
+        if C < 1:
+            raise ValueError(f"SampledSoftmax: label_count = {C} < 1")
+        if not 1 <= S <= _lib.SAMPLED_MAX:
+            raise ValueError(f"SampledSoftmax: num_sampled = {S} outside [1, {_lib.SAMPLED_MAX}]")
+        if not (math.isfinite(power) and power > 0):
+            raise ValueError(f"SampledSoftmax: power = {power} must be finite and > 0")
+        if counts is None:
+            w = np.ones(C, dtype=np.float64)
+        else:
+            if isinstance(counts, torch.Tensor):
+                counts = counts.detach().cpu().numpy()
+            n = np.asarray(counts, dtype=np.float64)
+            if n.ndim != 1 or n.shape[0] != C:
+                raise ValueError(f"SampledSoftmax: counts must be 1-D of length label_count = {C}, got shape {n.shape}")
+            if not (np.isfinite(n).all() and (n > 0).all()):
+                raise ValueError("SampledSoftmax: every count must be finite and > 0 (pass counts + 1 when some label "
+                                 "never occurs)")
+            with np.errstate(over="ignore", under="ignore"):
+                w = n ** power
+            if not (np.isfinite(w).all() and (w > 0).all()):
+                raise ValueError(f"SampledSoftmax: counts ** {power} leaves the finite positive fp64 range")
+        cdf = np.cumsum(w)
+        total = cdf[-1]
+        if not math.isfinite(total):
+            raise ValueError("SampledSoftmax: the sum of counts ** power is not finite in fp64")
+        self.label_count, self.num_sampled, self.power = C, S, power
+        self.cdf_host = cdf / total                  # cdf_host[-1] == 1 exactly
+        self.log_q_host = np.log(w) - np.log(total)
+        self._dev = {}
+
+    def device_tables(self, device):
+        """-> (cdf fp64 [C], log_q fp64 [C]) on `device`, uploaded on its first use there"""
+        device = torch.device(device)
+        if device.type == "cuda" and device.index is None:
+            device = torch.device("cuda", torch.cuda.current_device())
+        t = self._dev.get(device)
+        if t is None:
+            if capturing():
+                raise RuntimeError("SampledSoftmax: the proposal tables would be uploaded under CUDA-graph capture: run "
+                                   "one step eagerly on this device first")
+            t = (torch.from_numpy(self.cdf_host).to(device), torch.from_numpy(self.log_q_host).to(device))
+            self._dev[device] = t
+        return t
+
+    def sample(self, key, device=None):
+        """-> int64 [num_sampled] candidate ids drawn from q with Philox key `key` (c2v_sampled_candidates): an int, or an
+        int64 [1] CUDA tensor holding it (read on the device when the kernel runs).  device: where to draw (the key
+        tensor's device, else the current CUDA device)."""
+        lib = _lib.load()
+        key_dev = key if isinstance(key, torch.Tensor) else None
+        if key_dev is not None:
+            _need_cuda(key_dev)
+            if key_dev.dtype != torch.int64 or key_dev.numel() != 1:
+                raise TypeError("SampledSoftmax.sample: a key tensor must be int64 with one element")
+            device = key_dev.device
+        elif device is None:
+            device = torch.device("cuda", torch.cuda.current_device())
+        cdf, _ = self.device_tables(device)
+        with torch.cuda.device(cdf.device):
+            out = _empty((self.num_sampled,), torch.int64, cdf.device)
+            k = 0 if key_dev is not None else int(key) & 0xFFFFFFFFFFFFFFFF
+            rc = lib.c2v_sampled_candidates(_ptr(cdf), self.label_count, self.num_sampled, k, _ptr(key_dev), _ptr(out),
+                                            _stream(cdf.device))
+            _lib.check(rc, "c2v_sampled_candidates")
+        return out
+
+
+def sampled_gather(w_out, b_out, log_q, candidates, label):
+    """-> (ids int64 [S + B], w_hat [S + B, H], b_hat [S + B]) of the compact head (c2v_sampled_gather)"""
+    lib = _lib.load()
+    _need_cuda(w_out, b_out, log_q, candidates, label)
+    C, H = w_out.shape
+    S, B = candidates.numel(), label.numel()
+    dev = w_out.device
+    w_out, b_out = _f32c(w_out, "output_weight"), _f32c(b_out, "output_bias")
+    candidates, label = _idx(candidates, "candidates"), _idx(label, "label")
+    with torch.cuda.device(dev):
+        ids = _empty((S + B,), torch.int64, dev)
+        w_hat = _empty((S + B, H), torch.float32, dev)
+        b_hat = _empty((S + B,), torch.float32, dev)
+        rc = lib.c2v_sampled_gather(_ptr(w_out), _ptr(b_out), _ptr(log_q), C, H, _ptr(candidates), S, _ptr(label), B,
+                                    _ptr(w_hat), _ptr(b_hat), _ptr(ids), _stream(dev))
+        _lib.check(rc, "c2v_sampled_gather")
+    return ids, w_hat, b_hat
+
+
+def sampled_loss(logits, ids, S):
+    """-> (loss 0-d, lse [B]) of the compact logits [B, S + B] (c2v_sampled_loss)"""
+    lib = _lib.load()
+    B = logits.shape[0]
+    dev = logits.device
+    with torch.cuda.device(dev):
+        lse = _empty((B,), torch.float32, dev)
+        loss = _empty((), torch.float32, dev)
+        rc = lib.c2v_sampled_loss(_ptr(logits), _ptr(ids), int(S), B, _ptr(lse), _ptr(loss), _stream(dev))
+        _lib.check(rc, "c2v_sampled_loss")
+    return loss, lse
+
+
+def sampled_dlogits_(logits, ids, lse, S, scale, scale_device=None):
+    """overwrites the compact logits [B, S + B] with d loss / d logits (c2v_sampled_dlogits); returns them"""
+    lib = _lib.load()
+    B = logits.shape[0]
+    dev = logits.device
+    sd = _f32c(scale_device, "scale_device") if scale_device is not None else None
+    with torch.cuda.device(dev):
+        rc = lib.c2v_sampled_dlogits(_ptr(logits), _ptr(ids), _ptr(lse), int(S), B, float(scale), _ptr(sd), _stream(dev))
+        _lib.check(rc, "c2v_sampled_dlogits")
+    return logits
+
+
+def scatter_rows_add(ids, rows, bias, dst, dst_bias):
+    """dst[ids[e]] += rows[e] and dst_bias[ids[e]] += bias[e] in a fixed order (c2v_scatter_rows_add); either pair may
+    be None"""
+    lib = _lib.load()
+    n = ids.numel()
+    ref = dst if dst is not None else dst_bias
+    C = ref.shape[0]
+    H = dst.shape[1] if dst is not None else 1
+    dev = ref.device
+    rows = _f32c(rows, "rows") if rows is not None else None
+    bias = _f32c(bias, "bias") if bias is not None else None
+    nbytes = lib.c2v_scatter_rows_add_workspace_bytes(n)
+    if nbytes == 0:
+        raise ValueError(f"scatter_rows_add: {n} ids outside [1, 2^31)")
+    with torch.cuda.device(dev):
+        ws = _empty((nbytes,), torch.uint8, dev)
+        rc = lib.c2v_scatter_rows_add(_ptr(ids), n, _ptr(rows), _ptr(bias), H, C, _ptr(dst), _ptr(dst_bias), _ptr(ws),
+                                      nbytes, _stream(dev))
+        _lib.check(rc, "c2v_scatter_rows_add")

@@ -250,6 +250,48 @@ class _LabelLossOptsFn(torch.autograd.Function):
         return d_cv, d_w, d_b, None, None, None, None, None, None
 
 
+class _SampledLossFn(torch.autograd.Function):
+    """sampled softmax over the plain head (functional.SampledSoftmax): the label head's own GEMM and backward run on the
+    compact head W_out[ids], b_out[ids] - log(S q(ids)) with ids = (candidates, label), whose [B, S + B] logits hold every
+    logit the loss needs; the gradients of the S + B compact rows are added into dense [C, H] / [C] gradients in a fixed
+    order.  The compact logits are kept for the backward, which overwrites them with d loss / d logits."""
+
+    @staticmethod
+    def forward(ctx, cv, w_out, b_out, label, candidates, sampler, algo):
+        S, B, H = candidates.numel(), cv.shape[0], w_out.shape[1]
+        if any(ctx.needs_input_grad[:3]):
+            algo = int(algo) | CF.NO_PDL            # the calls that feed autograd use plain stream-ordered launches
+        _, log_q = sampler.device_tables(cv.device)
+        ids, w_hat, b_hat = CF.sampled_gather(w_out, b_out, log_q, candidates, label)
+        # a workspace of this call's own: the module's label cache trusts W_out's version counter and would reuse the full
+        # head's image; this one holds w_hat's image from the forward's GEMM to the backward's
+        cache = CF.PrepCache()
+        dims = CF.make_dims(1, 1, S + B, H, H, H)
+        logits = CF.label_logits(dims, CF.make_params(w_out=w_hat, b_out=b_hat), cv, algo, cache=cache, weight=w_hat)
+        loss, lse = CF.sampled_loss(logits, ids, S)
+        ctx.save_for_backward(cv, w_hat, ids, lse)
+        ctx.logits, ctx.cfg = logits, (dims, cache, int(algo) & 0xff, S, w_out.shape[0])
+        return loss
+
+    @staticmethod
+    def backward(ctx, d_loss):
+        cv, w_hat, ids, lse = ctx.saved_tensors
+        dims, cache, algo, S, C = ctx.cfg
+        if ctx.logits is None:
+            raise RuntimeError("forward_sampled_loss: the backward overwrites the compact logits and runs once per forward "
+                               "(retain_graph=True is not supported)")
+        g = CF.sampled_dlogits_(ctx.logits, ids, lse, S, 1.0 / cv.shape[0], d_loss.reshape(1))
+        ctx.logits = None
+        need = ctx.needs_input_grad
+        d_cv, dw_hat, db_hat = CF.label_backward(dims, CF.make_params(w_out=w_hat), cv, g, need[0], need[1], need[2],
+                                                 algo=algo, cache=cache, weight=w_hat)
+        d_w = torch.zeros((C, cv.shape[1]), dtype=torch.float32, device=cv.device) if need[1] else None
+        d_b = torch.zeros((C,), dtype=torch.float32, device=cv.device) if need[2] else None
+        if need[1] or need[2]:
+            CF.scatter_rows_add(ids, dw_hat, db_hat, d_w, d_b)
+        return d_cv, d_w, d_b, None, None, None, None
+
+
 class _LossArgmaxOptsFn(torch.autograd.Function):
     """_LossArgmaxFn with a criterion (c2v_loss_argmax_opts): the loss is summed in a fixed order"""
 
@@ -517,6 +559,51 @@ class Code2Vec(nn.Module):
             loss = criterion(F.log_softmax(outputs, dim=1) if type(criterion) is nn.NLLLoss else outputs, label)
             mx, am = torch.max(outputs.detach(), dim=1)
         return loss, am, mx, code_vector, attention
+
+    def forward_sampled_loss(self, starts, paths, ends, label, sampler, candidates=None):
+        """-> (loss, code_vector [b,H], attention [b,L]): the sampled-softmax training loss of the plain head
+        (Jean et al. 2015; TensorFlow's sampled_softmax_loss with num_true=1, remove_accidental_hits=True and
+        subtract_log_q=True).  With S = sampler.num_sampled candidates s_j drawn i.i.d. from sampler's q:
+            z_i+ = cv_i . w_{y_i} + b_{y_i} - log(S q(y_i)),   z_ij = cv_i . w_{s_j} + b_{s_j} - log(S q(s_j))
+            loss = mean_i [ log(exp z_i+ + sum_{j: s_j != y_i} exp z_ij) - z_i+ ]
+        loss is autograd-connected: its gradients are exact for the drawn candidates and reach W_out / b_out (rows that
+        are neither a candidate nor a label of the batch get exactly 0; a candidate drawn twice counts twice), the code
+        vectors and every encoder parameter.  Train with it, evaluate with forward_loss() / metrics.Evaluator: the
+        parameters are those of the full head.
+        The candidates are drawn with a key taken as the training forward takes its dropout key (torch's CPU generator,
+        or the device key stream after use_device_rng()), so torch.manual_seed keeps runs repeatable; candidates= (int64
+        [S'] on the model's device, 1 <= S' <= 65536) replaces the draw, with q still from sampler.  A label outside
+        [0, label_count) makes the loss NaN, as in forward_loss.  Nothing is read back to the host.
+        NotImplementedError with option.angular_margin_loss; ValueError if sampler.label_count != option.label_count."""
+        if self.option.angular_margin_loss:
+            raise NotImplementedError("forward_sampled_loss: the angular-margin head has no sampled loss; use forward_loss")
+        if not isinstance(sampler, CF.SampledSoftmax):
+            raise TypeError(f"forward_sampled_loss: sampler must be a functional.SampledSoftmax, got {type(sampler).__name__}")
+        if sampler.label_count != self.option.label_count:
+            raise ValueError(f"forward_sampled_loss: the sampler covers {sampler.label_count} labels, the model "
+                             f"{self.option.label_count}")
+        code_vector, attention, dims = self._encode(starts, paths, ends)
+        dev = code_vector.device
+        label = CF._idx(label, "label", (code_vector.shape[0],))
+        if candidates is None:
+            if self._rng_base is not None:
+                key = self._next_device_key(dev)
+            else:
+                if CF.capturing():
+                    raise RuntimeError("forward_sampled_loss draws its key on the host and would replay the same candidates "
+                                       "at every replay of a CUDA graph: call Code2Vec.use_device_rng() before capturing it")
+                key = self._next_seed()
+            candidates = sampler.sample(key, dev)
+        else:
+            if not isinstance(candidates, torch.Tensor) or candidates.dim() != 1 or \
+                    not 1 <= candidates.numel() <= _lib.SAMPLED_MAX:
+                raise ValueError(f"forward_sampled_loss: candidates must be a 1-D int64 tensor of 1 .. {_lib.SAMPLED_MAX} ids")
+            if candidates.device != dev:
+                raise ValueError(f"forward_sampled_loss: candidates are on {candidates.device}, the model on {dev}")
+            candidates = CF._idx(candidates, "candidates")
+        w_out, b_out = self._head()
+        loss = _SampledLossFn.apply(code_vector, w_out, b_out, label, candidates, sampler, self._label_algo)
+        return loss, code_vector, attention
 
     # -- additive convenience (the reference does torch.max(preds, dim=1) at main.py:285) ----
     @torch.no_grad()

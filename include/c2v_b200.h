@@ -583,6 +583,42 @@ int c2v_sparse_adam_step_merged(float *param, float *exp_avg, float *exp_avg_sq,
                                 float scale, double lr, double beta1, double beta2, double eps, int64_t step,
                                 void *stream);
 
+/* ---- sampled softmax over the plain label head (Jean et al. 2015; TF's sampled_softmax_loss, num_true = 1) ------------
+ * For B code vectors cv_i with labels y_i and S candidates s_j drawn i.i.d. from q:
+ *   z_i+ = cv_i . w_{y_i} + b_{y_i} - log(S q(y_i)),  z_ij = cv_i . w_{s_j} + b_{s_j} - log(S q(s_j))
+ *   loss = (1/B) sum_i [ log(exp z_i+ + sum_{j: s_j != y_i} exp z_ij) - z_i+ ]
+ * Every entry point returns C2V_EINVAL, naming the argument, before any CUDA call, and reads nothing on the host. */
+#define C2V_SAMPLED_MAX 65536
+/* S candidate ids int64 [S] (device) from the CDF cdf fp64 [C] (device; ascending, cdf[C - 1] == 1): draw j takes the
+ * Philox4x32-10 block with counter (j >> 1, 0, 0, 1) and key (key_lo, key_hi) -- the dropout mask's counters all have word
+ * 3 = 0 --, words (0, 1) for even j and (2, 3) for odd j as hi, lo, u = ((hi << 32 | lo) >> 11) 2^-53, and returns the
+ * first c with u < cdf[c].  key_device (8-byte aligned, device) when not NULL holds the key instead of `key`.
+ * 1 <= S <= C2V_SAMPLED_MAX, C >= 1. */
+int c2v_sampled_candidates(const double *cdf, int64_t C, int32_t S, uint64_t key, const uint64_t *key_device,
+                           int64_t *candidates, void *stream);
+/* The compact head: ids [S + B] = (candidates, label), w_hat [S + B, H] = output_weight[ids] and
+ * b_hat [S + B] = output_bias[ids] - (log S + log_q[ids]), the correction in fp64 (log_q fp64 [C]).  An id outside
+ * [0, C) gets a zero row and a NaN bias (its row's loss is then NaN). */
+int c2v_sampled_gather(const float *output_weight, const float *output_bias, const double *log_q, int64_t C, int32_t H,
+                       const int64_t *candidates, int32_t S, const int64_t *label, int32_t B, float *w_hat,
+                       float *b_hat, int64_t *ids, void *stream);
+/* From logits [B, S + B] = cv . w_hat^T + b_hat (c2v_label_logits on the compact head): lse [B] over row i's included
+ * columns -- candidate j unless ids[j] == ids[S + i], and column S + i -- and loss (device scalar) = the mean of
+ * lse_i - z_i,S+i, both in a fixed order. */
+int c2v_sampled_loss(const float *logits, const int64_t *ids, int32_t S, int32_t B, float *lse, float *loss,
+                     void *stream);
+/* Overwrites the logits with d loss / d logits: (softmax - onehot) scale (* *scale_device when not NULL) on the included
+ * columns, exactly 0 on the others; feed it to c2v_label_backward_ws on the compact head.  B <= 65535. */
+int c2v_sampled_dlogits(float *logits, const int64_t *ids, const float *lse, int32_t S, int32_t B, float scale,
+                        const float *scale_device, void *stream);
+/* dst[ids[e]] += rows[e] ([n, H] -> [C, H]) and dst_bias[ids[e]] += bias[e] ([n] -> [C]) for e < n; rows / dst and
+ * bias / dst_bias go in pairs, either pair may be NULL, not both.  Ids outside [0, C) are skipped.  The ids are sorted
+ * and each distinct id's entries are summed in entry order and written once: the result is the same bits on every run.
+ * n and C in [1, 2^31).  The workspace size is 0 for n outside that range. */
+size_t c2v_scatter_rows_add_workspace_bytes(int64_t n);
+int c2v_scatter_rows_add(const int64_t *ids, int64_t n, const float *rows, const float *bias, int32_t H, int64_t C,
+                         float *dst, float *dst_bias, void *workspace, size_t workspace_bytes, void *stream);
+
 /* ---- host-buffer call: what a reference-side caller with CPU tensors uses ----------
  * One whole Code2Vec.forward + torch.max for a batch held in HOST memory (pinned
  * for full speed): copies the int64 indices in, runs encode + label head +
